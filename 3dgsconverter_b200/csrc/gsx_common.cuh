@@ -1,4 +1,4 @@
-// gsx_common.cuh -- shared helpers for the gsx sm_100a kernels.
+// gsx_common.cuh -- shared helpers for the gsx sm_90a kernels.
 //
 // Arithmetic contract (SURVEY.md Appendix A): every float operation that feeds a
 // keep-mask is IEEE binary32 round-to-nearest with NO fma contraction.  The whole

@@ -4,10 +4,8 @@
 // 209,217-224 as driven by converter.py:194-236) for the columns the filters need: xyz (12 B/pt),
 // opacity (4 B/pt) and the original row index (4 B/pt).  The 248-byte records stay on the host and
 // are gathered ONCE, with the surviving indices, when the caller reads `DataProcessor.data`.
-// Stable (order-preserving), like NumPy boolean indexing.  Two forms, A/B in profiles/r02_stream_kernels_probe.json
-// (64 M rows, 50 % survivors): count -> multi-level scan -> scatter (0.72 ms) and the shipped single pass with
-// decoupled look-back over per-tile survivor counts (k_cmp_onepass, 0.66 ms).  A first single-pass version that staged
-// the survivors' DATA in 40 KiB of shared memory per block was slower than both (0.85 ms: occupancy).
+// Stable (order-preserving), like NumPy boolean indexing: one pass with decoupled look-back over per-tile survivor
+// counts (k_cmp_onepass) instead of count -> multi-level scan -> scatter, which reads the mask twice.
 #include "gsx_common.cuh"
 #include "gsx_compact.cuh"
 #include "gsx_radix.cuh"

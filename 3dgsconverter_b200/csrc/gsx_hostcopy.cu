@@ -2,9 +2,8 @@
 //
 // The reference's call sites hand libgsx ordinary NumPy arrays (np.column_stack at data_processor.py:139, the
 // shN block at sog.py:536-549).  cudaMemcpyAsync from pageable memory is staged by the driver through one
-// internal pinned buffer on ONE CPU thread: ~11 GB/s measured on the B200 box (profiles/r02_bench_n1.json:
-// 19.6 ms end to end from a pageable cloud against 11.1 ms from a pinned one), i.e. the PCIe Gen5 link
-// (~55 GB/s) idles 80 % of the time and the upload costs more than the whole filter.
+// internal pinned buffer on ONE CPU thread, so the PCIe link idles most of the time and the upload can
+// cost more than the whole filter.
 //
 // Here T host threads each own two pinned chunks and one copy stream: a thread memcpy()s its next chunk of
 // the user's buffer into a free pinned chunk and enqueues the DMA itself, so T memcpys and the DMAs of earlier
@@ -30,9 +29,8 @@ namespace {
 
 constexpr size_t kStagedMin = 8u << 20;      // below this the plain path is as fast
 constexpr int kMaxThreads = 16;
-size_t kChunk = 4u << 20;                    // pinned chunk (GSX_COPY_CHUNK_KB, default 4 MiB; A/B in
-                                             // profiles/r02c_copy_threads_probe.json: 1 MiB chunks lose 25 % on a 1.1 GB
-                                             // upload, 256 KiB chunks lose half)
+size_t kChunk = 4u << 20;                    // pinned chunk (GSX_COPY_CHUNK_KB, default 4 MiB; smaller chunks
+                                             // measured slower on large uploads)
 
 // The helper threads are created once and parked on a condition variable: creating 7 threads and giving each a CUDA
 // context binding cost more than the copy itself for a 120 MB cloud.  Leaked on purpose (no static destruction order
@@ -218,8 +216,8 @@ int copy_h2d(void* dst_dev, const void* src_host, size_t bytes, cudaStream_t st)
 }
 
 // Make the pages of a (typically fresh, never touched) host destination resident BEFORE the download needs them: a
-// first touch costs ~0.5-1.5 us per 4 KiB page (measured: 7.5 GB/s staged D2H into np.empty against 40+ GB/s into
-// touched memory), and the caller has nothing else to do while the GPU computes.  Content is preserved.
+// first touch of a 4 KiB page costs a page fault, which slows a staged D2H into np.empty far below a copy into
+// touched memory, and the caller has nothing else to do while the GPU computes.  Content is preserved.
 int prefault_host(void* dst_host, size_t bytes) {
     if (bytes < (1u << 20) || !staged_enabled()) return GSX_OK;
     int dev = 0;

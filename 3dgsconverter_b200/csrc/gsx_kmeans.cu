@@ -1,4 +1,4 @@
-// gsx_kmeans.cu -- batched Lloyd K-Means (SOG codebooks) for sm_100a.
+// gsx_kmeans.cu -- batched Lloyd K-Means (SOG codebooks) for sm_90a (H100).
 //
 // Replaces gpu_ops.py:57-73 (k_means_assign), :75-96 (k_means_update) and the loop at :186-188.
 // Arithmetic contract: SURVEY A.5 -- strict float32, no fma: dist = (((0 + d0^2) + d1^2) + ...),
@@ -666,7 +666,7 @@ int kmeans_lloyd(const float* X, const int64_t* row_off, int nprob, int K, int D
                     "kmeans: tensor-core assign needs D in {9,24,45} and K <= 256 (got K=%d D=%d)", K, D);
     const bool use_tc = assign_mode == GSX_KM_ASSIGN_TENSOR || assign_mode == GSX_KM_ASSIGN_TENSOR_BF16 ||
                         (assign_mode == GSX_KM_ASSIGN_AUTO && kmeans_tc_supported(K, D));
-    const int tc_variant = assign_mode == GSX_KM_ASSIGN_TENSOR_BF16 ? 2 : 0;   // TF32 is the measured-faster default
+    const int tc_variant = assign_mode == GSX_KM_ASSIGN_TENSOR_BF16 ? 2 : 0;   // 0: TF32, the only variant built
     const bool prefilter = assign_mode == GSX_KM_ASSIGN_FMA_PREFILTER;
     GSX_REQUIRE(nprob >= 1 && K >= 1 && D >= 1 && max_iter >= 0, GSX_ERR_ARG, "kmeans: bad shape");
     const int64_t n_total = row_off[nprob] - row_off[0];

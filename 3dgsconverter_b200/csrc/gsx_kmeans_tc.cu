@@ -1,4 +1,4 @@
-// gsx_kmeans_tc.cu -- K-Means assign step on the 5th-gen tensor cores (tcgen05 + TMEM), sm_100a.
+// gsx_kmeans_tc.cu -- K-Means assign step on the Hopper tensor cores (wgmma, TF32), sm_90a.
 //
 // Replaces gpu_ops.py:57-73 (k_means_assign) with bit-identical labels.  The contract (SURVEY A.5) is a strict
 // float32 (sub, mul, add -- no fma, dims ascending) distance per (point, centroid), lowest index winning ties;
@@ -6,13 +6,15 @@
 //        s_c = x . c - 0.5 ||c||^2            (E_c = ||x||^2 - 2 s_c is the squared distance),
 // so the kernel
 //   1. computes S = [X | 1 1 1] . [C | b_hi b_mid b_lo]^T  for a tile of 128 points x (up to) 256 centroids with
-//      tcgen05.mma.kind::tf32 (A = the points, B = the centroids, both K-major in shared memory, the accumulator
-//      128 lanes x 256 columns of TMEM); the bias -0.5||c||^2 is split into three TF32-exact pieces and rides in
-//      three padding columns of the K dimension, so the bias costs nothing and adds no rounding;
-//   2. reads the scores back with tcgen05.ld (thread r <-> TMEM lane r <-> point r), takes the row maximum and
+//      wgmma.mma_async ... .tf32 (A = the points, B = the centroids, both K-major in shared memory; each of the two
+//      warpgroups owns 64 point rows and holds their float32 scores in registers); the bias -0.5||c||^2 is split
+//      into three TF32-exact pieces and rides in three padding columns of the K dimension, so the bias costs
+//      nothing and adds no rounding;
+//   2. takes the row maximum (a row is spread over the four threads of a quad in the wgmma accumulator layout) and
 //      builds the set of centroids whose score is within a rounding-error margin M of it;
 //   3. evaluates the strict contract distance only for those candidates (one candidate: it IS the answer, no
-//      evaluation at all), ascending index, strict '<'.
+//      evaluation at all), ascending index, strict '<' -- the quad then keeps the lexicographic minimum of
+//      (distance, index), which is exactly what the serial ascending scan returns.
 // Margin (DESIGN.md 4.6): with |s~_c - t_c| <= eta for every centroid (t_c the real-arithmetic score, s~_c what
 // the tensor core returns) and |a_c - E_c| <= g E_c for the strict float32 distance a_c, the contract's answer
 // c* satisfies  s~_{c*} >= s~_max - (2 eta + g/(1-g) E_{c'}),  E_{c'} <= ||x||^2 - 2 s~_max + 2 eta.
@@ -23,23 +25,17 @@
 //
 // Data movement: a tile is 128 consecutive rows of X = 128*D*4 contiguous bytes; one elected thread moves it
 // global -> shared with a 1-D TMA bulk copy (cp.async.bulk, completion on an mbarrier) one tile ahead of the
-// MMA, then every thread re-lays its own row into the UMMA canonical layout (conflict-free for odd D).
+// MMA, then every thread re-lays its half row into the GMMA canonical K-major layout (no swizzle).
 #include "gsx_common.cuh"
 #include "gsx_kmeans.cuh"
-
-#include <cuda_bf16.h>
 
 namespace gsx {
 
 #define GSX_FULL 0xffffffffu
 
-constexpr int kTcThreads = 256;   // two threads per point row (TMEM lane): they split the centroid columns
-constexpr int kTcRows = 128;      // UMMA M
-constexpr int kTcMaxN = 256;      // UMMA N limit == max centroids of the tensor-core path
-#ifndef GSX_KM_TC16
-#define GSX_KM_TC16 0   // variant B (split bf16): measured slower than TF32 and it stalls on tests/test_kmeans_prefilter_gpu.py::
-                        // test_prefilter_adversarial -- kept as a build-time experiment, not part of the shipped library
-#endif
+constexpr int kTcThreads = 256;   // two warpgroups; for the operand re-layout: two threads per point row
+constexpr int kTcRows = 128;      // points per tile: 2 x wgmma M=64
+constexpr int kTcMaxN = 256;      // max centroids of the tensor-core path (4 x wgmma N=64)
 constexpr long long kWaitCycles = 1ll << 31;   // ~1 s: a protocol bug reports an error instead of hanging the GPU
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -75,55 +71,35 @@ __device__ __forceinline__ void bulk_g2s(void* dst_smem, const void* src_gmem, u
                  : "memory");
 }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-__device__ __forceinline__ void tmem_alloc(uint32_t* slot_smem, uint32_t ncols) {  // one full warp
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(slot_smem)),
-                 "r"(ncols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// GMMA shared-memory descriptor, K-major, no swizzle (layout type 0, cute::GMMA::GmmaDescriptor): core matrix =
+// 8 rows x 16 B stored as 128 contiguous bytes, lbo = byte distance of the two core matrices adjacent in K,
+// sbo = byte distance of adjacent 8-row groups.
+__device__ __forceinline__ uint64_t gmma_desc(uint32_t saddr, uint32_t lbo, uint32_t sbo) {
+    return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)(lbo >> 4) << 16) | ((uint64_t)(sbo >> 4) << 32);
 }
-__device__ __forceinline__ void tmem_free(uint32_t taddr, uint32_t ncols) {  // the same warp
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-
-// UMMA shared-memory descriptor, K-major, no swizzle (cute::UMMA::SmemDescriptor): core matrix = 8 rows x 16 B,
-// lbo = byte distance of the two core matrices that are adjacent in K, sbo = byte distance of 8-row groups.
-__device__ __forceinline__ uint64_t umma_desc(uint32_t saddr, uint32_t lbo, uint32_t sbo) {
-    return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)(lbo >> 4) << 16) | ((uint64_t)(sbo >> 4) << 32) |
-           (1ull << 46);
-}
-// D[tmem] (+)= A[smem] . B[smem]^T, TF32 inputs, float32 accumulate; issued by ONE thread
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate) {
+// d[64 x 64] (+)= A[64 x 8] . B[64 x 8]^T, TF32 inputs, float32 accumulate; issued by the whole warpgroup
+__device__ __forceinline__ void wgmma_tf32_n64(float (&d)[32], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
     asm volatile(
         "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
-}
-// 32 consecutive float32 columns of this thread's TMEM lane
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float (&v)[32]) {
-    uint32_t r[32];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
+        "setp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
         "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,"
-        "%29,%30,%31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
+        "%29,%30,%31}, %32, %33, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+          "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+          "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(adesc), "l"(bdesc), "r"(accumulate)
         : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+}
+// keeps the compiler from moving accumulator reads / writes across the asynchronous MMA
+template <int NB>
+__device__ __forceinline__ void acc_fence(float (&acc)[NB][32]) {
 #pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
+    for (int b = 0; b < NB; ++b)
+#pragma unroll
+        for (int i = 0; i < 32; ++i) asm volatile("" : "+f"(acc[b][i])::"memory");
 }
 
 __device__ __forceinline__ float tf32_trunc(float v) { return __uint_as_float(__float_as_uint(v) & 0xFFFFE000u); }
@@ -136,68 +112,51 @@ __device__ __forceinline__ uint32_t op_off(int row, int k) {
 
 struct TcShared {  // tail of the dynamic shared memory (after the operand tiles and the staging buffer)
     uint64_t bar_copy;
-    uint64_t bar_mma;
-    uint32_t tmem_base;
     float red[8];
     float xn[2][kTcRows];    // partial ||x||^2 of the two half rows
-    float pmax[2][kTcRows];  // partial row maxima of the two column halves
-    int pcnt[2][kTcRows];    // candidates in each column half
-    float pbest[kTcRows];    // strict result of the upper column half
-    int pbk[kTcRows];
 };
 
-// barrier of the two warps that share a TMEM lane quarter (warp q and warp q+4): ids 1..4, 64 threads
-__device__ __forceinline__ void pair_sync(int q) { asm volatile("bar.sync %0, 64;" ::"r"(q + 1) : "memory"); }
-
-// Work split: 256 threads = 8 warps.  Warp w may only read the TMEM lanes 32*(w%4) .. +31, so warps q and q+4 share
-// the 32 point rows of lane quarter q and split the centroid COLUMNS between them (lower / upper half of the 32-wide
-// column chunks); the pair exchanges its partial row maximum, candidate count and strict result through shared
-// memory behind a 64-thread named barrier.  Two CTAs per SM (2 x 256 TMEM columns) = 16 resident warps.
+// Work split: 256 threads = 2 warpgroups.  Warpgroup g computes the scores of the tile rows 64g .. 64g+63 against
+// NB*64 centroid columns.  In the accumulator layout, thread (warp w, lane l) of the warpgroup holds the rows
+// 16(w%4) + l/4 and +8 and, in every 64-column block, the columns 8j + 2(l%4) + {0,1}, j = 0..7: register
+// acc[b][4j + 2i + e] is (row + 8i, column 64b + 8j + 2(l%4) + e).  The four threads of a quad share their rows.
 // mode 0: labels; mode 1 (debug): dump the raw scores of the first tile to dump[128*npad] and return
-template <int D, int KP>
-__global__ void __launch_bounds__(kTcThreads, 2)
+template <int D, int KP, int NB>
+__global__ void __launch_bounds__(kTcThreads, 1)
     k_km_assign_tc(const float* __restrict__ X, long long x_floats, const float* __restrict__ C,
                    int* __restrict__ labels, const KmProb* __restrict__ probs, int nprob, int K, int npad,
-                   int tmem_cols, long long tiles_total, int desc_variant, int mode, float* __restrict__ dump,
-                   unsigned long long* __restrict__ tc_stats, int* __restrict__ err_flag) {
+                   long long tiles_total, int mode, float* __restrict__ dump, unsigned long long* __restrict__ tc_stats,
+                   int* __restrict__ err_flag) {
     static_assert(KP % 8 == 0 && KP >= D + 3, "K padding");
+    constexpr int NT = NB * 64;             // centroid columns computed (padding columns score -3e38)
     constexpr int G4 = KP / 4;              // float4 groups per operand row
     constexpr int GH = (G4 + 1) / 2;        // groups re-laid by the lower-half thread of a row
-    constexpr int NCH = kTcMaxN / 32;       // 32-column chunks of the accumulator (8)
     extern __shared__ __align__(1024) unsigned char smem[];
-    unsigned char* sB = smem;                                   // [kTcMaxN x KP] float32, UMMA K-major layout
+    unsigned char* sB = smem;                                   // [kTcMaxN x KP] float32, GMMA K-major layout
     unsigned char* sA = sB + kTcMaxN * KP * 4;                  // [128 x KP]
     float* sStage = reinterpret_cast<float*>(sA + kTcRows * KP * 4);  // 128*D floats + 8 (alignment slack)
     TcShared* sh = reinterpret_cast<TcShared*>(reinterpret_cast<unsigned char*>(sStage) + (kTcRows * D + 8) * 4);
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int q = warp & 3, half = warp >> 2;
-    const int row = q * 32 + lane;  // point row of the tile == TMEM lane
+    // operand re-layout: thread -> (row, half of the K groups)
+    const int lrow = (warp & 3) * 32 + lane, half = warp >> 2;
+    // epilogue: thread -> two rows and the quad's column pattern
+    const int wg = warp >> 2, quad = lane & 3;
+    const int erow0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
     if (tid == 0) {
         mbar_init(&sh->bar_copy, 1);
-        mbar_init(&sh->bar_mma, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 0) tmem_alloc(&sh->tmem_base, (uint32_t)tmem_cols);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = sh->tmem_base;
 
     const long long t0 = tiles_total * (long long)blockIdx.x / gridDim.x;
     const long long t1 = tiles_total * (long long)(blockIdx.x + 1) / gridDim.x;
     const bool x_aligned = (reinterpret_cast<uintptr_t>(X) & 15) == 0;
-    const uint32_t lbo = desc_variant == 1 ? (uint32_t)G4 * 128u : 128u;
-    const uint32_t sbo = desc_variant == 1 ? 128u : (uint32_t)G4 * 128u;
-    const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(npad >> 3) << 17) | ((kTcRows >> 4) << 24);
+    constexpr uint32_t kLbo = 128u, kSbo = (uint32_t)G4 * 128u;
     constexpr float kU = 5.9604645e-8f;                        // 2^-24
     constexpr float kGs = 2.f * (D + 3) * kU * 1.02f;          // >= 2 gamma_{D+2} / (1 - gamma_{D+2})
     constexpr float kEpsIn = 1.953125e-3f * 1.01f;             // 2^-9 (+): two TF32 conversions, 2^-10 each
     constexpr float kEpsAcc = 3.0517578e-5f;                   // 2^-15: accumulation + bias evaluation slack
-    // this thread's column chunks: the lower half of the chunks for warps 0-3, the upper half for warps 4-7
-    const int nch = npad >> 5;
-    const int ch_lo = half == 0 ? 0 : (nch + 1) / 2;
-    const int ch_hi = half == 0 ? (nch + 1) / 2 : nch;
 
     struct TileGeo { int p; long long row0; int rows; long long off_floats; bool bulk; uint32_t pre, bytes; };
     auto geo = [&](long long t) {
@@ -220,7 +179,7 @@ __global__ void __launch_bounds__(kTcThreads, 2)
         return g;
     };
 
-    uint32_t copy_phase = 0, mma_phase = 0;
+    uint32_t copy_phase = 0;
     bool failed = false;
     TileGeo cur{};
     if (t0 < t1) {
@@ -233,13 +192,13 @@ __global__ void __launch_bounds__(kTcThreads, 2)
     int cur_prob = -1;
     float Cm = 0.f;
     unsigned long long st_strict = 0, st_multi = 0, st_full = 0;
+    float acc[NB][32];
 
-    for (long long t = t0; t < t1 && !failed; ++t) {
+    for (long long t = t0; t < t1; ++t) {
         const TileGeo g = cur;
         const float* Cp = C + (size_t)g.p * K * D;
         if (g.p != cur_prob) {  // (re)load the centroids of this problem as the B operand
-            __syncthreads();    // nobody is still reading sB in a strict evaluation of the previous tile
-            for (int idx = tid; idx < npad * G4; idx += kTcThreads) {
+            for (int idx = tid; idx < NT * G4; idx += kTcThreads) {
                 const int c = idx / G4, j = idx - c * G4;
                 float v[4];
 #pragma unroll
@@ -251,7 +210,7 @@ __global__ void __launch_bounds__(kTcThreads, 2)
             }
             __syncthreads();
             float mx = 0.f;
-            for (int c = tid; c < npad; c += kTcThreads) {
+            for (int c = tid; c < NT; c += kTcThreads) {
                 float cn = 0.f;
                 if (c < K) {
                     for (int k = 0; k < D; ++k) {
@@ -281,14 +240,14 @@ __global__ void __launch_bounds__(kTcThreads, 2)
             cur_prob = g.p;
         }
 
-        // ---- this thread's half row: staging (bulk copy) or global -> UMMA layout, partial ||x||^2 on the way
+        // ---- this thread's half row: staging (bulk copy) or global -> GMMA layout, partial ||x||^2 on the way
         if (g.bulk) {
             if (!mbar_wait(&sh->bar_copy, copy_phase)) failed = true;
             copy_phase ^= 1;
         }
-        const bool live = row < g.rows;
         {
-            const float* src = g.bulk ? sStage + (g.pre >> 2) + row * D : X + g.off_floats + (long long)row * D;
+            const bool live = lrow < g.rows;
+            const float* src = g.bulk ? sStage + (g.pre >> 2) + lrow * D : X + g.off_floats + (long long)lrow * D;
             float xa = 0.f, xb = 0.f;  // two chains
             const int j0 = half == 0 ? 0 : GH, j1 = half == 0 ? GH : G4;
 #pragma unroll
@@ -306,551 +265,135 @@ __global__ void __launch_bounds__(kTcThreads, 2)
                             v[e] = k < D + 3 ? 1.0f : 0.f;
                         }
                     }
-                    *reinterpret_cast<float4*>(sA + op_off<KP>(row, 4 * j)) = make_float4(v[0], v[1], v[2], v[3]);
+                    *reinterpret_cast<float4*>(sA + op_off<KP>(lrow, 4 * j)) = make_float4(v[0], v[1], v[2], v[3]);
                 }
             }
-            sh->xn[half][row] = xa + xb;
+            sh->xn[half][lrow] = xa + xb;
         }
         fence_proxy_async();   // generic-proxy writes of sA / sB -> visible to the tensor core (async proxy)
-        tc_fence_before();     // this thread's tcgen05.ld of the previous tile are done before the next MMA
-        __syncthreads();
-        if (t + 1 < t1) cur = geo(t + 1);
-        if (tid == 0) {
-            tc_fence_after();
-            if (t + 1 < t1 && cur.bulk) {  // staging is free: every thread has copied its half row out
-                mbar_expect_tx(&sh->bar_copy, cur.bytes);
-                bulk_g2s(sStage, reinterpret_cast<const char*>(X) + (cur.off_floats * 4 - cur.pre), cur.bytes,
-                         &sh->bar_copy);
-            }
-            const uint32_t a0 = smem_u32(sA), b0 = smem_u32(sB);
-#pragma unroll
-            for (int j = 0; j < KP / 8; ++j) {  // one instruction = 8 TF32 along K = two core matrices
-                const uint32_t koff = (uint32_t)j * 256u;  // two 128-byte core matrices further along K
-                umma_tf32(tmem_base, umma_desc(a0 + koff, lbo, sbo), umma_desc(b0 + koff, lbo, sbo), idesc, j > 0);
-            }
-            umma_commit(&sh->bar_mma);
-        }
-        if (!mbar_wait(&sh->bar_mma, mma_phase)) failed = true;
-        mma_phase ^= 1;
-        tc_fence_after();
-        if (failed) break;
-
-        const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16);
-        if (mode == 1) {  // debug: raw scores of the tile
-            for (int w = ch_lo; w < ch_hi; ++w) {
-                float v[32];
-                tmem_ld32(taddr + w * 32, v);
-#pragma unroll
-                for (int i = 0; i < 32; ++i) dump[(size_t)row * npad + w * 32 + i] = v[i];
-            }
+        if (__syncthreads_or(failed)) {
+            failed = true;
             break;
         }
-
-        // ---- epilogue pass 1: row maximum over this thread's column chunks (four independent chains)
-        float m0 = -INFINITY, m1 = -INFINITY, m2 = -INFINITY, m3 = -INFINITY;
-#pragma unroll
-        for (int ww = 0; ww < NCH / 2; ++ww) {
-            const int w = ch_lo + ww;
-            if (w < ch_hi) {
-                float v[32];
-                tmem_ld32(taddr + w * 32, v);
-#pragma unroll
-                for (int i = 0; i < 32; i += 4) {
-                    m0 = fmaxf(m0, v[i]);
-                    m1 = fmaxf(m1, v[i + 1]);
-                    m2 = fmaxf(m2, v[i + 2]);
-                    m3 = fmaxf(m3, v[i + 3]);
-                }
-            }
-        }
-        sh->pmax[half][row] = fmaxf(fmaxf(m0, m1), fmaxf(m2, m3));
-        pair_sync(q);
-        const float smax = fmaxf(sh->pmax[0][row], sh->pmax[1][row]);
-        const float xn = sh->xn[0][row] + sh->xn[1][row];
-        const float xnu = xn * 1.0001f;
-        const float xnorm = sqrtf(xnu) * 1.0001f;
-        const float eta = (kEpsIn * xnorm * Cm + kEpsAcc * (xnorm * Cm + Cm * Cm)) * 1.5f + 1e-37f;
-        const float e_ub = fmaxf(xnu - 2.f * smax + 2.f * eta, 0.f);
-        const float marg = 2.f * eta + kGs * e_ub;
-        const float thr = smax - marg;
-        // ---- pass 2: candidate mask of this thread's chunks (two independent mask chains per chunk)
-        uint32_t mask[NCH / 2];
-        int cnt = 0;
-#pragma unroll
-        for (int ww = 0; ww < NCH / 2; ++ww) {
-            mask[ww] = 0;
-            const int w = ch_lo + ww;
-            if (w < ch_hi) {
-                float v[32];
-                tmem_ld32(taddr + w * 32, v);
-                uint32_t ma = 0, mb = 0;
-#pragma unroll
-                for (int i = 0; i < 32; i += 2) {
-                    if (v[i] >= thr) ma |= 1u << i;
-                    if (v[i + 1] >= thr) mb |= 1u << (i + 1);
-                }
-                mask[ww] = ma | mb;
-                cnt += __popc(ma | mb);
-            }
-        }
-        sh->pcnt[half][row] = cnt;
-        pair_sync(q);
-        const int total = sh->pcnt[0][row] + sh->pcnt[1][row];
-        // the shortcut is only legal when the margin is finite, a real centroid scored, and the strict distance
-        // of the winner cannot reach the contract's 1e20 "no label" sentinel.  Both threads of a row agree on it.
-        const bool bad = !(marg < 3.0e38f) || !(smax > -1.0e30f) || !(e_ub < 1.0e19f) || total == 0;
-        if (!bad && total == 1 && cnt == 1 && live) {  // the single candidate lies in this thread's half
-            int label = -1;
-#pragma unroll
-            for (int ww = 0; ww < NCH / 2; ++ww)
-                if (mask[ww]) label = (ch_lo + ww) * 32 + __ffs(mask[ww]) - 1;
-            labels[g.row0 + row] = label;
-        }
-        const bool need = live && (bad || total > 1);
-        if (__any_sync(GSX_FULL, need)) {  // same rows in both warps of the pair: both take this branch together
-            if (bad) {  // full strict scan over the real centroids of this half
-#pragma unroll
-                for (int ww = 0; ww < NCH / 2; ++ww) {
-                    const int left = K - (ch_lo + ww) * 32;
-                    mask[ww] = (ch_lo + ww < ch_hi) ? (left >= 32 ? 0xffffffffu : (left > 0 ? (1u << left) - 1u : 0u)) : 0u;
-                }
-            }
-            float best = 1e20f;
-            int bk = -1;
-            if (need && half == 0) {
-                ++st_multi;
-                if (bad) ++st_full;
-            }
-            for (;;) {
-                int c = -1;
-                if (need) {
-#pragma unroll
-                    for (int ww = NCH / 2 - 1; ww >= 0; --ww)
-                        if (mask[ww]) c = (ch_lo + ww) * 32 + __ffs(mask[ww]) - 1;
-                }
-                if (!__any_sync(GSX_FULL, c >= 0)) break;
-                if (c >= 0) {
-#pragma unroll
-                    for (int ww = 0; ww < NCH / 2; ++ww)
-                        if ((c >> 5) - ch_lo == ww) mask[ww] &= mask[ww] - 1;
-                    float acc = 0.f;
-#pragma unroll
-                    for (int j = 0; j < (D + 3) / 4; ++j) {
-                        const float4 xv = *reinterpret_cast<const float4*>(sA + op_off<KP>(row, 4 * j));
-                        const float4 cv = *reinterpret_cast<const float4*>(sB + op_off<KP>(c, 4 * j));
-                        const float xa[4] = {xv.x, xv.y, xv.z, xv.w}, ca[4] = {cv.x, cv.y, cv.z, cv.w};
-#pragma unroll
-                        for (int e = 0; e < 4; ++e)
-                            if (4 * j + e < D) {
-                                const float df = __fsub_rn(xa[e], ca[e]);
-                                acc = __fadd_rn(acc, __fmul_rn(df, df));
-                            }
-                    }
-                    ++st_strict;
-                    if (acc < best) best = acc, bk = c;
-                }
-            }
-            if (half == 1) {
-                sh->pbest[row] = best;
-                sh->pbk[row] = bk;
-            }
-            pair_sync(q);
-            if (half == 0 && need) {  // ascending index + strict '<': the lower half wins ties
-                const float hb = sh->pbest[row];
-                if (hb < best) bk = sh->pbk[row];
-                labels[g.row0 + row] = bk;
-            }
-            pair_sync(q);  // pbest / pbk are free again
-        }
-    }
-
-    if (failed && err_flag) atomicExch(err_flag, 1);
-    if (tc_stats) {
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            st_strict += __shfl_xor_sync(GSX_FULL, st_strict, o);
-            st_multi += __shfl_xor_sync(GSX_FULL, st_multi, o);
-            st_full += __shfl_xor_sync(GSX_FULL, st_full, o);
-        }
-        if (lane == 0) {
-            atomicAdd(tc_stats + 0, st_strict);
-            atomicAdd(tc_stats + 1, st_multi);
-            atomicAdd(tc_stats + 2, st_full);
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) tmem_free(tmem_base, (uint32_t)tmem_cols);
-}
-
-// =================================================================================================================
-// Second generation: split-bf16 scores + single-pass top-2 epilogue.
-//
-// ncu of the TF32 kernel above (profiles/r02_km_tc_ncu.json) shows it bound by the TMEM read path: tcgen05.ld moves
-// 64 B/clk/SM, the 128 x 256 float32 accumulator is 128 KiB = 2048 clk per pass, and the TF32 margin (2^-9 relative)
-// forces TWO passes (row maximum, then candidate mask) plus a strict evaluation for ~9 % of the points.  Here
-//   * x = x1 + x2 (+ 2^-18), c = c1 + c2 (+ 2^-18) with x1, x2, c1, c2 in bfloat16 (round-to-nearest splits);
-//     S = A1.B1^T + A1.B2^T + A2.B1^T (three kind::f16 MMAs per 16-wide K step, float32 accumulation in TMEM):
-//     |S - x.c| <= 3.1 * 2^-18 ||x|| ||c||, 100x tighter than TF32 -- the same shared-memory footprint (2 bytes x 2);
-//   * the accumulator is read ONCE: every score is turned into a key (low 8 mantissa bits replaced by the centroid
-//     column) and the thread keeps the two largest keys -- best score, its column, and the runner-up in 4
-//     instructions per element.  If the runner-up is below best - margin the best column IS the label (99.8 % of the
-//     points); only warps that contain an ambiguous point re-read their TMEM columns and evaluate the strict
-//     distance of the candidates (x and c re-read from global memory / L2: the operands in shared memory are bf16).
-// The bias -0.5||c||^2 rides in three bf16-exact pieces in padding columns of A1/B1 as before.
-// Margin: eta = 2^-16 (input split) + 2^-14 (key truncation, both ends) + 2^-19 (accumulation) relative to
-// ||x|| Cmax + Cmax^2/2, doubled; everything non-finite falls back to the full strict scan.
-template <int KP16>
-__device__ __forceinline__ uint32_t op16_off(int row, int k) {   // K-major bf16 operand, KP16 (multiple of 16) columns
-    return (uint32_t)((row >> 3) * (KP16 / 8) * 128 + (k >> 3) * 128 + (row & 7) * 16 + (k & 7) * 2);
-}
-
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-
-// 8 consecutive floats -> two 16-byte chunks of bf16: the round-to-nearest head and the head of the remainder
-__device__ __forceinline__ void split8(const float (&v)[8], uint4& hi, uint4& lo) {
-    uint32_t h[4], l[4];
-#pragma unroll
-    for (int e = 0; e < 4; ++e) {
-        const __nv_bfloat16 a1 = __float2bfloat16_rn(v[2 * e]), b1 = __float2bfloat16_rn(v[2 * e + 1]);
-        const float ra = __fsub_rn(v[2 * e], __bfloat162float(a1)), rb = __fsub_rn(v[2 * e + 1], __bfloat162float(b1));
-        const __nv_bfloat16 a2 = __float2bfloat16_rn(ra), b2 = __float2bfloat16_rn(rb);
-        h[e] = (uint32_t)__bfloat16_as_ushort(a1) | ((uint32_t)__bfloat16_as_ushort(b1) << 16);
-        l[e] = (uint32_t)__bfloat16_as_ushort(a2) | ((uint32_t)__bfloat16_as_ushort(b2) << 16);
-    }
-    hi = make_uint4(h[0], h[1], h[2], h[3]);
-    lo = make_uint4(l[0], l[1], l[2], l[3]);
-}
-
-struct Tc16Shared {
-    uint64_t bar_copy;
-    uint64_t bar_mma;
-    uint32_t tmem_base;
-    float red[8];
-    float xn[2][kTcRows];
-    float pb1[2][kTcRows];   // best key of each column half
-    float pb2[2][kTcRows];   // runner-up key of each column half
-    int pcnt[2][kTcRows];
-    float pbest[kTcRows];
-    int pbk[kTcRows];
-};
-
-#if GSX_KM_TC16
-
-template <int D, int KP>   // KP: padded K in bf16 elements, multiple of 16, >= D + 3
-__global__ void __launch_bounds__(kTcThreads, 2)
-    k_km_assign_tc16(const float* __restrict__ X, long long x_floats, const float* __restrict__ C,
-                     int* __restrict__ labels, const KmProb* __restrict__ probs, int nprob, int K, int npad,
-                     int tmem_cols, long long tiles_total, int mode, float* __restrict__ dump,
-                     unsigned long long* __restrict__ tc_stats, int* __restrict__ err_flag) {
-    static_assert(KP % 16 == 0 && KP >= D + 3, "K padding");
-    constexpr int G8 = KP / 8;              // 16-byte chunks (8 bf16) per operand row
-    constexpr int GH = (G8 + 1) / 2;        // chunks re-laid by the lower-half thread of a row
-    constexpr int NCH = kTcMaxN / 32;
-    constexpr uint32_t kOpA = kTcRows * KP * 2, kOpB = kTcMaxN * KP * 2;
-    extern __shared__ __align__(1024) unsigned char smem[];
-    unsigned char* sB1 = smem;
-    unsigned char* sB2 = sB1 + kOpB;
-    unsigned char* sA1 = sB2 + kOpB;
-    unsigned char* sA2 = sA1 + kOpA;
-    float* sStage = reinterpret_cast<float*>(sA2 + kOpA);
-    Tc16Shared* sh = reinterpret_cast<Tc16Shared*>(reinterpret_cast<unsigned char*>(sStage) + (kTcRows * D + 8) * 4);
-
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int q = warp & 3, half = warp >> 2;
-    const int row = q * 32 + lane;
-    if (tid == 0) {
-        mbar_init(&sh->bar_copy, 1);
-        mbar_init(&sh->bar_mma, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 0) tmem_alloc(&sh->tmem_base, (uint32_t)tmem_cols);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = sh->tmem_base;
-
-    const long long t0 = tiles_total * (long long)blockIdx.x / gridDim.x;
-    const long long t1 = tiles_total * (long long)(blockIdx.x + 1) / gridDim.x;
-    const bool x_aligned = (reinterpret_cast<uintptr_t>(X) & 15) == 0;
-    const uint32_t lbo = 128u, sbo = (uint32_t)G8 * 128u;
-    // kind::f16, A = B = bf16 (format 1), D = f32 (1): cute::UMMA::InstrDescriptor
-    const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(npad >> 3) << 17) | ((kTcRows >> 4) << 24);
-    constexpr float kU = 5.9604645e-8f;
-    constexpr float kGs = 2.f * (D + 3) * kU * 1.02f;
-    constexpr float kEps = 1.5258789e-5f /*2^-16*/ + 6.1035156e-5f /*2^-14*/ + 1.9073486e-6f /*2^-19*/;
-    const int nch = npad >> 5;
-    const int ch_lo = half == 0 ? 0 : (nch + 1) / 2;
-    const int ch_hi = half == 0 ? (nch + 1) / 2 : nch;
-
-    struct TileGeo { int p; long long row0; int rows; long long off_floats; bool bulk; uint32_t pre, bytes; };
-    auto geo = [&](long long t) {
-        TileGeo g;
-        int lo = 0, hi = nprob - 1;
-        while (lo < hi) {
-            int mid = (lo + hi + 1) >> 1;
-            if (probs[mid].tc_tile0 <= t) lo = mid; else hi = mid - 1;
-        }
-        g.p = lo;
-        const long long lt = t - probs[lo].tc_tile0;
-        const long long left = probs[lo].rows - lt * kTcRows;
-        g.rows = left < kTcRows ? (int)left : kTcRows;
-        g.row0 = probs[lo].row0 + lt * kTcRows;
-        g.off_floats = g.row0 * D;
-        const long long ob = g.off_floats * 4;
-        g.pre = (uint32_t)(ob & 15);
-        g.bytes = (g.pre + (uint32_t)g.rows * D * 4 + 15u) & ~15u;
-        g.bulk = x_aligned && ((ob - g.pre) + g.bytes <= x_floats * 4);
-        return g;
-    };
-
-    uint32_t copy_phase = 0, mma_phase = 0;
-    bool failed = false;
-    TileGeo cur{};
-    if (t0 < t1) {
-        cur = geo(t0);
-        if (tid == 0 && cur.bulk) {
+        if (t + 1 < t1) cur = geo(t + 1);
+        if (tid == 0 && t + 1 < t1 && cur.bulk) {  // staging is free: every thread has copied its half row out
             mbar_expect_tx(&sh->bar_copy, cur.bytes);
             bulk_g2s(sStage, reinterpret_cast<const char*>(X) + (cur.off_floats * 4 - cur.pre), cur.bytes, &sh->bar_copy);
         }
-    }
-    int cur_prob = -1;
-    float Cm = 0.f;
-    unsigned long long st_strict = 0, st_multi = 0, st_full = 0;
 
-    for (long long t = t0; t < t1 && !failed; ++t) {
-        const TileGeo g = cur;
-        const float* Cp = C + (size_t)g.p * K * D;
-        if (g.p != cur_prob) {  // (re)load the centroids of this problem: c = c1 + c2 in bf16, bias pieces in B1
-            __syncthreads();
-            float mx = 0.f;
-            for (int c = tid; c < npad; c += kTcThreads) {
-                float cn = 0.f;
-#pragma unroll
-                for (int j = 0; j < G8; ++j) {
-                    float v[8];
-#pragma unroll
-                    for (int e = 0; e < 8; ++e) {
-                        const int k = 8 * j + e;
-                        v[e] = (c < K && k < D) ? __ldg(Cp + (size_t)c * D + k) : 0.f;
-                        cn = __fmaf_rn(v[e], v[e], cn);
-                    }
-                    uint4 hi, lo;
-                    split8(v, hi, lo);
-                    *reinterpret_cast<uint4*>(sB1 + op16_off<KP>(c, 8 * j)) = hi;
-                    *reinterpret_cast<uint4*>(sB2 + op16_off<KP>(c, 8 * j)) = lo;
-                }
-                mx = fmaxf(mx, cn);
-                const float b = c < K ? -0.5f * cn : -3.0e38f;
-                const __nv_bfloat16 b1 = __float2bfloat16_rn(b);
-                const float r1 = c < K ? __fsub_rn(b, __bfloat162float(b1)) : 0.f;
-                const __nv_bfloat16 b2 = __float2bfloat16_rn(r1);
-                const float r2 = c < K ? __fsub_rn(r1, __bfloat162float(b2)) : 0.f;
-                const __nv_bfloat16 b3 = __float2bfloat16_rn(r2);
-                *reinterpret_cast<__nv_bfloat16*>(sB1 + op16_off<KP>(c, D)) = b1;       // after the chunk stores above
-                *reinterpret_cast<__nv_bfloat16*>(sB1 + op16_off<KP>(c, D + 1)) = b2;
-                *reinterpret_cast<__nv_bfloat16*>(sB1 + op16_off<KP>(c, D + 2)) = b3;
-            }
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(GSX_FULL, mx, o));
-            if (lane == 0) sh->red[warp] = mx;
-            __syncthreads();
-            mx = sh->red[0];
-#pragma unroll
-            for (int w = 1; w < kTcThreads / 32; ++w) mx = fmaxf(mx, sh->red[w]);
-            Cm = sqrtf(mx) * 1.0001f;
-            cur_prob = g.p;
-        }
-
-        if (g.bulk) {
-            if (!mbar_wait(&sh->bar_copy, copy_phase)) failed = true;
-            copy_phase ^= 1;
-        }
-        const bool live = row < g.rows;
+        // ---- scores of this warpgroup's 64 rows: NB blocks of 64 columns, KP/8 TF32 k-steps each
         {
-            const float* src = g.bulk ? sStage + (g.pre >> 2) + row * D : X + g.off_floats + (long long)row * D;
-            float xa = 0.f, xb = 0.f;
-            const int j0 = half == 0 ? 0 : GH, j1 = half == 0 ? GH : G8;
+            const uint32_t a0 = smem_u32(sA) + (uint32_t)(wg * 8) * kSbo, b0 = smem_u32(sB);
+            acc_fence<NB>(acc);
+            asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
 #pragma unroll
-            for (int jj = 0; jj < GH; ++jj) {
-                const int j = j0 + jj;
-                if (j < j1) {
-                    float v[8];
+            for (int b = 0; b < NB; ++b)
 #pragma unroll
-                    for (int e = 0; e < 8; ++e) {
-                        const int k = 8 * j + e;
-                        v[e] = (k < D && live) ? src[k] : 0.f;
-                        if (e & 1) xb = __fmaf_rn(v[e], v[e], xb); else xa = __fmaf_rn(v[e], v[e], xa);
-                    }
-                    uint4 hi, lo;
-                    split8(v, hi, lo);
-                    // the three bias columns D..D+2 of A1 hold 1.0 (bf16 0x3F80); A2 holds 0 there
-#pragma unroll
-                    for (int e = 0; e < 8; ++e) {
-                        const int k = 8 * j + e;
-                        if (k >= D && k < D + 3) {
-                            uint32_t* w32 = &hi.x + (e >> 1);
-                            *w32 = (e & 1) ? ((*w32 & 0x0000ffffu) | 0x3F800000u) : ((*w32 & 0xffff0000u) | 0x00003F80u);
-                        }
-                    }
-                    *reinterpret_cast<uint4*>(sA1 + op16_off<KP>(row, 8 * j)) = hi;
-                    *reinterpret_cast<uint4*>(sA2 + op16_off<KP>(row, 8 * j)) = lo;
-                }
-            }
-            sh->xn[half][row] = xa + xb;
+                for (int j = 0; j < KP / 8; ++j)  // one instruction = 8 TF32 along K = two core matrices = 256 B
+                    wgmma_tf32_n64(acc[b], gmma_desc(a0 + (uint32_t)j * 256u, kLbo, kSbo),
+                                   gmma_desc(b0 + (uint32_t)(b * 8) * kSbo + (uint32_t)j * 256u, kLbo, kSbo), j > 0);
+            asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+            asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+            acc_fence<NB>(acc);
         }
-        fence_proxy_async();
-        tc_fence_before();
-        __syncthreads();
-        if (t + 1 < t1) cur = geo(t + 1);
-        if (tid == 0) {
-            tc_fence_after();
-            if (t + 1 < t1 && cur.bulk) {
-                mbar_expect_tx(&sh->bar_copy, cur.bytes);
-                bulk_g2s(sStage, reinterpret_cast<const char*>(X) + (cur.off_floats * 4 - cur.pre), cur.bytes,
-                         &sh->bar_copy);
-            }
-            const uint32_t a1 = smem_u32(sA1), a2 = smem_u32(sA2), b1 = smem_u32(sB1), b2 = smem_u32(sB2);
-#pragma unroll
-            for (int j = 0; j < KP / 16; ++j) {  // one instruction = 16 bf16 along K = two core matrices = 256 bytes
-                const uint32_t ko = (uint32_t)j * 256u;
-                umma_bf16(tmem_base, umma_desc(a1 + ko, lbo, sbo), umma_desc(b1 + ko, lbo, sbo), idesc, j > 0);
-                umma_bf16(tmem_base, umma_desc(a1 + ko, lbo, sbo), umma_desc(b2 + ko, lbo, sbo), idesc, 1);
-                umma_bf16(tmem_base, umma_desc(a2 + ko, lbo, sbo), umma_desc(b1 + ko, lbo, sbo), idesc, 1);
-            }
-            umma_commit(&sh->bar_mma);
-        }
-        if (!mbar_wait(&sh->bar_mma, mma_phase)) failed = true;
-        mma_phase ^= 1;
-        tc_fence_after();
-        if (failed) break;
 
-        const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16);
-        if (mode == 1) {
-            for (int w = ch_lo; w < ch_hi; ++w) {
-                float v[32];
-                tmem_ld32(taddr + w * 32, v);
+        if (mode == 1) {  // debug: raw scores of the tile
 #pragma unroll
-                for (int i = 0; i < 32; ++i) dump[(size_t)row * npad + w * 32 + i] = v[i];
-            }
+            for (int b = 0; b < NB; ++b)
+#pragma unroll
+                for (int r = 0; r < 32; ++r) {
+                    const int row = erow0 + 8 * ((r >> 1) & 1);
+                    const int col = 64 * b + 8 * (r >> 2) + 2 * quad + (r & 1);
+                    if (col < npad) dump[(size_t)row * npad + col] = acc[b][r];
+                }
             break;
         }
 
-        // ---- single pass: keys (score with the column in the low 8 mantissa bits), two largest per thread
-        float k1a = -INFINITY, k2a = -INFINITY, k1b = -INFINITY, k2b = -INFINITY;   // two independent chains
+        // ---- epilogue, for each of this thread's two rows
 #pragma unroll
-        for (int ww = 0; ww < NCH / 2; ++ww) {
-            const int w = ch_lo + ww;
-            if (w < ch_hi) {
-                float v[32];
-                tmem_ld32(taddr + w * 32, v);
+        for (int i = 0; i < 2; ++i) {
+            const int row = erow0 + 8 * i;
+            const bool live = row < g.rows;
+            // pass 1: row maximum over this thread's columns, then over the quad
+            float m0 = -INFINITY, m1 = -INFINITY;
 #pragma unroll
-                for (int i = 0; i < 32; i += 2) {
-                    const float ka = __uint_as_float((__float_as_uint(v[i]) & 0xFFFFFF00u) | (uint32_t)(w * 32 + i));
-                    const float kb = __uint_as_float((__float_as_uint(v[i + 1]) & 0xFFFFFF00u) | (uint32_t)(w * 32 + i + 1));
-                    const float la = fminf(k1a, ka), lb = fminf(k1b, kb);
-                    k1a = fmaxf(k1a, ka);
-                    k1b = fmaxf(k1b, kb);
-                    k2a = fmaxf(k2a, la);
-                    k2b = fmaxf(k2b, lb);
+            for (int b = 0; b < NB; ++b)
+#pragma unroll
+                for (int j = 0; j < 8; ++j) {
+                    m0 = fmaxf(m0, acc[b][4 * j + 2 * i]);
+                    m1 = fmaxf(m1, acc[b][4 * j + 2 * i + 1]);
                 }
-            }
-        }
-        {
-            const float m1 = fmaxf(k1a, k1b);
-            const float m2 = fmaxf(fminf(k1a, k1b), fmaxf(k2a, k2b));
-            sh->pb1[half][row] = m1;
-            sh->pb2[half][row] = m2;
-        }
-        pair_sync(q);
-        const float o1 = sh->pb1[half ^ 1][row], o2 = sh->pb2[half ^ 1][row];
-        const float m1 = sh->pb1[half][row], m2 = sh->pb2[half][row];
-        const float best = fmaxf(m1, o1);
-        const float second = fmaxf(fminf(m1, o1), fmaxf(m2, o2));
-        const float xn = sh->xn[0][row] + sh->xn[1][row];
-        const float xnu = xn * 1.0001f;
-        const float xnorm = sqrtf(xnu) * 1.0001f;
-        const float scale = xnorm * Cm + 0.5f * Cm * Cm;
-        const float eta = kEps * scale * 2.0f + 1e-37f;
-        const float e_ub = fmaxf(xnu - 2.f * best + 2.f * eta, 0.f);
-        const float marg = 2.f * eta + kGs * e_ub;
-        const float thr = best - marg;
-        const bool bad = !(marg < 3.0e38f) || !(best > -1.0e30f) || !(e_ub < 1.0e19f);
-        const bool need = live && (bad || second >= thr);
-        if (!need && live && half == 0) labels[g.row0 + row] = (int)(__float_as_uint(best) & 0xFFu);
-        if (__any_sync(GSX_FULL, need)) {   // same rows in both warps of the pair: both take the branch
-            uint32_t mask[NCH / 2];
+            float smax = fmaxf(m0, m1);
+            smax = fmaxf(smax, __shfl_xor_sync(GSX_FULL, smax, 1));
+            smax = fmaxf(smax, __shfl_xor_sync(GSX_FULL, smax, 2));
+            const float xn = sh->xn[0][row] + sh->xn[1][row];
+            const float xnu = xn * 1.0001f;
+            const float xnorm = sqrtf(xnu) * 1.0001f;
+            const float eta = (kEpsIn * xnorm * Cm + kEpsAcc * (xnorm * Cm + Cm * Cm)) * 1.5f + 1e-37f;
+            const float e_ub = fmaxf(xnu - 2.f * smax + 2.f * eta, 0.f);
+            const float marg = 2.f * eta + kGs * e_ub;
+            const float thr = smax - marg;
+            // pass 2: candidate mask of this thread's columns; bit 16b + 2j + e <-> column 64b + 8j + 2 quad + e
+            uint64_t mask = 0;
 #pragma unroll
-            for (int ww = 0; ww < NCH / 2; ++ww) {
-                mask[ww] = 0;
-                const int w = ch_lo + ww;
-                if (w < ch_hi) {
-                    if (bad) {
-                        const int left = K - w * 32;
-                        mask[ww] = left >= 32 ? 0xffffffffu : (left > 0 ? (1u << left) - 1u : 0u);
-                    } else {
-                        float v[32];
-                        tmem_ld32(taddr + w * 32, v);
-                        uint32_t ma = 0;
+            for (int b = 0; b < NB; ++b)
 #pragma unroll
-                        for (int i = 0; i < 32; ++i)
-                            if (v[i] >= thr) ma |= 1u << i;
-                        mask[ww] = ma;
-                    }
+                for (int j = 0; j < 8; ++j) {
+                    if (acc[b][4 * j + 2 * i] >= thr) mask |= 1ull << (16 * b + 2 * j);
+                    if (acc[b][4 * j + 2 * i + 1] >= thr) mask |= 1ull << (16 * b + 2 * j + 1);
                 }
-            }
+            const int cnt = __popcll(mask);
+            int total = cnt + __shfl_xor_sync(GSX_FULL, cnt, 1);
+            total += __shfl_xor_sync(GSX_FULL, total, 2);
+            // the shortcut is only legal when the margin is finite, a real centroid scored, and the strict distance
+            // of the winner cannot reach the contract's 1e20 "no label" sentinel.  The quad agrees on all of it.
+            const bool bad = !(marg < 3.0e38f) || !(smax > -1.0e30f) || !(e_ub < 1.0e19f) || total == 0;
+            auto col_of = [&](int bit) { return 64 * (bit >> 4) + 8 * ((bit & 15) >> 1) + 2 * quad + (bit & 1); };
+            if (!bad && total == 1 && cnt == 1 && live) labels[g.row0 + row] = col_of(__ffsll((long long)mask) - 1);
+            const bool need = live && (bad || total > 1);
             if (!need) {
+                mask = 0;
+            } else if (bad) {  // full strict scan over the real centroids of this thread
+                mask = 0;
 #pragma unroll
-                for (int ww = 0; ww < NCH / 2; ++ww) mask[ww] = 0;
+                for (int bit = 0; bit < NB * 16; ++bit)
+                    if (col_of(bit) < K) mask |= 1ull << bit;
             }
-            float bestd = 1e20f;
+            float best = 1e20f;
             int bk = -1;
-            if (need && half == 0) {
+            while (mask) {  // ascending column order
+                const int c = col_of(__ffsll((long long)mask) - 1);
+                mask &= mask - 1;
+                float a = 0.f;
+#pragma unroll
+                for (int j = 0; j < (D + 3) / 4; ++j) {
+                    const float4 xv = *reinterpret_cast<const float4*>(sA + op_off<KP>(row, 4 * j));
+                    const float4 cv = *reinterpret_cast<const float4*>(sB + op_off<KP>(c, 4 * j));
+                    const float xa[4] = {xv.x, xv.y, xv.z, xv.w}, ca[4] = {cv.x, cv.y, cv.z, cv.w};
+#pragma unroll
+                    for (int e = 0; e < 4; ++e)
+                        if (4 * j + e < D) {
+                            const float df = __fsub_rn(xa[e], ca[e]);
+                            a = __fadd_rn(a, __fmul_rn(df, df));
+                        }
+                }
+                ++st_strict;
+                if (a < best) best = a, bk = c;
+            }
+            // quad: lexicographic minimum of (distance, index) == the serial ascending scan with strict '<'
+#pragma unroll
+            for (int o = 1; o <= 2; o <<= 1) {
+                const float ob = __shfl_xor_sync(GSX_FULL, best, o);
+                const int ok = __shfl_xor_sync(GSX_FULL, bk, o);
+                if (ob < best || (ob == best && ok >= 0 && (bk < 0 || ok < bk))) best = ob, bk = ok;
+            }
+            if (need && quad == 0) {
+                labels[g.row0 + row] = bk;
                 ++st_multi;
                 if (bad) ++st_full;
             }
-            const float* xr = X + g.off_floats + (long long)row * D;   // exact float32 row (L2-resident: just streamed)
-            for (;;) {
-                int c = -1;
-#pragma unroll
-                for (int ww = NCH / 2 - 1; ww >= 0; --ww)
-                    if (mask[ww]) c = (ch_lo + ww) * 32 + __ffs(mask[ww]) - 1;
-                if (!__any_sync(GSX_FULL, c >= 0)) break;
-                if (c >= 0) {
-#pragma unroll
-                    for (int ww = 0; ww < NCH / 2; ++ww)
-                        if ((c >> 5) - ch_lo == ww) mask[ww] &= mask[ww] - 1;
-                    const float* cr = Cp + (size_t)c * D;
-                    float acc = 0.f;
-#pragma unroll
-                    for (int k = 0; k < D; ++k) {
-                        const float df = __fsub_rn(__ldg(xr + k), __ldg(cr + k));
-                        acc = __fadd_rn(acc, __fmul_rn(df, df));
-                    }
-                    ++st_strict;
-                    if (acc < bestd) bestd = acc, bk = c;
-                }
-            }
-            if (half == 1) {
-                sh->pbest[row] = bestd;
-                sh->pbk[row] = bk;
-            }
-            pair_sync(q);
-            if (half == 0 && need) {
-                const float hb = sh->pbest[row];
-                if (hb < bestd) bk = sh->pbk[row];
-                labels[g.row0 + row] = bk;
-            }
-            pair_sync(q);
         }
+        __syncthreads();  // sA is rewritten for the next tile only after every strict evaluation and MMA read it
     }
 
     if (failed && err_flag) atomicExch(err_flag, 1);
@@ -867,80 +410,55 @@ __global__ void __launch_bounds__(kTcThreads, 2)
             atomicAdd(tc_stats + 2, st_full);
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) tmem_free(tmem_base, (uint32_t)tmem_cols);
 }
 
-template <int D, int KP>
-static int launch_tc16(const float* X, long long x_floats, const float* C, int* labels, const KmProb* probs, int nprob,
-                       int K, long long tiles, int mode, float* dump, unsigned long long* stats, int* err, cudaStream_t st) {
-    const int npad = (K + 31) / 32 * 32;
-    int cols = 32;
-    while (cols < npad) cols <<= 1;
-    const size_t smem = (size_t)2 * (kTcMaxN + kTcRows) * KP * 2 + (size_t)(kTcRows * D + 8) * 4 + sizeof(Tc16Shared) + 64;
-    static bool attr_done = false;
-    if (!attr_done) {
-        GSX_CUDA_CHECK(cudaFuncSetAttribute(k_km_assign_tc16<D, KP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        attr_done = true;
-    }
-    long long grid = (long long)sm_count() * 2;
-    if (grid > tiles) grid = tiles;
-    if (mode == 1) grid = 1;
-    if (grid < 1) grid = 1;
-    k_km_assign_tc16<D, KP><<<(int)grid, kTcThreads, smem, st>>>(X, x_floats, C, labels, probs, nprob, K, npad, cols, tiles,
-                                                                 mode, dump, stats, err);
-    return GSX_OK;
-}
-
-#endif  // GSX_KM_TC16
-
-template <int D, int KP>
+template <int D, int KP, int NB>
 static int launch_tc(const float* X, long long x_floats, const float* C, int* labels, const KmProb* probs, int nprob,
-                     int K, long long tiles, int variant, int mode, float* dump, unsigned long long* stats, int* err,
+                     int K, long long tiles, int mode, float* dump, unsigned long long* stats, int* err,
                      cudaStream_t st) {
     const int npad = (K + 31) / 32 * 32;
-    int cols = 32;
-    while (cols < npad) cols <<= 1;
     const size_t smem = (size_t)(kTcMaxN + kTcRows) * KP * 4 + (size_t)(kTcRows * D + 8) * 4 + sizeof(TcShared) + 64;
-    static bool attr_done = false;
-    if (!attr_done) {
-        GSX_CUDA_CHECK(cudaFuncSetAttribute(k_km_assign_tc<D, KP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        attr_done = true;
+    static int per_sm = 0;
+    if (per_sm == 0) {
+        GSX_CUDA_CHECK(cudaFuncSetAttribute(k_km_assign_tc<D, KP, NB>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                            (int)smem));
+        GSX_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_km_assign_tc<D, KP, NB>, kTcThreads, smem));
+        if (per_sm < 1) per_sm = 1;
     }
-    long long grid = (long long)sm_count() * 2;  // two CTAs per SM: 2 x 256 TMEM columns, 2 x ~97 KB shared memory
+    long long grid = (long long)sm_count() * per_sm;
     if (grid > tiles) grid = tiles;
     if (mode == 1) grid = 1;
     if (grid < 1) grid = 1;
-    k_km_assign_tc<D, KP><<<(int)grid, kTcThreads, smem, st>>>(X, x_floats, C, labels, probs, nprob, K, npad, cols, tiles,
-                                                               variant, mode, dump, stats, err);
+    k_km_assign_tc<D, KP, NB><<<(int)grid, kTcThreads, smem, st>>>(X, x_floats, C, labels, probs, nprob, K, npad, tiles,
+                                                                   mode, dump, stats, err);
     return GSX_OK;
 }
 
-bool kmeans_tc16_built() { return GSX_KM_TC16 != 0; }
+template <int D, int KP>
+static int launch_tc_n(const float* X, long long x_floats, const float* C, int* labels, const KmProb* probs, int nprob,
+                       int K, long long tiles, int mode, float* dump, unsigned long long* stats, int* err,
+                       cudaStream_t st) {
+    if (K <= 64) return launch_tc<D, KP, 1>(X, x_floats, C, labels, probs, nprob, K, tiles, mode, dump, stats, err, st);
+    if (K <= 128) return launch_tc<D, KP, 2>(X, x_floats, C, labels, probs, nprob, K, tiles, mode, dump, stats, err, st);
+    return launch_tc<D, KP, 4>(X, x_floats, C, labels, probs, nprob, K, tiles, mode, dump, stats, err, st);
+}
+
+// The split-bf16 variant (variant 2) is not part of this library.
+bool kmeans_tc16_built() { return false; }
 
 bool kmeans_tc_supported(int K, int D) { return (D == 9 || D == 24 || D == 45) && K >= 1 && K <= kTcMaxN; }
 
 int kmeans_assign_tc(const float* X, long long x_floats, const float* C, int* labels, const KmProb* probs_dev, int nprob,
                      int K, int D, long long tiles, int variant, int mode, float* dump, unsigned long long* stats,
                      int* err_flag_dev, cudaStream_t st) {
-    if (variant == 2) {  // split-bf16 scores, single-pass epilogue
-#if !GSX_KM_TC16
-        set_error("kmeans_tc: the split-bf16 variant is a build-time experiment (compile gsx_kmeans_tc.cu with -DGSX_KM_TC16=1)");
+    if (variant != 0) {
+        set_error("kmeans_tc: only the TF32 variant (0) is built, got %d", variant);
         return GSX_ERR_UNSUPPORTED;
-#else
-        switch (D) {
-            case 9: return launch_tc16<9, 16>(X, x_floats, C, labels, probs_dev, nprob, K, tiles, mode, dump, stats, err_flag_dev, st);
-            case 24: return launch_tc16<24, 32>(X, x_floats, C, labels, probs_dev, nprob, K, tiles, mode, dump, stats, err_flag_dev, st);
-            case 45: return launch_tc16<45, 48>(X, x_floats, C, labels, probs_dev, nprob, K, tiles, mode, dump, stats, err_flag_dev, st);
-            default: set_error("kmeans_tc: unsupported D=%d", D); return GSX_ERR_UNSUPPORTED;
-        }
-#endif
     }
     switch (D) {
-        case 9: return launch_tc<9, 16>(X, x_floats, C, labels, probs_dev, nprob, K, tiles, variant, mode, dump, stats, err_flag_dev, st);
-        case 24: return launch_tc<24, 32>(X, x_floats, C, labels, probs_dev, nprob, K, tiles, variant, mode, dump, stats, err_flag_dev, st);
-        case 45: return launch_tc<45, 48>(X, x_floats, C, labels, probs_dev, nprob, K, tiles, variant, mode, dump, stats, err_flag_dev, st);
+        case 9: return launch_tc_n<9, 16>(X, x_floats, C, labels, probs_dev, nprob, K, tiles, mode, dump, stats, err_flag_dev, st);
+        case 24: return launch_tc_n<24, 32>(X, x_floats, C, labels, probs_dev, nprob, K, tiles, mode, dump, stats, err_flag_dev, st);
+        case 45: return launch_tc_n<45, 48>(X, x_floats, C, labels, probs_dev, nprob, K, tiles, mode, dump, stats, err_flag_dev, st);
         default: set_error("kmeans_tc: unsupported D=%d", D); return GSX_ERR_UNSUPPORTED;
     }
 }

@@ -1,4 +1,4 @@
-// gsx_knn_exact.cu -- SOR with the reference's CPU-path semantics (exact KNN, float64) on sm_100a.
+// gsx_knn_exact.cu -- SOR with the reference's CPU-path semantics (exact KNN, float64) on sm_90a.
 //
 // Replaces /root/reference/gsconverter/processing/data_processor.py:155-173: scipy cKDTree over the
 // float32 coordinates promoted to float64, query k+1 nearest (the first is the point itself or a

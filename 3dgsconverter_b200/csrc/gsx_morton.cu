@@ -1,4 +1,4 @@
-// gsx_morton.cu -- Morton ordering as a shared primitive (SURVEY 8(f) item 3) for sm_100a.
+// gsx_morton.cu -- Morton ordering as a shared primitive (SURVEY 8(f) item 3) for sm_90a (H100).
 //
 //   gsx_morton_order   formats/compressed_ply.py:252-297 (_sort_morton_order): 3 x 10-bit Morton code of the position
 //                      normalised to the bounding box of the group, argsort, and RECURSION into every run of equal

@@ -1,4 +1,4 @@
-// gsx_radix.cu -- stable LSD radix sort of (uint64 key, int32 value) pairs, hand-written for sm_100a.
+// gsx_radix.cu -- stable LSD radix sort of (uint64 key, int32 value) pairs, hand-written for sm_90a (H100).
 //
 // Serves the hash-grid build (gpu_ops.py:227 `np.argsort(hashed)`; word = bucket | Morton code | index, keys only)
 // and, as (key, value) pairs, the Morton orderings of the exact-KNN path and of compressed_ply / ksplat and the SOG
@@ -390,7 +390,7 @@ static int onesweep_sort(uint64_t* keys0, uint64_t* keys1, int32_t* vals0, int32
     GSX_CUDA_CHECK(cudaMemsetAsync(ws, 0, ((size_t)kOsMaxPass * 256 + 64 + (size_t)npass * 256 * ntiles) * sizeof(uint32_t), st));
     static int hist_blocks = 0;
     if (!hist_blocks) {
-        int dev = 0, sms = 148;
+        int dev = 0, sms = 132;
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
         hist_blocks = sms * 8;
@@ -437,7 +437,7 @@ int radix_sort_pairs(uint64_t* keys0, uint64_t* keys1, int32_t* vals0, int32_t* 
     GSX_REQUIRE(ws_bytes >= radix_ws_bytes(n), GSX_ERR_WORKSPACE, "radix: workspace too small");
     GSX_REQUIRE(begin_bit >= 0 && end_bit <= 64 && begin_bit < end_bit, GSX_ERR_ARG, "radix: bad bit range");
     // onesweep whenever the look-back words can hold the counts (30 bits) -- GSX_RADIX_ONESWEEP=0 builds keep the
-    // three-kernel passes for the A/B in profiles/
+    // three-kernel passes for A/B comparisons
     if (GSX_RADIX_ONESWEEP && n < (1ll << 30))
         return onesweep_sort<true>(keys0, keys1, vals0, vals1, n, begin_bit, end_bit, (uint32_t*)ws, keys_sorted,
                                    vals_sorted, st);

@@ -1,4 +1,4 @@
-// gsx_records.cu -- device-resident splat records (SURVEY 8(f) items 2 and 4) for sm_100a.
+// gsx_records.cu -- device-resident splat records (SURVEY 8(f) items 2 and 4) for sm_90a (H100).
 //
 // The reference's interchange record is a packed row of F float32 fields (structures.py:23-59: 62 fields = 248 bytes
 // for SH degree 3).  Every filter of the reference extracts xyz / opacity with np.column_stack

@@ -1,10 +1,10 @@
-// gsx_sor.cu -- Statistical Outlier Removal, Taichi semantics, for sm_100a.
+// gsx_sor.cu -- Statistical Outlier Removal, Taichi semantics, for sm_90a (H100).
 //
 // Replaces /root/reference/gsconverter/processing/gpu_ops.py:193-263 (host driver
 // filter_sor_gpu) and :98-176 (Taichi kernel sor_compute_mean_dists).  Normative
 // arithmetic: SURVEY.md Appendix A.1.
 //
-// Design (B200-first, not a translation of the Taichi kernel):
+// Design (GPU-first, not a translation of the Taichi kernel):
 //   * grid build entirely on device: min/max reduce -> 64-bit key (bucket hash << 15 |
 //     5+5+5-bit Morton code of the position inside the cell) -> radix sort -> float4
 //     gather (w carries the original index, so the "unsort" is fused into the query
@@ -951,7 +951,7 @@ __device__ __forceinline__ float warp_sort32(float v, int lane) {
 #define GSX_KNN_FIRST_SORT 1
 #endif
 // long buckets that span fewer than this many supers (1024 points each) skip the super-box level (0: never).
-// A/B (profiles/r02c_knn_variants.log): 8 -> -1.4 % on the mixed cloud (within ~1 % run-to-run noise), 32 -> +6 %.
+// 8 was chosen by A/B timing against 32 on the mixed cloud.
 #ifndef GSX_KNN_FLAT_SUPERS
 #define GSX_KNN_FLAT_SUPERS 8
 #endif
@@ -1331,7 +1331,7 @@ __global__ void __launch_bounds__(256, GSX_KNN_MINBLOCKS)
 
 #ifndef GSX_KNN16
 #define GSX_KNN16 0   // 1: K <= 16 goes to the two-queries-per-warp kernel (gsx_sor_knn16.cuh) -- an A/B variant, it
-                      // measured SLOWER than the warp-per-query kernel (profiles/r02_knn16_variants.log)
+                      // measured SLOWER than the warp-per-query kernel
 #endif
 #include "gsx_sor_knn16.cuh"
 

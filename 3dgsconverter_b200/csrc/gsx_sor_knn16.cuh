@@ -11,7 +11,7 @@
 // The warp NEVER diverges: every loop runs while EITHER half still needs it (`__any_sync`) and a half that is done is
 // predicated off with no-op inputs (an empty range, a sentinel candidate, an all-ones key).  A first version let the
 // halves branch independently with half-warp masks on every shuffle / vote: once apart they never re-joined and every
-// instruction issued twice with 16 lanes -- 3x SLOWER than k_sor_knn (profiles/r02_knn16_variants.log).  All
+// instruction issued twice with 16 lanes -- 3x SLOWER than k_sor_knn.  All
 // shuffles here are full-mask with width 16 (or xor < 16), votes are full-mask ballots shifted to the half.
 //
 // Semantics are those of k_sor_knn (gpu_ops.py:98-176): same candidate set per query (the buckets of the 27 probes),

@@ -138,7 +138,7 @@ class DataProcessor:
         debug_print(f"SOR Filter (Remove Flyers) Params: K={k}, Sigma={threshold_factor:.2f}")
         num_points = self._count()
         _require_backend()
-        status_print("[SOR] Determining outliers on GPU (gsx / sm_100a)...")
+        status_print("[SOR] Determining outliers on GPU (gsx / sm_90a)...")
         if num_points == 0:
             return self.data
         chain = self._working_set()

@@ -1,4 +1,4 @@
-"""Drop-in for ``gsconverter/processing/gpu_ops.py`` backed by libgsx.so (hand-written sm_100a CUDA).
+"""Drop-in for ``gsconverter/processing/gpu_ops.py`` backed by libgsx.so (hand-written sm_90a CUDA).
 
 Same importable surface as the reference (gpu_ops.py:8-46,193-263):
 

@@ -1,7 +1,7 @@
-"""gsx -- host side of the B200-native filtering / clustering backend.
+"""gsx -- host side of the H100-native filtering / clustering backend.
 
 Python here is plumbing only: torch tensors are the device-buffer container and the
-stream source; all compute is in libgsx.so (hand-written sm_100a CUDA behind a C ABI).
+stream source; all compute is in libgsx.so (hand-written sm_90a CUDA behind a C ABI).
 """
 from . import _abi  # noqa: F401  (raises ImportError if libgsx.so has not been built)
 from ._abi import GsxError  # noqa: F401

@@ -20,7 +20,7 @@ class GsxError(RuntimeError):
 if not LIB_PATH.exists():
     raise ImportError(
         f"libgsx.so not found at {LIB_PATH}: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-        "(nvcc, sm_100a).  gsx has no CPU fallback.")
+        "(nvcc, sm_90a).  gsx has no CPU fallback.")
 
 lib = C.CDLL(str(LIB_PATH))
 

@@ -341,8 +341,7 @@ def sor_filter_distributed(xyz_local: torch.Tensor, k: int = 25, threshold_facto
     n = int(sum(sizes))
     means_full = torch.zeros(n, dtype=torch.float32, device=dev)
     # batches of 16 consecutive sorted positions dealt round-robin over the ranks: every rank samples the whole hash
-    # range, so the expensive clustered buckets do not all land on the owner of their hash range (measured at N=4:
-    # slowest rank 8.7 ms vs 6.6 ms mean with contiguous segments)
+    # range, so the expensive clustered buckets do not all land on the owner of their hash range
     ops.mean_dists_strided(grid, k, hash_mode, means_full, dist.get_world_size(group), rank)
     st.mark("knn")
     means_local = route_to_slabs(means_full, sizes, rank, group)

@@ -1,6 +1,6 @@
 """NumPy array <-> CUDA tensor through libgsx's staged copies (gsx_copy_h2d / gsx_copy_d2h, csrc/gsx_hostcopy.cu):
 pageable host buffers are moved by several host threads through pinned chunks, so the PCIe link stays busy
-(torch's `.to(device)` / `.cpu()` of a pageable array run on one thread at ~11 GB/s)."""
+(torch's `.to(device)` / `.cpu()` of a pageable array run on one thread)."""
 from __future__ import annotations
 
 import numpy as np

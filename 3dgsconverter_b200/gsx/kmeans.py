@@ -12,7 +12,7 @@ from .sor import _ptr, _stream
 
 
 def default_assign_mode() -> str:
-    """auto = tensor cores (tcgen05) when the shape allows it; GSX_KMEANS_ASSIGN overrides (labels are bit-identical
+    """auto = tensor cores (wgmma) when the shape allows it; GSX_KMEANS_ASSIGN overrides (labels are bit-identical
     in every mode -- the switch exists for A/B timing and tests)."""
     return os.environ.get("GSX_KMEANS_ASSIGN", "auto")
 
@@ -22,7 +22,7 @@ def tensor_core_supported(K: int, D: int) -> bool:
 
 
 def tensor_bf16_built() -> bool:
-    """The split-bf16 variant is a build-time experiment (-DGSX_KM_TC16=1), not part of the shipped library."""
+    """The split-bf16 variant is not part of this library (always False)."""
     return bool(lib.gsx_kmeans_tensor_core_supported(256, 45) & 2)
 
 

@@ -1,5 +1,5 @@
 /*
- * gsx.h -- C ABI of libgsx.so, the B200-native (sm_100a) backend for the per-point
+ * gsx.h -- C ABI of libgsx.so, the H100-native (sm_90a) backend for the per-point
  * filtering + codebook clustering hot path of francescofugazzi/3dgsconverter.
  *
  * The reference has no FFI of its own (it is pure Python + Taichi); the boundary it
@@ -228,15 +228,11 @@ int64_t gsx_kmeans_workspace_bytes(int64_t n_total, int32_t nprob, int32_t K, in
  *   STRICT         the contract's distance for every (point, centroid) on the FP32 pipes
  *   FMA_PREFILTER  D >= 9: one fma per (point, centroid, dim) scores every centroid, the strict distance is
  *                  evaluated only for the centroids within a proven rounding-error margin of the best score
- *   TENSOR         the same scheme with the score matrix X.C^T - ||c||^2/2 computed by tcgen05.mma (kind::tf32, float32
- *                  accumulators in TMEM, two-pass epilogue: row maximum, candidate mask); error if the shape is
+ *   TENSOR         the same scheme with the score matrix X.C^T - ||c||^2/2 computed by wgmma.mma_async (TF32, float32
+ *                  accumulators in registers, two-pass epilogue: row maximum, candidate mask); error if the shape is
  *                  unsupported (D in {9,24,45}, K <= 256)
- *   TENSOR_BF16    variant with split-bf16 operands (x = x1 + x2, three kind::f16 MMAs per K step, score error 2^-16
- *                  instead of 2^-9, so ~0.2 % instead of ~9 % of the points need a strict evaluation) and a single-pass
- *                  packed-key top-2 epilogue; measured slower than TENSOR on B200 (the top-2 costs more ALU work than
- *                  it saves in TMEM reads, profiles/r02_km_tc16_ncu.json).  A BUILD-TIME experiment: the shipped library
- *                  returns GSX_ERR_UNSUPPORTED for it unless gsx_kmeans_tc.cu was compiled with -DGSX_KM_TC16=1
- *                  (gsx_kmeans_tensor_core_supported reports bit 1 then)
+ *   TENSOR_BF16    a split-bf16 variant of TENSOR that this library does not build: returns GSX_ERR_UNSUPPORTED
+ *                  (gsx_kmeans_tensor_core_supported never reports bit 1)
  * tc_stats_dev (may be NULL): 3 uint64 counters accumulated by the TENSOR path {strict distance evaluations,
  * points with more than one candidate, points that needed the full strict scan}. */
 #define GSX_KM_ASSIGN_AUTO 0
@@ -302,7 +298,7 @@ int gsx_kmeans_host_batched(const float* X_host, const int64_t* row_off_host, in
                             int32_t max_iter, float* C_host_inout, int32_t* labels_host, int32_t assign_mode);
 /* Copies between a caller's HOST buffer and HBM, used by every *_host entry point above.  The reference's call sites
  * pass ordinary (pageable) NumPy arrays -- np.column_stack at data_processor.py:139, the shN block of
- * sog.py:536-549 -- which cudaMemcpy stages on one CPU thread at ~11 GB/s; these stage through a pool of pinned
+ * sog.py:536-549 -- which cudaMemcpy stages on one CPU thread; these stage through a pool of pinned
  * chunks filled / drained by several host threads (GSX_COPY_THREADS, default 8), each enqueueing its own DMAs, so
  * the PCIe link stays busy.  Pinned / registered / managed buffers and copies below 8 MiB take plain
  * cudaMemcpyAsync (GSX_STAGED_COPY=0 forces that path).

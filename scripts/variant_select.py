@@ -1,5 +1,5 @@
 """A/B of libgsx build variants on the GPU box, with a parity digest per variant; optionally installs the fastest one
-as 3dgsconverter_b200/lib/libgsx.so so that the tests / ncu / bench that follow in the same gpurun call use it.
+as 3dgsconverter_b200/lib/libgsx.so so that the tests and bench that follow use it.
 
     python scripts/variant_select.py [--install] [--n 10000000]
 

@@ -12,7 +12,7 @@ for p in (str(ROOT), str(PKG)):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100; select with -m gpu)")
     config.addinivalue_line("markers", "slow: takes more than a few seconds on CPU")
 
 

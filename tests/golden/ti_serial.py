@@ -1,8 +1,8 @@
-"""A serial stand-in for the sliver of Taichi that /root/reference/gsconverter/processing/gpu_ops.py uses, so
+"""A serial stand-in for the sliver of Taichi that the reference's gsconverter/processing/gpu_ops.py uses, so
 that the REFERENCE'S OWN KERNEL SOURCE (k_means_assign, k_means_update, sor_compute_mean_dists and the host
 drivers _kmeans_taichi / filter_sor_gpu around them) can be executed in this container, where the real taichi
 wheel cannot be installed.  TEST INFRASTRUCTURE ONLY -- used by make_taichi_goldens.py (which writes
-tests/golden/g4_reference_kernels.npz) and by the live CPU pin in tests/test_reference_kernels_pin.py.
+tests/golden/g4_reference_kernels.npz) and by make_taichi_golden_g9.py (tests/golden/g9_reference_stand_in_small.npz).
 
 `install()` puts a module named `taichi` into sys.modules.  Its `@ti.kernel` takes the decorated function's
 source text (inspect.getsource), rewrites the AST so that Python's untyped scalars behave like Taichi's

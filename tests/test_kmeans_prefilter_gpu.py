@@ -1,4 +1,4 @@
-"""GPU: K-Means with the exact pre-filters (fma scores on the FP32 pipes, or tcgen05 TF32 scores in TMEM) is
+"""GPU: K-Means with the exact pre-filters (fma scores on the FP32 pipes, or wgmma TF32 scores) is
 bit-identical to the oracle (labels, counts, centroids), including adversarial near-tie inputs and the fallbacks."""
 import numpy as np
 import pytest
@@ -21,7 +21,7 @@ def _check(X, k, it, cuda, mode, seed=1234):
     if mode.startswith("tensor") and not gk.tensor_core_supported(k, X.shape[1]):
         pytest.skip("shape not supported by the tensor-core path")
     if mode == "tensor_bf16" and not gk.tensor_bf16_built():
-        pytest.skip("split-bf16 variant not compiled in (build-time experiment, -DGSX_KM_TC16=1)")
+        pytest.skip("split-bf16 variant is not part of this library")
     C, L, cnt = gk.kmeans_lloyd(torch.from_numpy(X).to(cuda), k, it, torch.from_numpy(init).to(cuda), assign=mode)
     assert np.array_equal(L.cpu().numpy(), Lo)
     assert np.array_equal(cnt.cpu().numpy(), cnto)

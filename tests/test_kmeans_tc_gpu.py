@@ -1,4 +1,4 @@
-"""GPU: the tcgen05 (tensor-core) K-Means assign -- score GEMM in TMEM, candidate margin, strict re-evaluation.
+"""GPU: the wgmma (tensor-core) K-Means assign -- score GEMM in registers, candidate margin, strict re-evaluation.
 Labels / counts / centroids bit-identical to the oracle and to the strict CUDA-core kernel at the C3 chunk size
 (SURVEY 8(d): one full 781 250 x 45 chunk vs the oracle, all-chunk run-to-run determinism)."""
 import numpy as np
@@ -14,7 +14,7 @@ def _tf32(a):
 @pytest.mark.parametrize("variant,rel", [(0, 2.0 ** -9), (2, 2.0 ** -15)])
 @pytest.mark.parametrize("D,K", [(45, 256), (45, 50), (24, 100), (9, 16)])
 def test_tc_scores_are_the_gemm(D, K, variant, rel, cuda, gsx_lib):
-    """The TMEM accumulator holds x.c - ||c||^2/2 (layout / descriptor check) within the input-conversion error the
+    """The accumulator holds x.c - ||c||^2/2 (layout / descriptor check) within the input-conversion error the
     margin assumes: variant 0 = kind::tf32 (2^-10 per operand), variant 2 = split-bf16, three kind::f16 products."""
     import torch
     from gsx import kmeans as gk
@@ -22,7 +22,7 @@ def test_tc_scores_are_the_gemm(D, K, variant, rel, cuda, gsx_lib):
     X = rng.normal(0, 0.15, (128, D)).astype(np.float32)
     C = rng.normal(0, 0.15, (K, D)).astype(np.float32)
     if variant == 2 and not gk.tensor_bf16_built():
-        pytest.skip("split-bf16 variant not compiled in (build-time experiment, -DGSX_KM_TC16=1)")
+        pytest.skip("split-bf16 variant is not part of this library")
     S = gk.tc_debug_scores(torch.from_numpy(X).to(cuda), torch.from_numpy(C).to(cuda), variant).cpu().numpy()[:, :K]
     exact = X.astype(np.float64) @ C.astype(np.float64).T - 0.5 * (C.astype(np.float64) ** 2).sum(1)[None]
     bound = rel * (np.linalg.norm(X, axis=1)[:, None] * np.linalg.norm(C, axis=1)[None] + 0.5 * (C ** 2).sum(1)[None]) + 1e-7
@@ -54,7 +54,7 @@ def test_tc_bf16_variant_margin_is_tight(cuda, gsx_lib):
     import torch
     from gsx import kmeans as gk
     if not gk.tensor_bf16_built():
-        pytest.skip("split-bf16 variant not compiled in (build-time experiment, -DGSX_KM_TC16=1)")
+        pytest.skip("split-bf16 variant is not part of this library")
     n, D, K = 400_000, 45, 256
     g = torch.Generator(device=cuda).manual_seed(9)
     proto = torch.randn(1024, D, device=cuda, generator=g) * 0.15

@@ -1,5 +1,5 @@
 """GPU (>= 2 devices): the sharded drivers over NCCL reproduce the single-GPU results bit for bit.
-Skipped on a one-GPU box; run with `gpurun --gpus 2 -- python -m pytest tests/test_multigpu_nccl.py -m gpu`."""
+Skipped on a machine with one GPU; run on two or more with `python -m pytest tests/test_multigpu_nccl.py -m gpu`."""
 import os
 import sys
 from pathlib import Path
