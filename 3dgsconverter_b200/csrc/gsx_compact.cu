@@ -5,7 +5,8 @@
 // opacity (4 B/pt) and the original row index (4 B/pt).  The 248-byte records stay on the host and
 // are gathered ONCE, with the surviving indices, when the caller reads `DataProcessor.data`.
 // Stable (order-preserving), like NumPy boolean indexing: one pass with decoupled look-back over per-tile survivor
-// counts (k_cmp_onepass) instead of count -> multi-level scan -> scatter, which reads the mask twice.
+// counts (k_cmp_onepass) when n < 2^30, where its 30-bit look-back counts cannot overflow; from 2^30 rows on,
+// count -> multi-level scan -> scatter (k_cmp_count, k_cmp_scatter), which reads the mask twice.
 #include "gsx_common.cuh"
 #include "gsx_compact.cuh"
 #include "gsx_radix.cuh"
@@ -61,10 +62,6 @@ __global__ void __launch_bounds__(kCmpBlock)
     idx_out[pos] = idx ? idx[i] : (int32_t)i;
 }
 
-#ifndef GSX_COMPACT_ONEPASS
-#define GSX_COMPACT_ONEPASS 1   // single pass with decoupled look-back; 0 = the count -> scan -> scatter form (A/B)
-#endif
-#if GSX_COMPACT_ONEPASS
 constexpr int kOpThreads = 256, kOpPer = 8, kOpTile = kOpThreads * kOpPer;   // 2048 rows per tile
 constexpr uint32_t kLbAgg = 1u << 30, kLbInc = 1u << 31, kLbVal = (1u << 30) - 1u;
 
@@ -163,7 +160,6 @@ __global__ void __launch_bounds__(kOpThreads)
         xyz_out[3 * obase + t3] = __ldg(xyz + 3 * (tbase + s_src[t]) + c);
     }
 }
-#endif
 
 int64_t compact_workspace_bytes(int64_t n) {
     if (n < 1) n = 1;
@@ -181,8 +177,7 @@ int compact_points(const uint8_t* mask, int64_t n, const float* xyz, const float
     }
     GSX_REQUIRE(ws_bytes >= compact_workspace_bytes(n), GSX_ERR_WORKSPACE, "compact: workspace too small");
     GSX_REQUIRE((opacity == nullptr) == (opacity_out == nullptr), GSX_ERR_ARG, "compact: opacity in/out mismatch");
-#if GSX_COMPACT_ONEPASS
-    {
+    if (n < (1ll << 30)) {   // the look-back words carry 30-bit survivor counts (kLbVal)
         const int64_t tiles = (n + kOpTile - 1) / kOpTile;   // (fits the two-pass workspace: fewer tiles than blocks)
         uint32_t* words = (uint32_t*)ws;                      // [0] tile counter, [1] total, [16 ..] look-back words
         GSX_CUDA_CHECK(cudaMemsetAsync(words, 0, (size_t)(tiles + 16) * 4, st));
@@ -195,7 +190,6 @@ int compact_points(const uint8_t* mask, int64_t n, const float* xyz, const float
         *count_host = (int64_t)total1;
         return GSX_OK;
     }
-#endif
     const int64_t blocks = (n + kCmpBlock - 1) / kCmpBlock;
     uint32_t* counts = (uint32_t*)ws;          // blocks + 1 (total in the extra slot after the scan)
     uint32_t* sws = counts + blocks + 64;

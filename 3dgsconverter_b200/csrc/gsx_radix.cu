@@ -2,8 +2,8 @@
 //
 // Serves the hash-grid build (gpu_ops.py:227 `np.argsort(hashed)`; word = bucket | Morton code | index, keys only)
 // and, as (key, value) pairs, the Morton orderings of the exact-KNN path and of compressed_ply / ksplat and the SOG
-// lexsort.  8-bit digits.  Two forms of a pass: the onesweep form further down is the one used (see there); the
-// three-kernel form is kept for n >= 2^30 and as the A/B baseline (-DGSX_RADIX_ONESWEEP=0):
+// lexsort.  8-bit digits.  Two forms of a pass: the onesweep form further down is the one used whenever n < 2^30 (see
+// there); the three-kernel form serves n >= 2^30, where the onesweep look-back words cannot hold the counts:
 //   k_rs_hist    per-tile digit histogram (tile = 4096 keys, one CTA)  -> hist[digit][tile]
 //   exclusive scan of the digit-major matrix (multi-level block scan)   -> global base of (digit, tile)
 //   k_rs_scatter per-tile stable ranks: every warp owns 512 consecutive keys, ranks them 32 at a time
@@ -18,9 +18,6 @@
 namespace gsx {
 
 #define GSX_FULL 0xffffffffu
-#ifndef GSX_RADIX_ONESWEEP
-#define GSX_RADIX_ONESWEEP 1
-#endif
 constexpr int kRsThreads = 256;
 constexpr int kRsPerThread = 16;
 constexpr int kRsTile = kRsThreads * kRsPerThread;  // 4096
@@ -436,9 +433,8 @@ int radix_sort_pairs(uint64_t* keys0, uint64_t* keys1, int32_t* vals0, int32_t* 
     GSX_REQUIRE(n >= 1 && n < 4294967296ll, GSX_ERR_ARG, "radix: n out of range");
     GSX_REQUIRE(ws_bytes >= radix_ws_bytes(n), GSX_ERR_WORKSPACE, "radix: workspace too small");
     GSX_REQUIRE(begin_bit >= 0 && end_bit <= 64 && begin_bit < end_bit, GSX_ERR_ARG, "radix: bad bit range");
-    // onesweep whenever the look-back words can hold the counts (30 bits) -- GSX_RADIX_ONESWEEP=0 builds keep the
-    // three-kernel passes for A/B comparisons
-    if (GSX_RADIX_ONESWEEP && n < (1ll << 30))
+    // onesweep whenever the look-back words can hold the counts (30 bits)
+    if (n < (1ll << 30))
         return onesweep_sort<true>(keys0, keys1, vals0, vals1, n, begin_bit, end_bit, (uint32_t*)ws, keys_sorted,
                                    vals_sorted, st);
     const int64_t ntiles = (n + kRsTile - 1) / kRsTile;

@@ -40,20 +40,24 @@ namespace gsx {
 #define GSX_D2LIM_BITS 0x60ad78ebu
 #define GSX_FULL 0xffffffffu
 
-#ifndef GSX_MORTON_BITS
-#define GSX_MORTON_BITS 15
-#endif
-constexpr int kMortonBits = GSX_MORTON_BITS;       // in-cell Morton code: kMortonBits/3 bits per axis
-constexpr float kMortonScale = (float)(1 << (GSX_MORTON_BITS / 3));
+constexpr int kMortonBits = 15;       // in-cell Morton code: kMortonBits/3 bits per axis
+constexpr float kMortonScale = (float)(1 << (kMortonBits / 3));
 constexpr float kMortonMax = kMortonScale - 1.f;
-#ifndef GSX_SMALL_BUCKET
-#define GSX_SMALL_BUCKET 64
-#endif
-constexpr int kSmallBucket = GSX_SMALL_BUCKET;  // buckets up to this size are scanned without box tests
-#ifndef GSX_QUERY_BATCH
-#define GSX_QUERY_BATCH 16
-#endif
-constexpr int kQueryBatch = GSX_QUERY_BATCH;   // consecutive queries grabbed per warp
+// tuning constants of the query kernel (kSmallBucket also bounds the serial walk of k_sor_bucket_tail)
+constexpr int kSmallBucket = 64;      // buckets up to this size are scanned without box tests
+constexpr int kQueryBatch = 16;       // consecutive queries grabbed per warp
+constexpr int kMergeThreshold = 9;    // serial insert ~11 instr each vs ~95 for a full merge
+constexpr int kKnnMinBlocks = 8;      // __launch_bounds__ minimum of resident CTAs per SM
+// long buckets that span fewer than this many supers (1024 points each) skip the super-box level.
+// 8 was chosen by A/B timing against 32 on the mixed cloud.
+constexpr int kFlatSupers = 8;
+// names the query kernel's tuning constants in every bench line (gsx_build_info).  epi_smem=1 (batched epilogue),
+// first_sort=1 (first merge as a plain sort), knn16=0 (one query per warp for every K), tma=0 (no TMA staging) and
+// i32=1 (32-bit positions) describe fixed properties of the kernel; they stay so that bench lines remain comparable.
+const char* sor_build_info() {
+    return "knn=r02c;epi_smem=1;first_sort=1;query_batch=16;minblocks=8;merge_threshold=9;small_bucket=64;"
+           "flat_supers=8;knn16=0;tma=0;i32=1";
+}
 
 // ------------------------------------------------------------------ workspace layout
 
@@ -404,6 +408,37 @@ __global__ void __launch_bounds__(1024)
     }
 }
 
+// Box of the sorted positions [s, end) of one bucket, as this lane's part of a warp-wide reduction (the caller
+// reduces lo/hi over the warp): the points of the partial chunks at either end, and the boxes of the whole chunks in
+// between (caabb must be complete).
+__device__ __forceinline__ void bucket_box_partial(const float4* __restrict__ spos, const float4* __restrict__ caabb,
+                                                   int64_t s, int64_t end, int lane, float (&lo)[3], float (&hi)[3]) {
+    lo[0] = lo[1] = lo[2] = INFINITY;
+    hi[0] = hi[1] = hi[2] = -INFINITY;
+    int64_t cf = (s + 31) >> 5, cl = end >> 5;  // full chunks [cf, cl)
+    int64_t head_end = cf * 32, tail_begin = cl * 32;
+    if (cf > cl) {  // the bucket lies inside one chunk: reduce it point by point
+        head_end = end;
+        tail_begin = end;
+        cf = cl = 0;
+    }
+    for (int64_t t = s + lane; t < head_end; t += 32) {
+        float4 p = spos[t];
+        lo[0] = fminf(lo[0], p.x), lo[1] = fminf(lo[1], p.y), lo[2] = fminf(lo[2], p.z);
+        hi[0] = fmaxf(hi[0], p.x), hi[1] = fmaxf(hi[1], p.y), hi[2] = fmaxf(hi[2], p.z);
+    }
+    for (int64_t c = cf + lane; c < cl; c += 32) {
+        float4 a = caabb[2 * c], b = caabb[2 * c + 1];
+        lo[0] = fminf(lo[0], a.x), lo[1] = fminf(lo[1], a.y), lo[2] = fminf(lo[2], a.z);
+        hi[0] = fmaxf(hi[0], a.w), hi[1] = fmaxf(hi[1], b.x), hi[2] = fmaxf(hi[2], b.y);
+    }
+    for (int64_t t = tail_begin + lane; t < end; t += 32) {
+        float4 p = spos[t];
+        lo[0] = fminf(lo[0], p.x), lo[1] = fminf(lo[1], p.y), lo[2] = fminf(lo[2], p.z);
+        hi[0] = fmaxf(hi[0], p.x), hi[1] = fmaxf(hi[1], p.y), hi[2] = fmaxf(hi[2], p.z);
+    }
+}
+
 // Bounding box of every occupied bucket (exact over its points): lets the query kernel skip whole buckets whose
 // box is farther than the current K-th best, and visit the 27 probes nearest first.  Each warp takes the bucket
 // starts among its 32 sorted positions (startbits) and reduces each bucket cooperatively (stride 32 over the
@@ -430,29 +465,8 @@ __device__ __forceinline__ void
         const int64_t s = chunk * 32 + src;
         const uint32_t hb = __shfl_sync(GSX_FULL, my_h, src);
         const int64_t end = __shfl_sync(GSX_FULL, my_end, src);
-        float lo[3] = {INFINITY, INFINITY, INFINITY}, hi[3] = {-INFINITY, -INFINITY, -INFINITY};
-        int64_t cf = (s + 31) >> 5, cl = end >> 5;  // full chunks [cf, cl)
-        int64_t head_end = cf * 32, tail_begin = cl * 32;
-        if (cf > cl) {  // the bucket lies inside one chunk: reduce it point by point
-            head_end = end;
-            tail_begin = end;
-            cf = cl = 0;
-        }
-        for (int64_t t = s + lane; t < head_end; t += 32) {
-            float4 p = spos[t];
-            lo[0] = fminf(lo[0], p.x), lo[1] = fminf(lo[1], p.y), lo[2] = fminf(lo[2], p.z);
-            hi[0] = fmaxf(hi[0], p.x), hi[1] = fmaxf(hi[1], p.y), hi[2] = fmaxf(hi[2], p.z);
-        }
-        for (int64_t c = cf + lane; c < cl; c += 32) {
-            float4 a = caabb[2 * c], b = caabb[2 * c + 1];
-            lo[0] = fminf(lo[0], a.x), lo[1] = fminf(lo[1], a.y), lo[2] = fminf(lo[2], a.z);
-            hi[0] = fmaxf(hi[0], a.w), hi[1] = fmaxf(hi[1], b.x), hi[2] = fmaxf(hi[2], b.y);
-        }
-        for (int64_t t = tail_begin + lane; t < end; t += 32) {
-            float4 p = spos[t];
-            lo[0] = fminf(lo[0], p.x), lo[1] = fminf(lo[1], p.y), lo[2] = fminf(lo[2], p.z);
-            hi[0] = fmaxf(hi[0], p.x), hi[1] = fmaxf(hi[1], p.y), hi[2] = fmaxf(hi[2], p.z);
-        }
+        float lo[3], hi[3];
+        bucket_box_partial(spos, caabb, s, end, lane, lo, hi);
 #pragma unroll
         for (int a = 0; a < 3; ++a)
 #pragma unroll
@@ -664,29 +678,8 @@ __global__ void __launch_bounds__(256)
         }
         const float4 p0 = spos[s];
         const uint32_t hb = bucket_of(p0.x, p0.y, p0.z, bx, by, bz, cell, n, M64);
-        float lo[3] = {INFINITY, INFINITY, INFINITY}, hi[3] = {-INFINITY, -INFINITY, -INFINITY};
-        int64_t cf = (s + 31) >> 5, cl = end >> 5;  // full chunks [cf, cl)
-        int64_t head_end = cf * 32, tail_begin = cl * 32;
-        if (cf > cl) {
-            head_end = end;
-            tail_begin = end;
-            cf = cl = 0;
-        }
-        for (int64_t t = s + lane; t < head_end; t += 32) {
-            float4 p = spos[t];
-            lo[0] = fminf(lo[0], p.x), lo[1] = fminf(lo[1], p.y), lo[2] = fminf(lo[2], p.z);
-            hi[0] = fmaxf(hi[0], p.x), hi[1] = fmaxf(hi[1], p.y), hi[2] = fmaxf(hi[2], p.z);
-        }
-        for (int64_t c = cf + lane; c < cl; c += 32) {
-            float4 a = caabb[2 * c], b = caabb[2 * c + 1];
-            lo[0] = fminf(lo[0], a.x), lo[1] = fminf(lo[1], a.y), lo[2] = fminf(lo[2], a.z);
-            hi[0] = fmaxf(hi[0], a.w), hi[1] = fmaxf(hi[1], b.x), hi[2] = fmaxf(hi[2], b.y);
-        }
-        for (int64_t t = tail_begin + lane; t < end; t += 32) {
-            float4 p = spos[t];
-            lo[0] = fminf(lo[0], p.x), lo[1] = fminf(lo[1], p.y), lo[2] = fminf(lo[2], p.z);
-            hi[0] = fmaxf(hi[0], p.x), hi[1] = fmaxf(hi[1], p.y), hi[2] = fmaxf(hi[2], p.z);
-        }
+        float lo[3], hi[3];
+        bucket_box_partial(spos, caabb, s, end, lane, lo, hi);
 #pragma unroll
         for (int a = 0; a < 3; ++a) {
             lo[a] = ord_to_float(__reduce_min_sync(GSX_FULL, float_to_ord(lo[a])));
@@ -947,20 +940,6 @@ __device__ __forceinline__ float warp_sort32(float v, int lane) {
     return v;
 }
 
-#ifndef GSX_KNN_FIRST_SORT
-#define GSX_KNN_FIRST_SORT 1
-#endif
-// long buckets that span fewer than this many supers (1024 points each) skip the super-box level (0: never).
-// 8 was chosen by A/B timing against 32 on the mixed cloud.
-#ifndef GSX_KNN_FLAT_SUPERS
-#define GSX_KNN_FLAT_SUPERS 8
-#endif
-// Epilogue of a query (gpu_ops.py:163-174: serial float32 sum of the valid distances, mean) -- batched: every query
-// of a batch parks its K ascending distances and its row number in shared memory, and after the batch lane q sums
-// query q (16 serial sums run side by side instead of one shuffle + add per rank on lane 0 of every query).
-#ifndef GSX_KNN_EPI_SMEM
-#define GSX_KNN_EPI_SMEM 1
-#endif
 template <int NREG>
 struct TopK {
     float v0, v1;  // lane l holds rank l (v0) and rank 32+l (v1) of the ascending d^2 list
@@ -992,7 +971,6 @@ struct TopK {
     // >= rank K-1, so they never change the K smallest (only the multiset of values matters, A.1-7).
     __device__ __forceinline__ void merge32(float nv, int lane) {
         nv = warp_sort32(nv, lane);
-#if GSX_KNN_FIRST_SORT
         // the first merge of a query meets an empty list (32 sentinels): the sorted candidates ARE the merged list --
         // skips the reversal and the 5 merge stages (the sentinel is the largest value either side can hold)
         if (__all_sync(GSX_FULL, v0 == __uint_as_float(GSX_D2LIM_BITS))) {
@@ -1000,7 +978,6 @@ struct TopK {
             refresh_tau();
             return;
         }
-#endif
         float r = __shfl_sync(GSX_FULL, nv, 31 - lane);
         float m = fminf(v0, r);
 #pragma unroll
@@ -1011,33 +988,15 @@ struct TopK {
 };
 
 // positions in the hash-sorted order fit 31 bits (n < 2^31 - 64): 32-bit index arithmetic in the scan loops
-#ifndef GSX_KNN_I32
-#define GSX_KNN_I32 1
-#endif
-#if GSX_KNN_I32
 typedef int pos_t;
-#else
-typedef int64_t pos_t;
-#endif
-// A/B variant named by BASELINE.json's north_star: stage the query's centre bucket (<= 64 points = 1 KiB) into shared
-// memory with a 1-D TMA bulk copy (cp.async.bulk + mbarrier) once per cell change, and scan it from there.
-#ifndef GSX_KNN_TMA
-#define GSX_KNN_TMA 0
-#endif
-
-#ifndef GSX_MERGE_THRESHOLD
-#define GSX_MERGE_THRESHOLD 9
-#endif
-constexpr int kMergeThreshold = GSX_MERGE_THRESHOLD;  // serial insert ~11 instr each vs ~95 for a full merge
 
 // distance of the query to candidate j and ballot/shfl insertion of the lanes that beat tau
 template <int NREG, bool STATS>
 __device__ __forceinline__ void scan32(const float4* __restrict__ spos, pos_t j, bool valid, float qx, float qy,
-                                       float qz, TopK<NREG>& tk, int lane, unsigned long long& n_scanned,
-                                       const float4* sbuf = nullptr) {
+                                       float qz, TopK<NREG>& tk, int lane, unsigned long long& n_scanned) {
     float d2 = INFINITY;
     if (valid) {
-        float4 c = sbuf ? sbuf[lane] : __ldg(spos + j);
+        float4 c = __ldg(spos + j);
         float ax = __fsub_rn(qx, c.x), ay = __fsub_rn(qy, c.y), az = __fsub_rn(qz, c.z);
         d2 = __fadd_rn(__fadd_rn(__fmul_rn(ax, ax), __fmul_rn(ay, ay)), __fmul_rn(az, az));
     }
@@ -1056,11 +1015,12 @@ __device__ __forceinline__ void scan32(const float4* __restrict__ spos, pos_t j,
     }
 }
 
-#ifndef GSX_KNN_MINBLOCKS
-#define GSX_KNN_MINBLOCKS 8
-#endif
+// ES > 0: batched epilogue (gpu_ops.py:163-174: serial float32 sum of the valid distances, mean) -- every query of a
+// batch parks its K ascending distances and its row number in shared memory, and after the batch lane q sums query q
+// (16 serial sums run side by side instead of one shuffle + add per rank on lane 0 of every query).  ES = 0: the
+// per-query shuffle epilogue (K > 32).
 template <int NREG, bool STATS, int ES>
-__global__ void __launch_bounds__(256, GSX_KNN_MINBLOCKS)
+__global__ void __launch_bounds__(256, kKnnMinBlocks)
     k_sor_knn(const float4* __restrict__ spos, const int2* __restrict__ tab_se, const float4* __restrict__ tab_box,
               const uint32_t* __restrict__ cellbits, const float4* __restrict__ caabb,
               const float4* __restrict__ saabb, float* __restrict__ final_means, unsigned int* __restrict__ work,
@@ -1074,16 +1034,6 @@ __global__ void __launch_bounds__(256, GSX_KNN_MINBLOCKS)
     // odd so that the lanes of the final pass (one query each) read distinct banks
     extern __shared__ float s_epi[];
     float* const epi = s_epi + (threadIdx.x >> 5) * (kQueryBatch * (ES > 0 ? ES : 1));
-#if GSX_KNN_TMA
-    __shared__ __align__(128) float4 s_stage[8][kSmallBucket];
-    __shared__ __align__(8) unsigned long long s_bar[8];
-    float4* wbuf = s_stage[threadIdx.x >> 5];
-    const uint32_t bar_addr = (uint32_t)__cvta_generic_to_shared(&s_bar[threadIdx.x >> 5]);
-    uint32_t bar_phase = 0;
-    int staged_s = -1, staged_c = 0;
-    if (lane == 0) asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar_addr) : "memory");
-    __syncwarp();
-#endif
     // probe offsets of lane p<27 in the reference's loop order (dx outer, dz inner)
     const int pdx = lane / 9 - 1, pdy = (lane / 3) % 3 - 1, pdz = lane % 3 - 1;
 
@@ -1097,40 +1047,21 @@ __global__ void __launch_bounds__(256, GSX_KNN_MINBLOCKS)
         if (qb >= q_end) break;
         int64_t qe = qb + kQueryBatch < q_end ? qb + kQueryBatch : q_end;
         // the 27 probes of a query depend only on its cell: consecutive hash-sorted queries mostly share
-        // it, so the hashes and table entries are recomputed only when the cell changes
-#ifndef GSX_KNN_CELLBITS
-#define GSX_KNN_CELLBITS 1
-#endif
-#if GSX_KNN_CELLBITS
-        // one bit per sorted position (k_sor_finish): "another grid cell than the position before".  A batch is 16
+        // it, so the hashes and table entries are recomputed only when the cell changes.
+        // One bit per sorted position (k_sor_finish): "another grid cell than the position before".  A batch is 16
         // consecutive positions inside one 32-bit word (kQueryBatch divides 32, batches are aligned to q_begin).
         const uint32_t cellword = __ldg(cellbits + (qb >> 5));
-#else
-        int cgx = 0x7fffffff, cgy = 0, cgz = 0;
-#endif
         int ps = 0, pc = 0;                                  // lane p: bucket range of probe p
         float blx = 0.f, bly = 0.f, blz = 0.f, bhx = 0.f, bhy = 0.f, bhz = 0.f;  // and its bounding box
         const pos_t qb_p = (pos_t)qb, qe_p = (pos_t)qe;      // positions fit 31 bits (pos_t): 32-bit loop bookkeeping
 #pragma unroll 1
         for (pos_t i = qb_p; i < qe_p; ++i) {
             const float4 q = __ldg(spos + i);
-#if GSX_KNN_CELLBITS
             const uint32_t w_i = (i >> 5) == (qb_p >> 5) ? cellword : __ldg(cellbits + (i >> 5));
             if (i == qb_p || ((w_i >> (i & 31)) & 1u)) {   // warp-uniform by construction
                 const int gx = (int)floorf(__fdiv_rn(__fsub_rn(q.x, bx), cell));
                 const int gy = (int)floorf(__fdiv_rn(__fsub_rn(q.y, by), cell));
                 const int gz = (int)floorf(__fdiv_rn(__fsub_rn(q.z, bz), cell));
-#else
-            const int gx = (int)floorf(__fdiv_rn(__fsub_rn(q.x, bx), cell));
-            const int gy = (int)floorf(__fdiv_rn(__fsub_rn(q.y, by), cell));
-            const int gz = (int)floorf(__fdiv_rn(__fsub_rn(q.z, bz), cell));
-#ifndef GSX_CELL_REUSE
-#define GSX_CELL_REUSE 1
-#endif
-            // (vote makes the predicate provably warp-uniform: no reconvergence code in the loop below)
-            if (!GSX_CELL_REUSE || __any_sync(GSX_FULL, gx != cgx || gy != cgy || gz != cgz)) {
-                cgx = gx, cgy = gy, cgz = gz;
-#endif
                 ps = 0, pc = 0;
                 if (lane < 27) {
                     uint32_t h = probe_hash(gx + pdx, gy + pdy, gz + pdz, n, M, hash_mode);
@@ -1142,38 +1073,6 @@ __global__ void __launch_bounds__(256, GSX_KNN_MINBLOCKS)
                         blx = b0.x, bly = b0.y, blz = b0.z, bhx = b1.x, bhy = b1.y, bhz = b1.z;
                     }
                 }
-#if GSX_KNN_TMA
-                {   // stage the centre bucket of the new cell (if it is a small one) for the queries that share it
-                    const int s13 = __shfl_sync(GSX_FULL, ps, 13), c13 = __shfl_sync(GSX_FULL, pc, 13);
-                    staged_c = 0;
-                    if (c13 > 0 && c13 <= kSmallBucket) {
-                        __syncwarp();   // every lane is done with the previous contents of wbuf
-                        if (lane == 0) {
-                            const uint32_t bytes = (uint32_t)c13 * 16u;
-                            asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar_addr), "r"(bytes) : "memory");
-                            asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                                             (uint32_t)__cvta_generic_to_shared(wbuf)),
-                                         "l"(spos + s13), "r"(bytes), "r"(bar_addr)
-                                         : "memory");
-                        }
-                        uint32_t ok = 0;
-                        for (unsigned spin = 0; !ok && spin < (1u << 24); ++spin) {   // bounded: never hang the GPU
-                            asm volatile(
-                                "{\n\t.reg .pred p;\n\t"
-                                "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-                                "selp.u32 %0, 1, 0, p;\n\t}"
-                                : "=r"(ok)
-                                : "r"(bar_addr), "r"(bar_phase)
-                                : "memory");
-                        }
-                        bar_phase ^= 1u;
-                        if (__all_sync(GSX_FULL, ok != 0)) {
-                            staged_s = s13;
-                            staged_c = c13;
-                        }
-                    }
-                }
-#endif
             }
             if (STATS) {
                 int tot = pc;
@@ -1219,17 +1118,9 @@ __global__ void __launch_bounds__(256, GSX_KNN_MINBLOCKS)
                 const int s = __shfl_sync(GSX_FULL, ps, p), c = __shfl_sync(GSX_FULL, pc, p);
                 const pos_t e = (pos_t)s + c;
                 if (c <= kSmallBucket) {
-#if GSX_KNN_TMA
-                    const bool from_smem = staged_c > 0 && s == staged_s;   // warp-uniform
-#pragma unroll 1
-                    for (pos_t base = s; base < e; base += 32)
-                        scan32<NREG, STATS>(spos, base + lane, base + lane < e, q.x, q.y, q.z, tk, lane, st_scanned,
-                                            from_smem ? wbuf + (base - s) : nullptr);
-#else
 #pragma unroll 1
                     for (pos_t base = s; base < e; base += 32)
                         scan32<NREG, STATS>(spos, base + lane, base + lane < e, q.x, q.y, q.z, tk, lane, st_scanned);
-#endif
                     continue;
                 }
                 const int skip = p == 13 ? skip_chunk : -1;
@@ -1254,15 +1145,13 @@ __global__ void __launch_bounds__(256, GSX_KNN_MINBLOCKS)
                         scan32<NREG, STATS>(spos, j, j >= s && j < e, q.x, q.y, q.z, tk, lane, st_scanned);
                     }
                 };
-#if GSX_KNN_FLAT_SUPERS > 0
                 // a bucket of a few supers: every super box is near the query (it sits in or next to this bucket), so
                 // the super level prunes nothing -- test the chunk boxes directly, 32 at a time (exact either way: a
                 // chunk is skipped only when its lower bound is >= the current tau, and tau never grows)
-                if (ls - fs < GSX_KNN_FLAT_SUPERS) {
+                if (ls - fs < kFlatSupers) {
                     for (int cb = fc; cb <= lc; cb += 32) chunk_group(cb);
                     continue;
                 }
-#endif
                 for (int sb = fs; sb <= ls; sb += 32) {
                     const int sid = sb + lane;
                     unsigned skey = 0xffffffffu;
@@ -1329,65 +1218,27 @@ __global__ void __launch_bounds__(256, GSX_KNN_MINBLOCKS)
     }
 }
 
-#ifndef GSX_KNN16
-#define GSX_KNN16 0   // 1: K <= 16 goes to the two-queries-per-warp kernel (gsx_sor_knn16.cuh) -- an A/B variant, it
-                      // measured SLOWER than the warp-per-query kernel
-#endif
-#include "gsx_sor_knn16.cuh"
-
 __global__ void k_fill_f32(float* p, int64_t n, float v) {
     int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) p[i] = v;
 }
 
-template <int NREG, bool STATS, int ES>
+// ES = row stride of the batched shared-memory epilogue (0: per-query shuffle epilogue)
+template <int NREG, int ES>
 static int launch_knn(SorWs& w, int64_t q_begin, int64_t q_end, int q_stride, int q_phase, int K, int hash_mode,
                       const float* bmin, float cell,
                       float* final_means, unsigned long long* stats, uint64_t M, int64_t want, cudaStream_t st) {
+    const auto kernel = stats ? k_sor_knn<NREG, true, ES> : k_sor_knn<NREG, false, ES>;
     int per_sm = 0;
     const size_t smem = (size_t)8 * kQueryBatch * ES * sizeof(float);
-    GSX_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_sor_knn<NREG, STATS, ES>, 256, smem));
+    GSX_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, 256, smem));
     int64_t grid = (int64_t)sm_count() * (per_sm > 0 ? per_sm : 4);  // persistent: exactly the resident CTAs
     if (grid > want) grid = want;
     if (grid < 1) grid = 1;
-    k_sor_knn<NREG, STATS, ES><<<(int)grid, 256, smem, st>>>(w.spos, w.tab_se, w.tab_box, w.cellbits, w.caabb, w.saabb, final_means, w.counters,
-                                                      q_begin, q_end, q_stride, q_phase, K, hash_mode, bmin[0], bmin[1],
-                                                      bmin[2], cell,
-                                                      (uint32_t)w.n, M, stats);
+    kernel<<<(int)grid, 256, smem, st>>>(w.spos, w.tab_se, w.tab_box, w.cellbits, w.caabb, w.saabb, final_means, w.counters,
+                                         q_begin, q_end, q_stride, q_phase, K, hash_mode, bmin[0], bmin[1], bmin[2], cell,
+                                         (uint32_t)w.n, M, stats);
     return GSX_OK;
-}
-
-template <bool STATS>
-static int launch_knn16(SorWs& w, int64_t q_begin, int64_t q_end, int q_stride, int q_phase, int K, int hash_mode,
-                        const float* bmin, float cell, float* final_means, unsigned long long* stats, uint64_t M,
-                        int64_t want, cudaStream_t st) {
-    int per_sm = 0;
-    GSX_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_sor_knn16<STATS>, 256, 0));
-    int64_t grid = (int64_t)sm_count() * (per_sm > 0 ? per_sm : 4);
-    want = (want + 1) / 2;   // a block takes 16 batches at a time, not 8
-    if (grid > want) grid = want;
-    if (grid < 1) grid = 1;
-    k_sor_knn16<STATS><<<(int)grid, 256, 0, st>>>(w.spos, w.tab_se, w.tab_box, w.cellbits, w.caabb, w.saabb, final_means,
-                                                  w.counters, q_begin, q_end, q_stride, q_phase, K, hash_mode, bmin[0],
-                                                  bmin[1], bmin[2], cell, (uint32_t)w.n, M, stats);
-    return GSX_OK;
-}
-
-// compile-time configuration of the query kernel (A/B variants differ only here): recorded next to every ncu capture
-// and checked by bench.py before it uses a capture's instruction count for the roofline
-#define GSX_STR2(x) #x
-#define GSX_STR(x) GSX_STR2(x)
-#if GSX_KNN_FLAT_SUPERS > 0
-#define GSX_FLAT_INFO ";flat_supers=" GSX_STR(GSX_KNN_FLAT_SUPERS)
-#else
-#define GSX_FLAT_INFO ""
-#endif
-const char* sor_build_info() {
-    return "knn=r02c"
-           ";epi_smem=" GSX_STR(GSX_KNN_EPI_SMEM) ";first_sort=" GSX_STR(GSX_KNN_FIRST_SORT)
-           ";query_batch=" GSX_STR(GSX_QUERY_BATCH) ";minblocks=" GSX_STR(GSX_KNN_MINBLOCKS)
-           ";merge_threshold=" GSX_STR(GSX_MERGE_THRESHOLD) ";small_bucket=" GSX_STR(GSX_SMALL_BUCKET)
-           GSX_FLAT_INFO ";knn16=" GSX_STR(GSX_KNN16) ";tma=" GSX_STR(GSX_KNN_TMA) ";i32=" GSX_STR(GSX_KNN_I32);
 }
 
 int sor_mean_dists(SorWs& w, int64_t q_begin, int64_t q_end, int q_stride, int q_phase, int k, int hash_mode,
@@ -1412,18 +1263,12 @@ int sor_mean_dists(SorWs& w, int64_t q_begin, int64_t q_end, int q_stride, int q
     int64_t nq = (q_end - q_begin + q_stride - 1) / q_stride + kQueryBatch;   // this launch's share (upper bound)
     int64_t want = (nq + (int64_t)kQueryBatch * 8 - 1) / ((int64_t)kQueryBatch * 8);
     int rc;
-    if (GSX_KNN16 && K <= 16)
-        rc = stats ? launch_knn16<true>(w, q_begin, q_end, q_stride, q_phase, K, hash_mode, bmin, cell, final_means, stats, M, want, st)
-                   : launch_knn16<false>(w, q_begin, q_end, q_stride, q_phase, K, hash_mode, bmin, cell, final_means, stats, M, want, st);
-    else {
-#define GSX_KNN_ARGS w, q_begin, q_end, q_stride, q_phase, K, hash_mode, bmin, cell, final_means, stats, M, want, st
-        // ES = row stride of the batched shared-memory epilogue (0: per-query shuffle epilogue)
-        constexpr int ES16 = GSX_KNN_EPI_SMEM ? 17 : 0, ES32 = GSX_KNN_EPI_SMEM ? 33 : 0;
-        if (K <= 16) rc = stats ? launch_knn<1, true, ES16>(GSX_KNN_ARGS) : launch_knn<1, false, ES16>(GSX_KNN_ARGS);
-        else if (K <= 32) rc = stats ? launch_knn<1, true, ES32>(GSX_KNN_ARGS) : launch_knn<1, false, ES32>(GSX_KNN_ARGS);
-        else rc = stats ? launch_knn<2, true, 0>(GSX_KNN_ARGS) : launch_knn<2, false, 0>(GSX_KNN_ARGS);
-#undef GSX_KNN_ARGS
-    }
+    if (K <= 16)
+        rc = launch_knn<1, 17>(w, q_begin, q_end, q_stride, q_phase, K, hash_mode, bmin, cell, final_means, stats, M, want, st);
+    else if (K <= 32)
+        rc = launch_knn<1, 33>(w, q_begin, q_end, q_stride, q_phase, K, hash_mode, bmin, cell, final_means, stats, M, want, st);
+    else
+        rc = launch_knn<2, 0>(w, q_begin, q_end, q_stride, q_phase, K, hash_mode, bmin, cell, final_means, stats, M, want, st);
     if (rc) return rc;
     GSX_KERNEL_CHECK();
     return GSX_OK;

@@ -37,7 +37,7 @@ extern "C" {
 /* ---- library ---------------------------------------------------------------------- */
 const char* gsx_last_error(void);
 int gsx_version(void);          /* 100*major + minor */
-const char* gsx_build_info(void); /* compile-time switches of the SOR query kernel ("knn=r02c;epi_smem=1;..."): names the
+const char* gsx_build_info(void); /* tuning constants of the SOR query kernel ("knn=r02c;epi_smem=1;..."): names the
                                    * build an ncu capture / a bench line was taken with */
 int gsx_device_sm_count(void);  /* SMs of the current device (grid sizing), <0 on error */
 long long gsx_kernel_launches(void); /* cumulative number of gsx kernels launched by this process */

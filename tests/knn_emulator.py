@@ -33,7 +33,7 @@ def _lb(q, lo, hi):
 
 def emulate(pos, k, mode="i32wrap", chunk=4, fan=4, small_bucket=6, morton_bits=2, flat_supers=0, group=32):
     """final_means float32[N] computed with the kernel's algorithm (chunk = points per chunk, fan = chunks per
-    super, small_bucket = largest bucket scanned without box tests, flat_supers = GSX_KNN_FLAT_SUPERS: a long bucket
+    super, small_bucket = largest bucket scanned without box tests, flat_supers = kFlatSupers: a long bucket
     spanning fewer supers than this tests its chunk boxes directly, `group` at a time, without the super level)."""
     pos = np.ascontiguousarray(pos, dtype=np.float32)
     n = len(pos)

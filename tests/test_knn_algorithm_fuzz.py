@@ -39,7 +39,7 @@ def test_pruning_actually_prunes():
 
 @pytest.mark.parametrize("flat,group", [(2, 3), (8, 4), (1000, 5)])
 def test_flat_walk_of_long_buckets_is_exact(flat, group):
-    """GSX_KNN_FLAT_SUPERS (shipped: 8): a long bucket spanning fewer supers than that tests its chunk boxes directly,
+    """kFlatSupers (shipped: 8): a long bucket spanning fewer supers than that tests its chunk boxes directly,
     `group` at a time, in bucket order instead of nearest-super-first -- a different visiting ORDER, the same rule
     (a chunk is skipped only while its lower bound is >= the current tau), hence the same bits."""
     for name, pts in _clouds():
