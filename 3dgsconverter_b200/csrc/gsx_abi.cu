@@ -6,6 +6,7 @@
 
 #include "gsx_common.cuh"
 #include "gsx_compact.cuh"
+#include "gsx_compressed_ply.cuh"
 #include "gsx_density.cuh"
 #include "gsx_hostcopy.cuh"
 #include "gsx_hostrows.cuh"
@@ -571,6 +572,19 @@ int gsx_chunk_minmax(const float* rows_dev, int64_t n, int32_t F, const int32_t*
                      void* ws, int64_t ws_bytes, void* stream) {
     return chunk_minmax(rows_dev, n, F, order_dev, chunk, cols_host, ncol, clip_lo, clip_hi, lo_dev, hi_dev, ws, ws_bytes,
                         (cudaStream_t)stream);
+}
+
+/* ------------------------------------------------------------------ compressed PLY packing */
+int gsx_cply_pack(const float* rows_dev, int64_t n, int32_t F, const int32_t* order_dev, const int32_t* cols14_host,
+                  const int32_t* rest_cols_host, int32_t n_rest, const float* lo_pos_dc_dev, const float* hi_pos_dc_dev,
+                  const float* lo_scale_dev, const float* hi_scale_dev, float* chunk_dev, uint32_t* vertex_dev,
+                  uint8_t* sh_dev, uint64_t* rest_nonzero_dev, void* stream) {
+    return cply_pack(rows_dev, n, F, order_dev, cols14_host, rest_cols_host, n_rest, lo_pos_dc_dev, hi_pos_dc_dev,
+                     lo_scale_dev, hi_scale_dev, chunk_dev, vertex_dev, sh_dev, (unsigned long long*)rest_nonzero_dev,
+                     (cudaStream_t)stream);
+}
+int gsx_cply_narrow_sh(const uint8_t* sh_dev, int64_t n, int32_t width, int32_t keep, uint8_t* out_dev, void* stream) {
+    return cply_narrow_sh(sh_dev, n, width, keep, out_dev, (cudaStream_t)stream);
 }
 
 /* free / total device memory of the current device (sizing decisions of the host-buffer entry points) */

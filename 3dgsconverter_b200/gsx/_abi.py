@@ -91,6 +91,9 @@ _SIGS = {
     "gsx_morton_order": (C.c_int, [_vp, _i64, _vp, _i32, C.POINTER(_i32), _vp, _i64, _vp]),
     "gsx_chunk_minmax": (C.c_int, [_vp, _i64, _i32, _vp, _i32, C.POINTER(_i32), _i32, C.c_float, C.c_float, _vp, _vp, _vp,
                                    _i64, _vp]),
+    "gsx_cply_pack": (C.c_int, [_vp, _i64, _i32, _vp, C.POINTER(_i32), C.POINTER(_i32), _i32, _vp, _vp, _vp, _vp, _vp, _vp,
+                                _vp, _vp, _vp]),
+    "gsx_cply_narrow_sh": (C.c_int, [_vp, _i64, _i32, _i32, _vp, _vp]),
     "gsx_copy_h2d": (C.c_int, [_vp, _vp, _i64, _vp]),
     "gsx_copy_d2h": (C.c_int, [_vp, _vp, _i64, _vp]),
     "gsx_host_gather_rows": (C.c_int, [_vp, _i64, _i64, _vp, _i64, _vp]),

@@ -1,0 +1,147 @@
+"""PlayCanvas compressed PLY export on the device: formats/compressed_ply.py:126-250 (CompressedPlyFormat.write) over
+DeviceRecords.  The Morton order (gsx_morton_order), the chunk bounds (gsx_chunk_minmax) and the per-splat packing
+(gsx_cply_pack) run on the GPU; only the packed 16 B per splat plus the SH bytes come back to the host.
+
+    enc = encode(records)                       # DeviceRecords -> CompressedPly (device tensors)
+    chunk_data, vertex_data, sh_data = enc.to_host()
+    write_ply("out.compressed.ply", chunk_data, vertex_data, sh_data)
+"""
+from __future__ import annotations
+
+import ctypes as C
+from dataclasses import dataclass
+
+import numpy as np
+import torch
+
+from ._abi import lib, check
+from .sor import _ptr, _stream
+
+CHUNK = 256
+PACK_FIELDS = ("x", "y", "z", "f_dc_0", "f_dc_1", "f_dc_2", "opacity", "scale_0", "scale_1", "scale_2",
+               "rot_0", "rot_1", "rot_2", "rot_3")
+CHUNK_DTYPE = np.dtype([(f, "<f4") for f in (
+    "min_x", "min_y", "min_z", "max_x", "max_y", "max_z",
+    "min_scale_x", "min_scale_y", "min_scale_z", "max_scale_x", "max_scale_y", "max_scale_z",
+    "min_r", "min_g", "min_b", "max_r", "max_g", "max_b")])
+VERTEX_DTYPE = np.dtype([(f, "<u4") for f in ("packed_position", "packed_rotation", "packed_scale", "packed_color")])
+
+
+def sh_keep_limit(last_nonzero: int) -> int:
+    """compressed_ply.py:158-167: how many leading f_rest_i the file keeps, from the last non-zero index."""
+    return 45 if last_nonzero >= 24 else 24 if last_nonzero >= 9 else 9 if last_nonzero >= 0 else 0
+
+
+@dataclass
+class CompressedPly:
+    chunk: torch.Tensor             # float32 [C, 18]
+    vertex: torch.Tensor            # int32 [N, 4]: the four uint32 words of every splat
+    sh: torch.Tensor | None         # uint8 [N, len(sh_names)]
+    sh_names: tuple
+    order: torch.Tensor             # int32 [N]: record index of the j-th splat of the file
+
+    def to_host(self):
+        """(chunk_data, vertex_data, sh_data): the structured arrays the reference passes to _write_ply_file."""
+        from .hostcopy import to_host
+        chunk_data = to_host(self.chunk).reshape(-1).view(CHUNK_DTYPE)
+        vertex_data = to_host(self.vertex).reshape(-1).view(VERTEX_DTYPE)
+        sh_data = None
+        if self.sh is not None:
+            sh_data = to_host(self.sh).reshape(-1).view(np.dtype([(n, "u1") for n in self.sh_names]))
+        return chunk_data, vertex_data, sh_data
+
+
+def encode(records, order: torch.Tensor | None = None) -> CompressedPly:
+    """Pack `records` (DeviceRecords) the way CompressedPlyFormat.write does.  order: None = the recursive Morton order
+    of the reference (gsx_morton_order, ties in ascending index); otherwise a permutation of range(N) (int32)."""
+    from .morton import chunk_minmax, morton_order
+    missing = [f for f in PACK_FIELDS if f not in records.col]
+    if missing:
+        raise ValueError(f"compressed PLY needs the fields {missing}")
+    n, dev = len(records), records.rows.device
+    if order is None:
+        order = morton_order(records.xyz_opacity()[0])
+    else:
+        order = order.to(device=dev, dtype=torch.int32).contiguous()
+        if order.shape != (n,):
+            raise ValueError(f"order must have shape ({n},), got {tuple(order.shape)}")
+        if n:
+            lo, hi = torch.aminmax(order)
+            if int(lo) < 0 or int(hi) >= n:
+                raise ValueError("order holds indices outside [0, N)")
+    rest = [(i, records.col[f"f_rest_{i}"]) for i in range(45) if f"f_rest_{i}" in records.col]
+    cols = [records.col[f] for f in PACK_FIELDS]
+    nchunk = (n + CHUNK - 1) // CHUNK
+    lo6, hi6 = chunk_minmax(records.rows, cols[:6], order, CHUNK)
+    lo3, hi3 = chunk_minmax(records.rows, cols[7:10], order, CHUNK, clip=(-20.0, 20.0))
+    chunk = torch.empty((nchunk, 18), dtype=torch.float32, device=dev)
+    vertex = torch.empty((n, 4), dtype=torch.int32, device=dev)
+    sh = torch.empty((n, len(rest)), dtype=torch.uint8, device=dev)
+    nonzero = torch.empty(1, dtype=torch.int64, device=dev)
+    c14 = (C.c_int32 * 14)(*cols)
+    crest = (C.c_int32 * max(len(rest), 1))(*[c for _, c in rest])
+    check(lib.gsx_cply_pack(_ptr(records.rows), n, records.F, _ptr(order), c14, crest, len(rest), _ptr(lo6), _ptr(hi6),
+                            _ptr(lo3), _ptr(hi3), _ptr(chunk), _ptr(vertex), _ptr(sh), _ptr(nonzero), _stream()),
+          "gsx_cply_pack")
+    mask = 0
+    if n:
+        from .hostcopy import to_host
+        mask = int(to_host(nonzero).view(np.uint64)[0])
+    last = max((i for k, (i, _) in enumerate(rest) if mask >> k & 1), default=-1)
+    limit = sh_keep_limit(last)
+    keep = sum(1 for i, _ in rest if i < limit)
+    if keep == 0:
+        sh = None
+    elif keep < len(rest):
+        narrow = torch.empty((n, keep), dtype=torch.uint8, device=dev)
+        check(lib.gsx_cply_narrow_sh(_ptr(sh), n, len(rest), keep, _ptr(narrow), _stream()), "gsx_cply_narrow_sh")
+        sh = narrow
+    names = tuple(f"f_rest_{i}" for i, _ in rest[:keep])
+    return CompressedPly(chunk, vertex, sh, names, order)
+
+
+_PLY_TYPES = {("f", 4): ("float", "<f4"), ("u", 4): ("uint", "<u4"), ("u", 1): ("uchar", "u1")}
+
+
+def write_ply(path, chunk_data: np.ndarray, vertex_data: np.ndarray, sh_data: np.ndarray | None = None) -> None:
+    """Binary little-endian PLY with the elements chunk, vertex and (if given) sh -- what _write_ply_file writes through
+    plyfile (compressed_ply.py:380-385), for users of gsx without plyfile."""
+    elements = [("chunk", chunk_data), ("vertex", vertex_data)] + ([("sh", sh_data)] if sh_data is not None else [])
+    lines = ["ply", "format binary_little_endian 1.0"]
+    layouts = []
+    for name, a in elements:
+        lines.append(f"element {name} {len(a)}")
+        fields = []
+        for f in a.dtype.names:
+            dt = a.dtype.fields[f][0]
+            if (dt.kind, dt.itemsize) not in _PLY_TYPES:
+                raise ValueError(f"{name}.{f}: unsupported PLY property type {dt}")
+            ply_type, np_type = _PLY_TYPES[(dt.kind, dt.itemsize)]
+            lines.append(f"property {ply_type} {f}")
+            fields.append((f, np_type))
+        layouts.append(np.dtype(fields))
+    lines.append("end_header")
+    with open(path, "wb") as fh:
+        fh.write(("\n".join(lines) + "\n").encode("ascii"))
+        for (_, a), layout in zip(elements, layouts):
+            fh.write(np.ascontiguousarray(a.astype(layout)).tobytes())
+
+
+def dropin_write(self, data: np.ndarray, path, **kwargs) -> None:
+    """Replacement for CompressedPlyFormat.write: packed-float32 records are encoded on the device and written by the
+    class's own _write_ply_file; anything gsx refuses or fails on goes to the original write (the CPU path)."""
+    from .records import DeviceRecords, is_packed_f32
+    try:
+        if not is_packed_f32(data):
+            raise ValueError("compressed PLY on the device needs packed all-float32 records")
+        chunk_data, vertex_data, sh_data = encode(DeviceRecords.from_structured(data)).to_host()
+    except Exception:  # noqa: BLE001  (the reference's convention: exception => CPU path)
+        return self._gsx_reference_write(data, path, **kwargs)
+    self._write_ply_file(path, chunk_data, vertex_data, sh_data)
+
+
+def install(cls) -> None:
+    """Make cls.write the device writer, keeping the original as cls._gsx_reference_write (idempotent)."""
+    if "_gsx_reference_write" not in cls.__dict__:
+        cls._gsx_reference_write = cls.write
+        cls.write = dropin_write

@@ -7,6 +7,9 @@ formats/sog.py:11 import from there):
   * ``gpu_ops.kmeans``, ``gpu_ops.filter_sor_gpu``, ``gpu_ops.HAS_TAICHI``
   * the ``DataProcessor`` class (same public surface; the filters run on libgsx and keep their
     working set in HBM; ``defer=True`` gathers the host records once, when ``.data`` is read)
+and, when ``gsconverter.formats.compressed_ply`` imports, ``CompressedPlyFormat.write`` (Morton order, chunk bounds
+and packing on the device, the file still written by the class's own ``_write_ply_file``; records gsx refuses go to
+the original ``write``).
 Host-only helpers and everything else of the reference stay as they are.
 """
 from __future__ import annotations
@@ -96,6 +99,16 @@ def patch(verbose: bool = False, defer: bool = True, codebook: str = "sklearn", 
             sog = None
     if sog is not None and codebook == "gpu" and hasattr(sog, "MiniBatchKMeans"):
         sog.MiniBatchKMeans = _GsxCodebookKMeans      # sog.py:561 -> exact 1-D Lloyd on the GPU
+    cply = sys.modules.get("gsconverter.formats.compressed_ply")
+    if cply is None:
+        try:
+            cply = importlib.import_module("gsconverter.formats.compressed_ply")
+        except Exception:  # noqa: BLE001  (writer not importable: nothing to patch there)
+            cply = None
+    if cply is not None and hasattr(cply, "CompressedPlyFormat"):
+        from .compressed_ply import install
+        install(cply.CompressedPlyFormat)             # compressed_ply.py:126-250 -> packing on the GPU
     if verbose:
-        print("[gsx] gsconverter.processing patched: SOR / density / bbox / alpha / K-Means run on libgsx.so")
+        print("[gsx] gsconverter.processing patched: SOR / density / bbox / alpha / K-Means / compressed PLY packing "
+              "run on libgsx.so")
     return True

@@ -289,6 +289,25 @@ int gsx_morton_order(const float* xyz_dev, int64_t n, int32_t* order_dev, int32_
 int gsx_chunk_minmax(const float* rows_dev, int64_t n, int32_t F, const int32_t* order_dev, int32_t chunk,
                      const int32_t* cols_host, int32_t ncol, float clip_lo, float clip_hi, float* lo_dev, float* hi_dev,
                      void* ws, int64_t ws_bytes, void* stream);
+/* compressed_ply.py:174-246 (CompressedPlyFormat.write after the Morton sort): the packed chunk, vertex and SH blocks of
+ * the PlayCanvas compressed PLY, one 256-splat chunk per CTA, rows taken in order_dev (gsx_morton_order).
+ *   cols14_host: columns of x y z f_dc_0 f_dc_1 f_dc_2 opacity scale_0 scale_1 scale_2 rot_0 rot_1 rot_2 rot_3;
+ *   rest_cols_host[n_rest] (n_rest <= 45): the columns of the present f_rest_i, i < 45, in ascending i.
+ *   lo/hi_pos_dc_dev [C,6]: gsx_chunk_minmax of x y z f_dc_0..2 over the ordered rows (no clip);
+ *   lo/hi_scale_dev [C,3]: the same of scale_0..2 with clip [-20, 20]  (C = ceil(n/256)).
+ * Outputs: chunk_dev float32[C,18] (min_x..max_z, min/max_scale_x..z, min_r..max_b; colour = f32(f32(f_dc*SH_C0)+0.5)),
+ * vertex_dev uint32[n,4] {packed_position, packed_rotation, packed_scale, packed_color}, sh_dev uint8[n,n_rest]
+ * (may be NULL when n_rest == 0), *rest_nonzero_dev (device uint64, zeroed here) = bit k set iff packed SH column k holds
+ * a value != 0 -- the input of the SH-degree rule of :141-169, which the caller applies (gsx_cply_narrow_sh).
+ * NumPy-2 float32 arithmetic, bit-exact except the alpha byte (expf: one count on ~1e-5 of the splats).  vertex_dev and
+ * sh_dev 16-byte aligned; n < 2^31; n = 0 launches nothing.  (NaN inputs are not supported.) */
+int gsx_cply_pack(const float* rows_dev, int64_t n, int32_t F, const int32_t* order_dev, const int32_t* cols14_host,
+                  const int32_t* rest_cols_host, int32_t n_rest, const float* lo_pos_dc_dev, const float* hi_pos_dc_dev,
+                  const float* lo_scale_dev, const float* hi_scale_dev, float* chunk_dev, uint32_t* vertex_dev,
+                  uint8_t* sh_dev, uint64_t* rest_nonzero_dev, void* stream);
+/* compressed_ply.py:163-169: out_dev[j, :keep] = sh_dev[j, :keep] for the uint8 [n, width] block of gsx_cply_pack, when
+ * the detected SH degree keeps fewer columns than were packed.  0 <= keep <= width <= 45. */
+int gsx_cply_narrow_sh(const uint8_t* sh_dev, int64_t n, int32_t width, int32_t keep, uint8_t* out_dev, void* stream);
 
 /* The SOG shN schedule (formats/sog.py:536-549: up to 64 chunks of one SH block, each clustered by its own
  * gpu_ops.kmeans call) in ONE call on HOST buffers: one upload of the block, one batched launch per phase.
