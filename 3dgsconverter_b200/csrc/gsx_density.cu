@@ -14,6 +14,7 @@
 #include "gsx_density.cuh"
 #include "gsx_sor.cuh"
 
+#include <limits.h>
 #include <math.h>
 #include <stdlib.h>
 #include <vector>
@@ -23,12 +24,16 @@ namespace gsx {
 constexpr int kAxisBits = 21;
 constexpr long long kAxisLim = 1ll << kAxisBits;
 
+// A NaN quotient, or one outside the int64 range, gives INT64_MIN on host and device alike: what the reference's
+// np.floor(...).astype(np.int64) gives on x86.  (The device conversion alone saturates +inf to INT64_MAX, and the
+// host one is undefined there.)
 __host__ __device__ __forceinline__ long long voxel_of(float v, float voxel) {
 #ifdef __CUDA_ARCH__
-    return (long long)floorf(__fdiv_rn(v, voxel));
+    const float f = floorf(__fdiv_rn(v, voxel));
 #else
-    return (long long)floorf(v / voxel);
+    const float f = floorf(v / voxel);
 #endif
+    return fabsf(f) < 9.2233720368547758e18f ? (long long)f : LLONG_MIN;   // -2^63 itself maps to INT64_MIN too
 }
 
 __device__ __forceinline__ uint64_t mix64(uint64_t x) {
@@ -53,6 +58,13 @@ struct VoxGrid {
     long long dim[3];  // extent in voxels
 };
 
+// Whether voxel q lies in the box.  Compares before subtracting, so INT64_MIN - q0 is never formed.  Only rows with a
+// NaN coordinate fall outside the box of the one-shot path (the box is the finite min/max of the cloud).
+__device__ __forceinline__ bool in_box(long long qx, long long qy, long long qz, const VoxGrid& g) {
+    return qx >= g.q0[0] && qx <= g.q0[0] + (g.dim[0] - 1) && qy >= g.q0[1] && qy <= g.q0[1] + (g.dim[1] - 1) &&
+           qz >= g.q0[2] && qz <= g.q0[2] + (g.dim[2] - 1);
+}
+
 int64_t density_workspace_bytes(int64_t n, int64_t cap) {
     if (n < 1) n = 1;
     if (cap < 1) cap = 1;
@@ -71,6 +83,10 @@ __global__ void __launch_bounds__(256) k_vox_count_grid(const float* __restrict_
     if (i >= n) return;
     long long qx = voxel_of(xyz[3 * i], voxel), qy = voxel_of(xyz[3 * i + 1], voxel),
               qz = voxel_of(xyz[3 * i + 2], voxel);
+    if (!in_box(qx, qy, qz, g)) {
+        atomicAdd(counters + 2, 1ull);  // points dropped (non-finite coordinates)
+        return;
+    }
     size_t idx = ((size_t)(qx - g.q0[0]) * g.dim[1] + (size_t)(qy - g.q0[1])) * g.dim[2] + (size_t)(qz - g.q0[2]);
     int old = atomicAdd(grid + idx, 1);
     if (old == 0) atomicAdd(counters + 1, 1ull);  // number of distinct voxels
@@ -101,6 +117,7 @@ __global__ void __launch_bounds__(256) k_vox_count_grid_agg(const float* __restr
     }
     __syncthreads();
     const int64_t base = (int64_t)blockIdx.x * (256 * kAggItems);
+    unsigned long long bad = 0;   // rows dropped (non-finite coordinates)
     auto commit = [&](unsigned int idx, int c) {
         int old = atomicAdd(grid + idx, c);
         if (old == 0) atomicAdd(counters + 1, 1ull);
@@ -121,6 +138,10 @@ __global__ void __launch_bounds__(256) k_vox_count_grid_agg(const float* __restr
         if (i >= n) break;
         long long qx = voxel_of(xyz[3 * i], voxel), qy = voxel_of(xyz[3 * i + 1], voxel),
                   qz = voxel_of(xyz[3 * i + 2], voxel);
+        if (!in_box(qx, qy, qz, g)) {
+            ++bad;
+            continue;
+        }
         const unsigned int idx =
             (unsigned int)(((size_t)(qx - g.q0[0]) * g.dim[1] + (size_t)(qy - g.q0[1])) * g.dim[2] + (size_t)(qz - g.q0[2]));
         unsigned int slot = (idx * 2654435761u) >> 22;  // 10 bits
@@ -136,6 +157,7 @@ __global__ void __launch_bounds__(256) k_vox_count_grid_agg(const float* __restr
         }
         if (!placed) commit(idx, 1);
     }
+    if (bad) atomicAdd(counters + 2, bad);
     __syncthreads();
     for (int t = threadIdx.x; t < kAggSlots; t += 256)
         if (sval[t] > 0) commit(skey[t], sval[t]);
@@ -160,12 +182,12 @@ __global__ void __launch_bounds__(512)
     const bool vec = (reinterpret_cast<uintptr_t>(xyz) & 15) == 0;
     unsigned long long bad = 0;
     auto add = [&](float x, float y, float z) {
-        const long long rx = voxel_of(x, voxel) - g.q0[0], ry = voxel_of(y, voxel) - g.q0[1], rz = voxel_of(z, voxel) - g.q0[2];
-        if (rx < 0 || ry < 0 || rz < 0 || rx >= g.dim[0] || ry >= g.dim[1] || rz >= g.dim[2]) {
+        const long long qx = voxel_of(x, voxel), qy = voxel_of(y, voxel), qz = voxel_of(z, voxel);
+        if (!in_box(qx, qy, qz, g)) {
             ++bad;
             return;
         }
-        atomicAdd(&sh_hist[(int)((rx * g.dim[1] + ry) * g.dim[2] + rz)], 1);
+        atomicAdd(&sh_hist[(int)(((qx - g.q0[0]) * g.dim[1] + (qy - g.q0[1])) * g.dim[2] + (qz - g.q0[2]))], 1);
     };
     for (int64_t t = g0 + threadIdx.x; t < g1; t += blockDim.x) {
         if (vec) {
@@ -243,6 +265,10 @@ __global__ void __launch_bounds__(256) k_vox_count_hash(const float* __restrict_
     if (i >= n) return;
     long long qx = voxel_of(xyz[3 * i], voxel), qy = voxel_of(xyz[3 * i + 1], voxel),
               qz = voxel_of(xyz[3 * i + 2], voxel);
+    if (!in_box(qx, qy, qz, g)) {
+        atomicAdd(counters + 2, 1ull);
+        return;
+    }
     uint64_t key = pack_rel(qx - g.q0[0], qy - g.q0[1], qz - g.q0[2]);
     uint64_t s = mix64(key) & slot_mask;
     for (;;) {
@@ -322,6 +348,10 @@ __global__ void __launch_bounds__(256) k_vox_count_hash_wide(const float* __rest
     if (i >= n) return;
     long long qx = voxel_of(xyz[3 * i], voxel), qy = voxel_of(xyz[3 * i + 1], voxel),
               qz = voxel_of(xyz[3 * i + 2], voxel);
+    if (!in_box(qx, qy, qz, g)) {
+        atomicAdd(counters + 2, 1ull);
+        return;
+    }
     unsigned long long a, b;
     wide_key(qx - g.q0[0], qy - g.q0[1], qz - g.q0[2], a, b);
     uint64_t s = wide_find_or_insert(a, b, ha, hb, slot_mask, true);
@@ -380,9 +410,12 @@ int density_voxel_count(const float* xyz, int64_t n, float voxel, int64_t min_po
     for (int a = 0; a < 3; ++a) {
         g.q0[a] = voxel_of(mm[a], voxel);  // floor(x/voxel) is monotone in x: min/max commute with it
         long long q1 = voxel_of(mm[3 + a], voxel);
+        GSX_REQUIRE(g.q0[a] != LLONG_MIN && q1 != LLONG_MIN, GSX_ERR_UNSUPPORTED,
+                    "density: non-finite or out-of-range coordinates on axis %d", a);
+        // q1 >= q0; the unsigned difference is exact where the signed one could overflow
+        GSX_REQUIRE((unsigned long long)q1 - (unsigned long long)g.q0[a] < (1ull << 31) - 1, GSX_ERR_UNSUPPORTED,
+                    "density: voxel grid extent on axis %d exceeds 2^31 voxels", a);
         g.dim[a] = q1 - g.q0[a] + 1;
-        GSX_REQUIRE(g.dim[a] >= 1 && g.dim[a] < (1ll << 31), GSX_ERR_UNSUPPORTED,
-                    "density: voxel grid extent %lld on axis %d exceeds 2^31 voxels", g.dim[a], a);
         if (g.dim[a] >= kAxisLim) wide = true;  // the packed 3 x 21-bit key does not fit: two-word keys
         cells *= (double)g.dim[a];
     }
@@ -400,7 +433,8 @@ int density_voxel_count(const float* xyz, int64_t n, float voxel, int64_t min_po
         size_t ncell = (size_t)g.dim[0] * g.dim[1] * g.dim[2];
         GSX_CUDA_CHECK(cudaMemsetAsync(blob, 0, ncell * 4, st));
         if (ncell <= (size_t)kSmemCells) {
-            int rc2 = launch_vox_count_smem(xyz, n, voxel, g, ncell, thr, (int*)blob, counters, dvox, cap, nullptr, st);
+            int rc2 = launch_vox_count_smem(xyz, n, voxel, g, ncell, thr, (int*)blob, counters, dvox, cap, counters + 2,
+                                            st);
             if (rc2) return rc2;
         } else if (ncell < 0xfffffff0ull) {
             int ablocks = (int)((n + 256 * kAggItems - 1) / (256 * kAggItems));
@@ -429,11 +463,15 @@ int density_voxel_count(const float* xyz, int64_t n, float voxel, int64_t min_po
         }
     }
     GSX_KERNEL_CHECK();
-    unsigned long long hc[2];
+    unsigned long long hc[3];   // dense voxels, distinct voxels, points outside the box
     GSX_CUDA_CHECK(cudaMemcpyAsync(hc, counters, sizeof(hc), cudaMemcpyDeviceToHost, st));
     GSX_CUDA_CHECK(cudaStreamSynchronize(st));
     *n_dense_host = (int64_t)hc[0];
     if (n_voxels_host) *n_voxels_host = (int64_t)hc[1];
+    // The reference puts a NaN row in a voxel outside the finite box.  Fewer than thr such rows make no dense voxel,
+    // so dropping them is exact; with thr or more, one of those voxels may be dense, and that is refused.
+    GSX_REQUIRE(hc[2] < (unsigned long long)thr, GSX_ERR_UNSUPPORTED,
+                "density: %llu points have non-finite (NaN) coordinates, at least min_points = %d", hc[2], thr);
     GSX_REQUIRE((int64_t)hc[0] <= cap, GSX_ERR_WORKSPACE, "density: %llu dense voxels exceed cap %lld", hc[0],
                 (long long)cap);
     int64_t nd = (int64_t)hc[0];
@@ -458,13 +496,13 @@ __global__ void __launch_bounds__(256) k_vox_count_grid_only(const float* __rest
                                                              unsigned long long* __restrict__ oob) {
     int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    long long rx = voxel_of(xyz[3 * i], voxel) - g.q0[0], ry = voxel_of(xyz[3 * i + 1], voxel) - g.q0[1],
-              rz = voxel_of(xyz[3 * i + 2], voxel) - g.q0[2];
-    if (rx < 0 || ry < 0 || rz < 0 || rx >= g.dim[0] || ry >= g.dim[1] || rz >= g.dim[2]) {
+    const long long qx = voxel_of(xyz[3 * i], voxel), qy = voxel_of(xyz[3 * i + 1], voxel),
+                    qz = voxel_of(xyz[3 * i + 2], voxel);
+    if (!in_box(qx, qy, qz, g)) {
         atomicAdd(oob, 1ull);
         return;
     }
-    atomicAdd(grid + ((size_t)rx * g.dim[1] + (size_t)ry) * g.dim[2] + (size_t)rz, 1);
+    atomicAdd(grid + ((size_t)(qx - g.q0[0]) * g.dim[1] + (size_t)(qy - g.q0[1])) * g.dim[2] + (size_t)(qz - g.q0[2]), 1);
 }
 
 __global__ void __launch_bounds__(256) k_vox_grid_dense(const int* __restrict__ grid, size_t ncell, VoxGrid g, int thr,

@@ -466,6 +466,12 @@ def density_filter_sharded(xyz_local: torch.Tensor, voxel_size=1.0, threshold_pe
         ops.grid_count(xyz_local, voxel_size, q0, dim, grid)
     dist.all_reduce(grid, op=dist.ReduceOp.SUM, group=group)
     min_points = int(n_total * (threshold_percentage / 100.0))  # data_processor.py:48 on the global count
+    # rows the grid did not count lie outside the global box: those with a NaN coordinate
+    n_oob = n_total - int(grid.sum(dtype=torch.int64).item())
+    if n_oob >= max(min_points, 1):   # the same refusal as gsx_density_voxel_count on the union cloud
+        from ._abi import GsxError
+        raise GsxError(f"density: {n_oob} points have non-finite (NaN) coordinates, at least "
+                       f"min_points = {max(min_points, 1)}")
     vox, cnt, n_unique = ops.grid_dense(grid, q0, dim, min_points, n_total)
     if len(vox) == 0:
         return torch.zeros(n_here, dtype=torch.bool, device=dev), dict(empty_info, voxels=n_unique)

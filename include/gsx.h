@@ -187,7 +187,9 @@ int64_t gsx_density_workspace_bytes(int64_t n, int64_t cap);
 /* q = floor(xyz / f32(voxel)) -> int64 triple (data_processor.py:39); counts per voxel (:43); every voxel
  * with count >= max(min_points,1) (:48-51) is returned to the HOST arrays dense_vox_host (int64[cap,3]) and
  * dense_cnt_host (int32[cap]), in no particular order; *n_dense_host = how many (> cap => GSX_ERR_WORKSPACE);
- * *n_voxels_host (may be NULL) = number of distinct voxels (len(unique_voxels), :45). */
+ * *n_voxels_host (may be NULL) = number of distinct voxels (len(unique_voxels), :45) inside the finite bounding
+ * box.  Rows with a NaN coordinate fall outside that box and are not counted; when max(min_points,1) or more such
+ * rows exist one of their voxels could be dense, and the call returns GSX_ERR_UNSUPPORTED. */
 int gsx_density_voxel_count(const float* xyz_dev, int64_t n, float voxel, int64_t min_points, int64_t* dense_vox_host,
                             int32_t* dense_cnt_host, int64_t cap, int64_t* n_dense_host, int64_t* n_voxels_host,
                             void* ws, int64_t ws_bytes, void* stream);
@@ -199,7 +201,9 @@ int gsx_density_member_mask(const float* xyz_dev, int64_t n, float voxel, const 
 /* Staged form for sharded clouds (one process per GPU): every rank counts its slab into an int32 grid over
  * the GLOBAL voxel box (q0[3], dim[3] voxels; from the all-reduced min/max via gsx_density_voxel_range), the
  * caller all-reduces the grid (sum) and extracts the dense voxels from it.  Same results as
- * gsx_density_voxel_count on the union cloud.  *oob_dev counts points outside the box (must stay 0). */
+ * gsx_density_voxel_count on the union cloud.  *oob_dev accumulates the points outside the box; over the global
+ * box these are the rows with a NaN coordinate, and a caller refuses when there are >= max(min_points,1) of them
+ * in the union cloud (gsx/dist.py: N minus the sum of the all-reduced grid). */
 void gsx_density_voxel_range(const float* minmax_host /*[6]*/, float voxel, int64_t* q0_out, int64_t* dim_out);
 int gsx_density_grid_count(const float* xyz_dev, int64_t n, float voxel, const int64_t* q0, const int64_t* dim,
                            int32_t* grid_dev, unsigned long long* oob_dev, void* stream);

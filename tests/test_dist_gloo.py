@@ -164,23 +164,31 @@ def test_query_range_partition():
             assert all(edges[i][1] == edges[i + 1][0] for i in range(w - 1))
 
 
+def _voxels(a, voxel):
+    """floor(a / f32(voxel)) as int64; NaN gives INT64_MIN, as on x86 and in the device kernels."""
+    with np.errstate(invalid="ignore"):
+        return np.floor(np.asarray(a, np.float32) / np.float32(voxel)).astype(np.int64)
+
+
 class OracleDensityOps:
     """NumPy stand-in for the CUDA density ops (collective logic under test, CPU/gloo)."""
 
     def minmax(self, xyz):
+        """Like the device min/max (fminf/fmaxf), NaN rows are left out of the box."""
         if xyz.shape[0] == 0:
             return torch.tensor([float("inf")] * 3 + [float("-inf")] * 3, dtype=torch.float32)
-        return torch.cat([xyz.min(dim=0).values, xyz.max(dim=0).values])
+        a = xyz.numpy()
+        return torch.from_numpy(np.r_[np.fmin.reduce(a, axis=0), np.fmax.reduce(a, axis=0)].astype(np.float32))
 
     def voxel_range(self, mm, voxel):
-        v = np.float32(voxel)
-        q0 = np.floor(mm[:3].astype(np.float32) / v).astype(np.int64)
-        q1 = np.floor(mm[3:].astype(np.float32) / v).astype(np.int64)
+        q0, q1 = _voxels(mm[:3], voxel), _voxels(mm[3:], voxel)
         return q0, q1 - q0 + 1
 
     def grid_count(self, xyz, voxel, q0, dim, grid):
-        q = np.floor(xyz.numpy() / np.float32(voxel)).astype(np.int64) - q0
-        flat = (q[:, 0] * dim[1] + q[:, 1]) * dim[2] + q[:, 2]
+        q = _voxels(xyz.numpy(), voxel)
+        inb = np.all((q >= q0) & (q <= q0 + dim - 1), axis=1)
+        r = q[inb] - q0
+        flat = (r[:, 0] * dim[1] + r[:, 1]) * dim[2] + r[:, 2]
         grid += torch.from_numpy(np.bincount(flat, minlength=grid.numel()).astype(np.int32))
 
     def grid_dense(self, grid, q0, dim, min_points, n_total):
@@ -189,7 +197,7 @@ class OracleDensityOps:
         return idx + q0, g[tuple(idx.T)], int((g > 0).sum())
 
     def member_mask(self, xyz, voxel, keep):
-        q = np.floor(xyz.numpy() / np.float32(voxel)).astype(np.int64)
+        q = _voxels(xyz.numpy(), voxel)
         ks = set(map(tuple, keep))
         return torch.from_numpy(np.array([tuple(v) in ks for v in q]))
 
@@ -238,6 +246,69 @@ def test_density_sharded_equals_single(sizes):
         got = np.concatenate([res[r][key][0] for r in range(world)])
         assert np.array_equal(got, want), key
         assert all(res[r][key][1]["clusters"] == info["clusters"] for r in range(world))
+
+
+def _nan_cloud(n, nan_rows):
+    """The mixed cloud with NaN in x (every third row also in y and z) at `nan_rows` rows spread over the cloud."""
+    from gsx import synth
+    xyz = synth.xyz(n, "mixed").copy()
+    rows = np.linspace(0, n - 1, nan_rows).astype(np.int64)
+    xyz[rows, 0] = np.nan
+    xyz[rows[::3], 1:] = np.nan
+    return xyz
+
+
+def _density_nan_worker(rank, world, port, sizes, nan_rows, q):
+    sys.path.insert(0, str(ROOT)); sys.path.insert(0, str(ROOT / "3dgsconverter_b200"))
+    os.environ["MASTER_ADDR"] = "127.0.0.1"
+    os.environ["MASTER_PORT"] = str(port)
+    dist.init_process_group("gloo", rank=rank, world_size=world)
+    from gsx import dist as gd
+    from gsx._abi import GsxError
+    off = sum(sizes[:rank])
+    out = {}
+    for k in nan_rows:
+        local = torch.from_numpy(_nan_cloud(sum(sizes), k)[off:off + sizes[rank]].copy())
+        try:
+            mask, info = gd.density_filter_sharded(local, sensitivity=0.5, keep_multicluster=True,
+                                                   ops=OracleDensityOps())
+            out[k] = (mask.numpy(), info["clusters"])
+        except GsxError as e:
+            out[k] = str(e)
+    q.put((rank, out))
+    dist.barrier()
+    dist.destroy_process_group()
+
+
+def test_density_sharded_nan_rows():
+    """Rows with a NaN coordinate fall outside the global box.  Below min_points of them (275 here) the mask equals
+    the oracle's, which puts them in a voxel of their own; at 400, split 200 / 200 so that no single slab reaches
+    min_points, every rank refuses."""
+    import oracle
+    sizes, world = (30_000, 20_000), 2
+    ctx = mp.get_context("spawn")
+    q = ctx.Queue()
+    port = 33500 + (os.getpid() % 2000)
+    procs = [ctx.Process(target=_density_nan_worker, args=(r, world, port, sizes, (100, 400), q)) for r in range(world)]
+    for p in procs:
+        p.start()
+    res = {}
+    for _ in range(world):
+        r, out = q.get(timeout=300)
+        res[r] = out
+    for p in procs:
+        p.join(60)
+        assert p.exitcode == 0
+    xyz = _nan_cloud(sum(sizes), 100)
+    with np.errstate(invalid="ignore"):
+        want, info = oracle.density_mask(xyz, sensitivity=0.5, keep_multicluster=True)
+    assert np.array_equal(np.concatenate([res[r][100][0] for r in range(world)]), want)
+    assert all(res[r][100][1] == info["clusters"] for r in range(world))
+    assert not want[np.isnan(xyz).any(axis=1)].any()
+    nan_rows = np.isnan(_nan_cloud(sum(sizes), 400)).any(axis=1)
+    assert nan_rows[:30_000].sum() < 275 and nan_rows[30_000:].sum() < 275
+    for r in range(world):
+        assert isinstance(res[r][400], str) and "non-finite" in res[r][400]
 
 
 class OracleBuildOps:
