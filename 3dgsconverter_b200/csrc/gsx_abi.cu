@@ -442,6 +442,53 @@ int gsx_quantize_to_codebook(const float* vals_dev, int64_t n, const float* code
     return quantize_to_codebook(vals_dev, n, codebook_host, m, labels_dev, ws, ws_bytes, (cudaStream_t)stream);
 }
 
+int gsx_sog_means_minmax(const float* rows_dev, int64_t n, int32_t F, const int32_t* cols3_host, float* ws_dev,
+                         int64_t ws_bytes, float* minmax_dev, void* stream) {
+    return sog_means_minmax(rows_dev, n, F, cols3_host, ws_dev, ws_bytes, minmax_dev, (cudaStream_t)stream);
+}
+
+int gsx_sog_means(const float* rows_dev, int64_t n, int32_t F, const int32_t* order_dev, const int32_t* cols3_host,
+                  const float* minmax_dev, int64_t pixels, uint8_t* means_l_dev, uint8_t* means_u_dev, void* stream) {
+    return sog_means(rows_dev, n, F, order_dev, cols3_host, minmax_dev, pixels, means_l_dev, means_u_dev,
+                     (cudaStream_t)stream);
+}
+
+int gsx_sog_quats(const float* rows_dev, int64_t n, int32_t F, const int32_t* order_dev, const int32_t* cols4_host,
+                  int64_t pixels, uint8_t* quats_dev, void* stream) {
+    return sog_quats(rows_dev, n, F, order_dev, cols4_host, pixels, quats_dev, (cudaStream_t)stream);
+}
+
+int gsx_sog_gather_values(const float* rows_dev, int64_t n, int32_t F, const int32_t* order_dev,
+                          const int32_t* cols_host, int32_t ncols, const int64_t* sel_dev, int64_t m, float* out_dev,
+                          void* stream) {
+    return sog_gather_values(rows_dev, n, F, order_dev, cols_host, ncols, sel_dev, m, out_dev, (cudaStream_t)stream);
+}
+
+int gsx_sog_scales_sh0(const float* rows_dev, int64_t n, int32_t F, const int32_t* order_dev,
+                       const int32_t* cols7_host, const float* scale_cb_dev, int32_t m_scale,
+                       const float* color_cb_dev, int32_t m_color, int64_t pixels, uint8_t* scales_dev,
+                       uint8_t* sh0_dev, void* stream) {
+    return sog_scales_sh0(rows_dev, n, F, order_dev, cols7_host, scale_cb_dev, m_scale, color_cb_dev, m_color, pixels,
+                          scales_dev, sh0_dev, (cudaStream_t)stream);
+}
+
+int gsx_sog_sh_gather(const float* rows_dev, int64_t n, int32_t F, const int32_t* order_dev, const int32_t* cols_host,
+                      int32_t ncols, float* out_dev, unsigned long long* nonzero_dev, void* stream) {
+    return sog_sh_gather(rows_dev, n, F, order_dev, cols_host, ncols, out_dev, nonzero_dev, (cudaStream_t)stream);
+}
+
+int gsx_sog_labels(const int32_t* labels_dev, int64_t n, int64_t chunk_size, int32_t nchunks,
+                   const int32_t* offsets_host, const int32_t* passthrough_host, int64_t pixels, uint8_t* out_dev,
+                   void* stream) {
+    return sog_labels(labels_dev, n, chunk_size, nchunks, offsets_host, passthrough_host, pixels, out_dev,
+                      (cudaStream_t)stream);
+}
+
+int gsx_sog_centroids(const float* palette_dev, int64_t P, int32_t coeffs, const float* cb_dev, int32_t m,
+                      int64_t pixels, uint8_t* out_dev, void* stream) {
+    return sog_centroids(palette_dev, P, coeffs, cb_dev, m, pixels, out_dev, (cudaStream_t)stream);
+}
+
 /* ------------------------------------------------------------------ K-Means */
 
 int64_t gsx_kmeans_workspace_bytes(int64_t n_total, int32_t nprob, int32_t K, int32_t D) {

@@ -13,6 +13,7 @@
 // every step is one __f*_rn operation in the reference's order, with no contraction.  The alpha channel goes through
 // expf and can differ from NumPy's SIMD exp by one count on ~1e-5 of the splats; everything else is bit-exact.
 #include "gsx_common.cuh"
+#include "gsx_sh_mask.cuh"
 #include "gsx_compressed_ply.cuh"
 
 namespace gsx {
@@ -141,9 +142,7 @@ __global__ void __launch_bounds__(kChunk) k_cply_pack(const float* __restrict__ 
                 mine[k] = sh_byte(v);
             }
     }
-    const uint32_t lo = __reduce_or_sync(0xffffffffu, (uint32_t)nz);
-    const uint32_t hi = __reduce_or_sync(0xffffffffu, (uint32_t)(nz >> 32));
-    if ((t & 31) == 0 && (lo | hi)) atomicOr(nonzero, (unsigned long long)hi << 32 | lo);
+    warp_or_column_mask(nz, nonzero);
     if (n_rest == 0) return;
     __syncthreads();
     // the chunk's SH bytes are one contiguous run of rows_here * n_rest bytes; chunk starts are 256 * n_rest apart, so

@@ -76,6 +76,15 @@ _SIGS = {
     "gsx_lexsort_workspace_bytes": (_i64, [_i64]),
     "gsx_lexsort_zyx": (C.c_int, [_vp, _i64, _vp, _vp, _i64, _vp]),
     "gsx_quantize_to_codebook": (C.c_int, [_vp, _i64, _f32p, _i32, _vp, _vp, _i64, _vp]),
+    "gsx_sog_means_minmax": (C.c_int, [_vp, _i64, _i32, C.POINTER(_i32), _vp, _i64, _vp, _vp]),
+    "gsx_sog_means": (C.c_int, [_vp, _i64, _i32, _vp, C.POINTER(_i32), _vp, _i64, _vp, _vp, _vp]),
+    "gsx_sog_quats": (C.c_int, [_vp, _i64, _i32, _vp, C.POINTER(_i32), _i64, _vp, _vp]),
+    "gsx_sog_gather_values": (C.c_int, [_vp, _i64, _i32, _vp, C.POINTER(_i32), _i32, _vp, _i64, _vp, _vp]),
+    "gsx_sog_scales_sh0": (C.c_int, [_vp, _i64, _i32, _vp, C.POINTER(_i32), _vp, _i32, _vp, _i32, _i64, _vp, _vp,
+                                     _vp]),
+    "gsx_sog_sh_gather": (C.c_int, [_vp, _i64, _i32, _vp, C.POINTER(_i32), _i32, _vp, _vp, _vp]),
+    "gsx_sog_labels": (C.c_int, [_vp, _i64, _i64, _i32, C.POINTER(_i32), C.POINTER(_i32), _i64, _vp, _vp]),
+    "gsx_sog_centroids": (C.c_int, [_vp, _i64, _i32, _vp, _i32, _i64, _vp, _vp]),
     "gsx_kmeans_workspace_bytes": (_i64, [_i64, _i32, _i32, _i32]),
     "gsx_kmeans_lloyd_device": (C.c_int, [_vp, C.POINTER(_i64), _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _i64,
                                           _i32, _vp, _vp]),

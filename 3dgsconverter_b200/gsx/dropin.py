@@ -9,7 +9,9 @@ formats/sog.py:11 import from there):
     working set in HBM; ``defer=True`` gathers the host records once, when ``.data`` is read)
 and, when ``gsconverter.formats.compressed_ply`` imports, ``CompressedPlyFormat.write`` (Morton order, chunk bounds
 and packing on the device, the file still written by the class's own ``_write_ply_file``; records gsx refuses go to
-the original ``write``).
+the original ``write``).  With ``patch(sog="device")`` also ``SogFormat.write`` (gsx.sog.encode: every texture,
+codebook and the chunked SH palette built on the device; opt-in because its position bytes can differ from NumPy's
+log by one count on a small fraction of the splats).
 Host-only helpers and everything else of the reference stay as they are.
 """
 from __future__ import annotations
@@ -49,9 +51,14 @@ class _GsxCodebookKMeans:
         return self
 
 
-def patch(verbose: bool = False, defer: bool = True, codebook: str = "sklearn", require_cuda: bool = True):
+def patch(verbose: bool = False, defer: bool = True, codebook: str = "sklearn", require_cuda: bool = True,
+          sog: str = "host"):
     """require_cuda: refuse (return False, leave the reference untouched) when no CUDA device is usable, so that a
-    CPU-only host keeps the reference's own SciPy / scikit-learn paths (there is no CPU fallback inside gsx)."""
+    CPU-only host keeps the reference's own SciPy / scikit-learn paths (there is no CPU fallback inside gsx).
+    sog: "host" keeps the reference's SogFormat.write (with the patched gpu_ops.kmeans and its batch-ahead);
+    "device" replaces it with gsx.sog's device encoder (records gsx refuses go to the original write)."""
+    if sog not in ("host", "device"):
+        raise ValueError(f"sog must be 'host' or 'device', not {sog!r}")
     if require_cuda:
         from . import backend_available
         if not backend_available():
@@ -91,14 +98,17 @@ def patch(verbose: bool = False, defer: bool = True, codebook: str = "sklearn", 
     if conv is not None and hasattr(conv, "DataProcessor"):
         conv.DataProcessor = Ours
     ref_gpu_ops._gsx_module = g     # batch-ahead statistics: gpu_ops._gsx_module.batch_stats
-    sog = sys.modules.get("gsconverter.formats.sog")
-    if sog is None:
+    sog_mod = sys.modules.get("gsconverter.formats.sog")
+    if sog_mod is None:
         try:
-            sog = importlib.import_module("gsconverter.formats.sog")
+            sog_mod = importlib.import_module("gsconverter.formats.sog")
         except Exception:  # noqa: BLE001  (optional dependency of the writer missing: nothing to patch there)
-            sog = None
-    if sog is not None and codebook == "gpu" and hasattr(sog, "MiniBatchKMeans"):
-        sog.MiniBatchKMeans = _GsxCodebookKMeans      # sog.py:561 -> exact 1-D Lloyd on the GPU
+            sog_mod = None
+    if sog_mod is not None and codebook == "gpu" and hasattr(sog_mod, "MiniBatchKMeans"):
+        sog_mod.MiniBatchKMeans = _GsxCodebookKMeans  # sog.py:561 -> exact 1-D Lloyd on the GPU
+    if sog_mod is not None and sog == "device" and hasattr(sog_mod, "SogFormat"):
+        from .sog import install as install_sog
+        install_sog(sog_mod.SogFormat)                # sog.py:249-639 -> textures and palette on the GPU
     cply = sys.modules.get("gsconverter.formats.compressed_ply")
     if cply is None:
         try:

@@ -221,6 +221,51 @@ int gsx_lexsort_zyx(const float* xyz_dev, int64_t n, int32_t* order_dev, void* w
 int gsx_quantize_to_codebook(const float* vals_dev, int64_t n, const float* codebook_host, int32_t m,
                              uint8_t* labels_dev, void* ws, int64_t ws_bytes, void* stream);
 
+/* ---- SOG writer on the device: SogFormat.write, formats/sog.py:258-602 (gsx/sog.py) ---------------- */
+/* Record rows are float32 [n, F]; every kernel reads row order_dev[j] for the j-th splat of the file (the lexsort
+ * order).  Textures are uchar4 [pixels] (pixels >= n, 4-byte aligned); the padding pixels are written too.  Float
+ * steps follow NumPy-2 float32 order; float -> u8/u16 conversions map NaN to 0.  n < 2^31.
+ * The position logarithm and the opacity exponential are not NumPy's SIMD functions: a means u16 or the sh0 alpha
+ * byte can differ by one count on a small fraction of the splats; everything else is bit-exact. */
+/* sog.py:279-287: minmax_dev[6] = min x, y, z, max x, y, z of sign(v) * log(|v| + 1), NaN-propagating as
+ * np.min / np.max.  cols3_host = columns of x, y, z; ws_dev >= 24576 B; n >= 1. */
+int gsx_sog_means_minmax(const float* rows_dev, int64_t n, int32_t F, const int32_t* cols3_host, float* ws_dev,
+                         int64_t ws_bytes, float* minmax_dev, void* stream);
+/* sog.py:289-309: means_l / means_u, the low and high bytes of clip((l - min) / (max - min) * 65535) as u16 (0/0 of a
+ * degenerate axis -> 0), alpha 255; padding 255. */
+int gsx_sog_means(const float* rows_dev, int64_t n, int32_t F, const int32_t* order_dev, const int32_t* cols3_host,
+                  const float* minmax_dev, int64_t pixels, uint8_t* means_l_dev, uint8_t* means_u_dev, void* stream);
+/* sog.py:315-386: quats (cols4_host = rot_0..3): the three non-largest components of the normalised, sign-fixed,
+ * sqrt(2)-scaled quaternion through quantize_vec, alpha = 252 + argmax |q|; padding 255. */
+int gsx_sog_quats(const float* rows_dev, int64_t n, int32_t F, const int32_t* order_dev, const int32_t* cols4_host,
+                  int64_t pixels, uint8_t* quats_dev, void* stream);
+/* sog.py:392-400, 435-441: out_dev[t] = v[s] of v = np.concatenate([col_0, .., col_ncols-1]) in file order, with
+ * s = sel_dev[t] (int64) or t when sel_dev is NULL -- the fit data of a 1-D codebook and its K-Means init rows. */
+int gsx_sog_gather_values(const float* rows_dev, int64_t n, int32_t F, const int32_t* order_dev,
+                          const int32_t* cols_host, int32_t ncols, const int64_t* sel_dev, int64_t m, float* out_dev,
+                          void* stream);
+/* sog.py:421-459: scales (scale_0..2 against scale_cb, alpha 255) and sh0 (f_dc_0..2 against color_cb, alpha
+ * clip(sigmoid(opacity) * 255)) in one pass; cols7_host = scale_0..2, f_dc_0..2, opacity; codebooks ascending,
+ * 1..256 entries, on the device; padding 0. */
+int gsx_sog_scales_sh0(const float* rows_dev, int64_t n, int32_t F, const int32_t* order_dev,
+                       const int32_t* cols7_host, const float* scale_cb_dev, int32_t m_scale,
+                       const float* color_cb_dev, int32_t m_color, int64_t pixels, uint8_t* scales_dev,
+                       uint8_t* sh0_dev, void* stream);
+/* sog.py:483-503: out_dev[j, k] = column cols_host[k] of the j-th splat (float32 [n, ncols], 1 <= ncols <= 45) and
+ * *nonzero_dev bit k = some value of that column != 0 (the band detection; -0.0 counts as zero). */
+int gsx_sog_sh_gather(const float* rows_dev, int64_t n, int32_t F, const int32_t* order_dev, const int32_t* cols_host,
+                      int32_t ncols, float* out_dev, unsigned long long* nonzero_dev, void* stream);
+/* sog.py:546-600: shN_labels.  Row j is in chunk c = j / chunk_size (nchunks <= 64); its label is labels_dev[j]
+ * (chunk-local, as gsx_kmeans_lloyd_device returns it) or j - c * chunk_size where passthrough_host[c] != 0;
+ * pixel = (label + offsets_host[c]) as u16 -> (lo, hi, 0, 255); padding 0. */
+int gsx_sog_labels(const int32_t* labels_dev, int64_t n, int64_t chunk_size, int32_t nchunks,
+                   const int32_t* offsets_host, const int32_t* passthrough_host, int64_t pixels, uint8_t* out_dev,
+                   void* stream);
+/* sog.py:566-588: shN_centroids.  The palette float32 [P, coeffs] (coeffs in {9, 24, 45}) against the ascending
+ * codebook cb_dev (1..256 entries), laid out as (P, coeffs / 3, 3) RGB pixels, alpha 255; padding 255. */
+int gsx_sog_centroids(const float* palette_dev, int64_t P, int32_t coeffs, const float* cb_dev, int32_t m,
+                      int64_t pixels, uint8_t* out_dev, void* stream);
+
 /* ---- K-Means: gpu_ops.py:57-96 (kernels) + :186-188 (Lloyd loop) ---------------------- */
 /* Batched over `nprob` independent problems stored back to back (SOG shN chunks, sog.py:527-549):
  * problem p has rows [row_off[p], row_off[p+1]) of X[*,D] and K centroids at C[p*K*D].
