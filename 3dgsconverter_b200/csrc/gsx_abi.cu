@@ -610,7 +610,7 @@ int64_t gsx_morton_workspace_bytes(int64_t n) { return morton_workspace_bytes(n)
 int gsx_morton_order(const float* xyz_dev, int64_t n, int32_t* order_dev, int32_t run_limit, int32_t* levels_out, void* ws,
                      int64_t ws_bytes, void* stream) {
     int lv = 0;
-    int rc = morton_order(xyz_dev, n, order_dev, run_limit, 16, &lv, ws, ws_bytes, (cudaStream_t)stream);
+    int rc = morton_order(xyz_dev, n, order_dev, run_limit, &lv, ws, ws_bytes, (cudaStream_t)stream);
     if (levels_out) *levels_out = lv;
     return rc;
 }

@@ -36,8 +36,14 @@ struct CplyCols {
     int32_t n_rest;
 };
 
-// np.clip(np.floor(x), 0, t).astype(np.uint32)
-__device__ __forceinline__ uint32_t floor_clip(float x, float t) { return (uint32_t)fminf(fmaxf(floorf(x), 0.f), t); }
+// np.clip(np.floor(x), 0, t).astype(np.uint32); NumPy keeps the NaN through the clip and its x86 cast loop converts
+// it to 0x80000000 (cvttps2dq), which the reference ORs into the packed word (DESIGN §4.5)
+__device__ __forceinline__ uint32_t floor_clip(float x, float t) {
+    return x != x ? 0x80000000u : (uint32_t)fminf(fmaxf(floorf(x), 0.f), t);
+}
+
+// np.clip(s, -20, 20), which keeps NaN
+__device__ __forceinline__ float clip20(float s) { return s != s ? s : fminf(fmaxf(s, -20.f), 20.f); }
 
 // normalize() of _normalize_and_pack_11_10_11 / _8888 (:300-304, :311-314)
 __device__ __forceinline__ uint32_t unorm(float v, float mn, float mx, float t) {
@@ -47,8 +53,11 @@ __device__ __forceinline__ uint32_t unorm(float v, float mn, float mx, float t) 
     return floor_clip(__fadd_rn(__fmul_rn(nv, t), 0.5f), t);
 }
 
-// f_dc * SH_C0 + 0.5 (:196-198); monotone in f_dc, so it maps the f_dc bounds onto the colour bounds
-__device__ __forceinline__ float dc_color(float f) { return __fadd_rn(__fmul_rn(f, kShC0), 0.5f); }
+// f_dc * SH_C0 + 0.5 (:196-198); monotone in f_dc, so it maps the f_dc bounds onto the colour bounds.  A NaN comes
+// out as x86 float arithmetic returns it (the operand, quieted), so a NaN colour bound keeps the f_dc NaN's bits.
+__device__ __forceinline__ float dc_color(float f) {
+    return f != f ? __uint_as_float(__float_as_uint(f) | 0x00400000u) : __fadd_rn(__fmul_rn(f, kShC0), 0.5f);
+}
 
 // pack_unorm(q * sign, 10) of _pack_quaternions (:331-333)
 __device__ __forceinline__ uint32_t quat_comp(float q, float s) {
@@ -57,7 +66,8 @@ __device__ __forceinline__ uint32_t quat_comp(float q, float s) {
 }
 
 // _pack_quaternions (:321-340): serial sum of squares (np.linalg.norm over 4 components), q /= norm + 1e-10, largest =
-// first index of max |q|, q *= sign(q[largest]) (sign(0) = 0), the other three in ascending order below 2 bits of index
+// first index of max |q| (np.argmax: the first NaN is the maximum), q *= sign(q[largest]) (sign(0) = 0, sign(NaN) =
+// NaN), the other three in ascending order below 2 bits of index
 __device__ __forceinline__ uint32_t pack_quat(float q0, float q1, float q2, float q3) {
     float ss = __fmul_rn(q0, q0);
     ss = __fadd_rn(ss, __fmul_rn(q1, q1));
@@ -67,10 +77,10 @@ __device__ __forceinline__ uint32_t pack_quat(float q0, float q1, float q2, floa
     q0 = __fdiv_rn(q0, d), q1 = __fdiv_rn(q1, d), q2 = __fdiv_rn(q2, d), q3 = __fdiv_rn(q3, d);
     uint32_t L = 0;
     float best = fabsf(q0), qL = q0;
-    if (fabsf(q1) > best) best = fabsf(q1), qL = q1, L = 1;
-    if (fabsf(q2) > best) best = fabsf(q2), qL = q2, L = 2;
-    if (fabsf(q3) > best) best = fabsf(q3), qL = q3, L = 3;
-    const float s = qL > 0.f ? 1.f : (qL < 0.f ? -1.f : 0.f);
+    if (best == best && (fabsf(q1) > best || q1 != q1)) best = fabsf(q1), qL = q1, L = 1;
+    if (best == best && (fabsf(q2) > best || q2 != q2)) best = fabsf(q2), qL = q2, L = 2;
+    if (best == best && (fabsf(q3) > best || q3 != q3)) best = fabsf(q3), qL = q3, L = 3;
+    const float s = qL > 0.f ? 1.f : (qL < 0.f ? -1.f : (qL == 0.f ? 0.f : qL));
     uint32_t r = L;
     if (L != 0) r = (r << 10) | quat_comp(q0, s);
     if (L != 1) r = (r << 10) | quat_comp(q1, s);
@@ -120,9 +130,9 @@ __global__ void __launch_bounds__(kChunk) k_cply_pack(const float* __restrict__ 
         const uint32_t pos = unorm(__ldg(r + cols.c[0]), sb[0], sb[3], 2047.f) << 21 |
                              unorm(__ldg(r + cols.c[1]), sb[1], sb[4], 1023.f) << 11 |
                              unorm(__ldg(r + cols.c[2]), sb[2], sb[5], 2047.f);
-        const float s0 = fminf(fmaxf(__ldg(r + cols.c[7]), -20.f), 20.f);
-        const float s1 = fminf(fmaxf(__ldg(r + cols.c[8]), -20.f), 20.f);
-        const float s2 = fminf(fmaxf(__ldg(r + cols.c[9]), -20.f), 20.f);
+        const float s0 = clip20(__ldg(r + cols.c[7]));
+        const float s1 = clip20(__ldg(r + cols.c[8]));
+        const float s2 = clip20(__ldg(r + cols.c[9]));
         const uint32_t scl = unorm(s0, sb[6], sb[9], 2047.f) << 21 | unorm(s1, sb[7], sb[10], 1023.f) << 11 |
                              unorm(s2, sb[8], sb[11], 2047.f);
         const float a = __fdiv_rn(1.f, __fadd_rn(1.f, expf(-__ldg(r + cols.c[6]))));

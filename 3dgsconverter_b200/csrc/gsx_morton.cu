@@ -8,6 +8,10 @@
 //                      sorted by our stable radix sort, and the next level's runs found by a flag/scan pass.
 //                      The reference uses np.argsort's default (unstable) kind: the order of equal codes inside a
 //                      finished run is unspecified there; we return the stable one (lowest original index first).
+//                      The levels run until no run is left.  A NaN position makes its run's box NaN on that axis, as
+//                      cx.min() does, and every code of the run is 0 on that axis.  A picked run that comes back as one
+//                      run (every axis has zero, infinite or NaN extent, and not all zero) is refused: the reference
+//                      recurses into the same rows for ever there (RecursionError).
 //   gsx_chunk_minmax   compressed_ply.py:206-246 (per-256-splat chunk min/max) and ksplat.py:426-441
 //                      (np.minimum/maximum.reduceat over buckets): min and max of `ncol` columns of a row-major
 //                      float32 matrix over consecutive chunks of the (optionally permuted) rows.
@@ -38,6 +42,17 @@ __device__ __forceinline__ uint32_t part1by2(uint32_t n) {
 __device__ __forceinline__ uint32_t f2o(float f) {
     uint32_t u = __float_as_uint(f);
     return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+// the same for a min (max) slot, with every NaN mapped below (above) every number, so a NaN wins the slot; o2f of
+// either extreme is a NaN
+__device__ __forceinline__ uint32_t f2o_lo(float f) { return f != f ? 0u : f2o(f); }
+__device__ __forceinline__ uint32_t f2o_hi(float f) { return f != f ? 0xffffffffu : f2o(f); }
+// NaN-propagating min / max (np.min / np.max); -0.0 is below +0.0, so the result does not depend on the order
+__device__ __forceinline__ float nan_min(float a, float b) {
+    return a != a ? a : (b != b ? b : (b < a || (b == a && signbit(b)) ? b : a));
+}
+__device__ __forceinline__ float nan_max(float a, float b) {
+    return a != a ? a : (b != b ? b : (b > a || (b == a && !signbit(b)) ? b : a));
 }
 __device__ __forceinline__ float o2f(uint32_t o) {
     return __uint_as_float((o & 0x80000000u) ? (o & 0x7fffffffu) : ~o);
@@ -83,19 +98,19 @@ __global__ void __launch_bounds__(256) k_mo_bounds(const float* __restrict__ xyz
             float lo = p[a], hi = p[a];
 #pragma unroll
             for (int o = 16; o > 0; o >>= 1) {
-                lo = fminf(lo, __shfl_xor_sync(GSX_FULL, lo, o));
-                hi = fmaxf(hi, __shfl_xor_sync(GSX_FULL, hi, o));
+                lo = nan_min(lo, __shfl_xor_sync(GSX_FULL, lo, o));
+                hi = nan_max(hi, __shfl_xor_sync(GSX_FULL, hi, o));
             }
             if ((threadIdx.x & 31) == 0) {
-                atomicMin(bounds + 6 * s + a, f2o(lo));
-                atomicMax(bounds + 6 * s + 3 + a, f2o(hi));
+                atomicMin(bounds + 6 * s + a, f2o_lo(lo));
+                atomicMax(bounds + 6 * s + 3 + a, f2o_hi(hi));
             }
         }
     } else if (act) {
 #pragma unroll
         for (int a = 0; a < 3; ++a) {
-            atomicMin(bounds + 6 * s + a, f2o(p[a]));
-            atomicMax(bounds + 6 * s + 3 + a, f2o(p[a]));
+            atomicMin(bounds + 6 * s + a, f2o_lo(p[a]));
+            atomicMax(bounds + 6 * s + 3 + a, f2o_hi(p[a]));
         }
     }
 }
@@ -152,7 +167,8 @@ __global__ void __launch_bounds__(256) k_mo_starts(const uint64_t* __restrict__ 
     if (e == 0 || keys[e] != keys[e - 1]) starts[rank[e]] = (int)e;
 }
 
-// next level's runs: groups longer than `limit` whose parent run still has extent
+// next level's runs: groups longer than `limit` whose parent run still has extent.  counter[1] = 1 when such a group
+// is its whole parent run (the run did not split: it would be picked again for ever)
 __global__ void __launch_bounds__(256) k_mo_pick(const int* __restrict__ starts, int nrun, int64_t m,
                                                  const uint64_t* __restrict__ keys, const int* __restrict__ dead,
                                                  const int* __restrict__ seg_start, const int* __restrict__ seg_off,
@@ -163,6 +179,7 @@ __global__ void __launch_bounds__(256) k_mo_pick(const int* __restrict__ starts,
     if (e - b <= limit) return;
     const int s = (int)(keys[b] >> 30);
     if (dead[s]) return;
+    if (e - b == seg_off[s + 1] - seg_off[s]) counter[1] = 1;
     const int pos = seg_start[s] + (b - seg_off[s]);
     picked[atomicAdd(counter, 1)] = make_int2(pos, e - b);
 }
@@ -181,8 +198,8 @@ int64_t morton_workspace_bytes(int64_t n) {
     return (int64_t)b;
 }
 
-int morton_order(const float* xyz, int64_t n, int32_t* order, int limit, int max_levels, int* levels_out, void* ws,
-                 int64_t ws_bytes, cudaStream_t st) {
+int morton_order(const float* xyz, int64_t n, int32_t* order, int limit, int* levels_out, void* ws, int64_t ws_bytes,
+                 cudaStream_t st) {
     GSX_NVTX("gsx::morton_order");
     GSX_REQUIRE(n >= 0 && n < 2147483584ll, GSX_ERR_ARG, "morton: n out of range");
     if (levels_out) *levels_out = 0;
@@ -212,7 +229,7 @@ int morton_order(const float* xyz, int64_t n, int32_t* order, int limit, int max
     if (n == 1) return GSX_OK;
     std::vector<int> h_start{0}, h_len{(int)n};
     int level = 0;
-    while (!h_start.empty() && level < max_levels) {
+    while (!h_start.empty()) {
         const int nseg = (int)h_start.size();
         std::vector<int> h_off(nseg + 1, 0);
         for (int s = 0; s < nseg; ++s) h_off[s + 1] = h_off[s] + h_len[s];
@@ -250,26 +267,30 @@ int morton_order(const float* xyz, int64_t n, int32_t* order, int limit, int max
         k_mo_pick<<<(int)((nrun + 255) / 256), 256, 0, st>>>(starts, (int)nrun, m, ks, dead, seg_start, seg_off, limit, counter,
                                                             picked);
         GSX_KERNEL_CHECK();
-        int npick = 0;
-        GSX_CUDA_CHECK(cudaMemcpyAsync(&npick, counter, 4, cudaMemcpyDeviceToHost, st));
+        int npick[2] = {0, 0};
+        GSX_CUDA_CHECK(cudaMemcpyAsync(npick, counter, 8, cudaMemcpyDeviceToHost, st));
         GSX_CUDA_CHECK(cudaStreamSynchronize(st));
-        std::vector<int2> hp((size_t)npick);
-        if (npick) {
-            GSX_CUDA_CHECK(cudaMemcpyAsync(hp.data(), picked, (size_t)npick * sizeof(int2), cudaMemcpyDeviceToHost, st));
+        ++level;
+        if (levels_out) *levels_out = level;
+        GSX_REQUIRE(!npick[1], GSX_ERR_UNSUPPORTED,
+                    "morton: a run of more than %d splats did not split at level %d (infinite or NaN extent)", limit,
+                    level);
+        std::vector<int2> hp((size_t)npick[0]);
+        if (npick[0]) {
+            GSX_CUDA_CHECK(cudaMemcpyAsync(hp.data(), picked, (size_t)npick[0] * sizeof(int2), cudaMemcpyDeviceToHost, st));
             GSX_CUDA_CHECK(cudaStreamSynchronize(st));
         }
         std::sort(hp.begin(), hp.end(), [](const int2& a, const int2& b) { return a.x < b.x; });  // atomics: any order
-        h_start.resize((size_t)npick);
-        h_len.resize((size_t)npick);
-        for (int i = 0; i < npick; ++i) h_start[i] = hp[i].x, h_len[i] = hp[i].y;
-        ++level;
+        h_start.resize((size_t)npick[0]);
+        h_len.resize((size_t)npick[0]);
+        for (int i = 0; i < npick[0]; ++i) h_start[i] = hp[i].x, h_len[i] = hp[i].y;
     }
-    if (levels_out) *levels_out = level;
     return GSX_OK;
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// chunk min/max: one block per chunk, `ncol` (<= 8) columns of a row-major [n, F] matrix, rows optionally permuted
+// chunk min/max: one block per chunk, `ncol` (<= 8) columns of a row-major [n, F] matrix, rows optionally permuted.
+// A NaN makes its chunk's min and max NaN (np.minimum.reduceat); of two zeros the min is -0.0 and the max +0.0.
 __global__ void __launch_bounds__(256) k_chunk_minmax(const float* __restrict__ rows, int F, const int32_t* __restrict__ order,
                                                       int64_t n, int chunk, int ncol, const int* __restrict__ cols,
                                                       float clip_lo, float clip_hi, float* __restrict__ lo_out,
@@ -285,9 +306,9 @@ __global__ void __launch_bounds__(256) k_chunk_minmax(const float* __restrict__ 
         for (int a = 0; a < 8; ++a)
             if (a < ncol) {
                 float v = __ldg(r + cols[a]);
-                v = fminf(fmaxf(v, clip_lo), clip_hi);
-                lo[a] = fminf(lo[a], v);
-                hi[a] = fmaxf(hi[a], v);
+                v = v != v ? v : fminf(fmaxf(v, clip_lo), clip_hi);   // np.clip keeps NaN
+                lo[a] = nan_min(lo[a], v);
+                hi[a] = nan_max(hi[a], v);
             }
     }
     __shared__ float slo[8][8], shi[8][8];
@@ -296,15 +317,15 @@ __global__ void __launch_bounds__(256) k_chunk_minmax(const float* __restrict__ 
     for (int a = 0; a < 8; ++a) {
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) {
-            lo[a] = fminf(lo[a], __shfl_xor_sync(GSX_FULL, lo[a], o));
-            hi[a] = fmaxf(hi[a], __shfl_xor_sync(GSX_FULL, hi[a], o));
+            lo[a] = nan_min(lo[a], __shfl_xor_sync(GSX_FULL, lo[a], o));
+            hi[a] = nan_max(hi[a], __shfl_xor_sync(GSX_FULL, hi[a], o));
         }
         if (lane == 0) slo[a][w] = lo[a], shi[a][w] = hi[a];
     }
     __syncthreads();
     if (threadIdx.x < ncol) {
         float l = slo[threadIdx.x][0], h = shi[threadIdx.x][0];
-        for (int k = 1; k < 8; ++k) l = fminf(l, slo[threadIdx.x][k]), h = fmaxf(h, shi[threadIdx.x][k]);
+        for (int k = 1; k < 8; ++k) l = nan_min(l, slo[threadIdx.x][k]), h = nan_max(h, shi[threadIdx.x][k]);
         lo_out[(size_t)blockIdx.x * ncol + threadIdx.x] = l;
         hi_out[(size_t)blockIdx.x * ncol + threadIdx.x] = h;
     }

@@ -10,7 +10,8 @@
 //                with match.any on the digit + per-warp shared-memory counters, warps are chained by a
 //                per-digit prefix over the 8 warps; the pairs are first placed in shared memory in locally
 //                sorted order so that the final global writes are coalesced runs per digit.
-// Only the bits [begin_bit, end_bit) are sorted (the hash needs ceil(log2 N) bits, not 32).
+// Only the bits [begin_bit, end_bit) are sorted (the hash needs ceil(log2 N) bits, not 32): the last pass's digit is
+// masked to the bits below end_bit, so bits at and above end_bit do not take part.
 // HBM traffic per pass: 8 B (hist) + 12 B read + 12 B written per pair.
 #include "gsx_common.cuh"
 #include "gsx_radix.cuh"
@@ -99,8 +100,11 @@ int exclusive_scan_u32_ws(uint32_t* data, int64_t n, uint32_t* ws, cudaStream_t 
 }
 
 // ------------------------------------------------------------------ radix passes
+// the digit of the pass starting at bit `shift`: 8 bits, or the bits below end_bit in the last pass
+static uint32_t digit_mask(int shift, int end_bit) { return end_bit - shift >= 8 ? 255u : (1u << (end_bit - shift)) - 1u; }
+
 __global__ void __launch_bounds__(kRsThreads) k_rs_hist(const uint64_t* __restrict__ keys, int64_t n, int shift,
-                                                        int64_t ntiles, uint32_t* __restrict__ hist) {
+                                                        uint32_t dmask, int64_t ntiles, uint32_t* __restrict__ hist) {
     __shared__ uint32_t sh[256];
     sh[threadIdx.x] = 0;
     __syncthreads();
@@ -108,7 +112,7 @@ __global__ void __launch_bounds__(kRsThreads) k_rs_hist(const uint64_t* __restri
 #pragma unroll 4
     for (int e = 0; e < kRsPerThread; ++e) {
         int64_t i = base + (int64_t)e * kRsThreads + threadIdx.x;
-        if (i < n) atomicAdd(&sh[(uint32_t)(keys[i] >> shift) & 255u], 1u);
+        if (i < n) atomicAdd(&sh[(uint32_t)(keys[i] >> shift) & dmask], 1u);
     }
     __syncthreads();
     hist[(size_t)threadIdx.x * ntiles + blockIdx.x] = sh[threadIdx.x];
@@ -120,7 +124,7 @@ constexpr size_t kRsScatterSmem = (size_t)kRsTile * 12 + (size_t)8 * 256 * 4 + 2
 __global__ void __launch_bounds__(kRsThreads)
     k_rs_scatter(const uint64_t* __restrict__ keys_in, const int32_t* __restrict__ vals_in,
                  uint64_t* __restrict__ keys_out, int32_t* __restrict__ vals_out, int64_t n, int shift,
-                 int64_t ntiles, const uint32_t* __restrict__ base_off) {
+                 uint32_t dmask, int64_t ntiles, const uint32_t* __restrict__ base_off) {
     extern __shared__ __align__(16) unsigned char rs_smem[];
     uint64_t* skeys = reinterpret_cast<uint64_t*>(rs_smem);                      // [kRsTile]
     int32_t* svals = reinterpret_cast<int32_t*>(rs_smem + (size_t)kRsTile * 8);  // [kRsTile]
@@ -144,7 +148,7 @@ __global__ void __launch_bounds__(kRsThreads)
     for (int e = 0; e < kRsPerThread; ++e) {
         const int64_t i = wbase + e * 32 + lane;
         const bool act = i < n;
-        const uint32_t d = act ? ((uint32_t)(key[e] >> shift) & 255u) : (256u + lane);  // unique when inactive
+        const uint32_t d = act ? ((uint32_t)(key[e] >> shift) & dmask) : (256u + lane);  // unique when inactive
         const unsigned peers = __match_any_sync(GSX_FULL, d);
         const uint32_t before = act ? wcnt[w][d] : 0u;
         rank[e] = before + __popc(peers & ((1u << lane) - 1u));
@@ -190,7 +194,7 @@ __global__ void __launch_bounds__(kRsThreads)
     for (int e = 0; e < kRsPerThread; ++e) {
         const int64_t i = wbase + e * 32 + lane;
         if (i < n) {
-            const uint32_t d = (uint32_t)(key[e] >> shift) & 255u;
+            const uint32_t d = (uint32_t)(key[e] >> shift) & dmask;
             const uint32_t lp = dstart[d] + wcnt[w][d] + rank[e];
             skeys[lp] = key[e];
             svals[lp] = vals_in[i];
@@ -201,7 +205,7 @@ __global__ void __launch_bounds__(kRsThreads)
     const int cnt = (int)(n - tbase < kRsTile ? n - tbase : kRsTile);
     for (int j = threadIdx.x; j < cnt; j += kRsThreads) {
         const uint64_t k = skeys[j];
-        const uint32_t d = (uint32_t)(k >> shift) & 255u;
+        const uint32_t d = (uint32_t)(k >> shift) & dmask;
         const uint32_t pos = gbase[d] + ((uint32_t)j - dstart[d]);
         keys_out[pos] = k;
         vals_out[pos] = svals[j];
@@ -226,14 +230,15 @@ constexpr int kOsMaxPass = 8;
 constexpr uint32_t kOsSpinLimit = 1u << 22;
 
 __global__ void __launch_bounds__(256) k_os_hist(const uint64_t* __restrict__ keys, int64_t n, int begin_bit,
-                                                  int npass, uint32_t* __restrict__ ghist) {
+                                                  int npass, uint32_t last_mask, uint32_t* __restrict__ ghist) {
     __shared__ uint32_t sh[kOsMaxPass * 256];
     for (int t = threadIdx.x; t < npass * 256; t += 256) sh[t] = 0;
     __syncthreads();
     const int64_t stride = (int64_t)gridDim.x * 256;
     for (int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x; i < n; i += stride) {
         const uint64_t k = keys[i] >> begin_bit;
-        for (int p = 0; p < npass; ++p) atomicAdd(&sh[p * 256 + ((uint32_t)(k >> (8 * p)) & 255u)], 1u);
+        for (int p = 0; p < npass; ++p)
+            atomicAdd(&sh[p * 256 + ((uint32_t)(k >> (8 * p)) & (p == npass - 1 ? last_mask : 255u))], 1u);
     }
     __syncthreads();
     for (int t = threadIdx.x; t < npass * 256; t += 256)
@@ -269,7 +274,7 @@ constexpr size_t os_pass_smem() {
 template <bool PAIRS>
 __global__ void __launch_bounds__(kRsThreads, PAIRS ? 3 : 4)
     k_os_pass(const uint64_t* __restrict__ keys_in, const int32_t* __restrict__ vals_in, uint64_t* __restrict__ keys_out,
-              int32_t* __restrict__ vals_out, int64_t n, int shift, const uint32_t* __restrict__ gbase_pass,
+              int32_t* __restrict__ vals_out, int64_t n, int shift, uint32_t dmask, const uint32_t* __restrict__ gbase_pass,
               uint32_t* lookback, unsigned int* tile_counter) {
     extern __shared__ __align__(16) unsigned char rs_smem[];
     uint64_t* skeys = reinterpret_cast<uint64_t*>(rs_smem);                      // [kRsTile]
@@ -297,7 +302,7 @@ __global__ void __launch_bounds__(kRsThreads, PAIRS ? 3 : 4)
     for (int e = 0; e < kRsPerThread; ++e) {
         const int64_t i = wbase + e * 32 + lane;
         const bool act = i < n;
-        const uint32_t d = act ? ((uint32_t)(key[e] >> shift) & 255u) : (256u + lane);
+        const uint32_t d = act ? ((uint32_t)(key[e] >> shift) & dmask) : (256u + lane);
         const unsigned peers = __match_any_sync(GSX_FULL, d);
         const uint32_t before = act ? wcnt[w][d] : 0u;
         const uint32_t r = before + __popc(peers & ((1u << lane) - 1u));
@@ -354,7 +359,7 @@ __global__ void __launch_bounds__(kRsThreads, PAIRS ? 3 : 4)
     for (int e = 0; e < kRsPerThread; ++e) {
         const int64_t i = wbase + e * 32 + lane;
         if (i < n) {
-            const uint32_t d = (uint32_t)(key[e] >> shift) & 255u;
+            const uint32_t d = (uint32_t)(key[e] >> shift) & dmask;
             const uint32_t lp = dstart[d] + wcnt[w][d] + ((rank2[e >> 1] >> (16 * (e & 1))) & 0xffffu);
             skeys[lp] = key[e];
             if (PAIRS) svals[lp] = vals_in[i];
@@ -364,7 +369,7 @@ __global__ void __launch_bounds__(kRsThreads, PAIRS ? 3 : 4)
     const int cnt = (int)(n - tbase < kRsTile ? n - tbase : kRsTile);
     for (int j = threadIdx.x; j < cnt; j += kRsThreads) {
         const uint64_t k = skeys[j];
-        const uint32_t d = (uint32_t)(k >> shift) & 255u;
+        const uint32_t d = (uint32_t)(k >> shift) & dmask;
         const uint32_t pos = gbase[d] + ((uint32_t)j - dstart[d]);
         keys_out[pos] = k;
         if (PAIRS) vals_out[pos] = svals[j];
@@ -394,7 +399,8 @@ static int onesweep_sort(uint64_t* keys0, uint64_t* keys1, int32_t* vals0, int32
     }
     int64_t hb = (n + 255) / 256;
     if (hb > hist_blocks) hb = hist_blocks;
-    k_os_hist<<<(unsigned)hb, 256, 0, st>>>(keys0, n, begin_bit, npass, ghist);
+    const uint32_t last_mask = digit_mask(begin_bit + 8 * (npass - 1), end_bit);
+    k_os_hist<<<(unsigned)hb, 256, 0, st>>>(keys0, n, begin_bit, npass, last_mask, ghist);
     GSX_KERNEL_CHECK();
     k_os_scan<<<npass, 256, 0, st>>>(ghist);
     GSX_KERNEL_CHECK();
@@ -403,7 +409,8 @@ static int onesweep_sort(uint64_t* keys0, uint64_t* keys1, int32_t* vals0, int32
     int32_t *vin = vals0, *vout = vals1;
     for (int p = 0; p < npass; ++p) {
         k_os_pass<PAIRS><<<(unsigned)ntiles, kRsThreads, os_pass_smem<PAIRS>(), st>>>(
-            kin, vin, kout, vout, n, begin_bit + 8 * p, ghist + p * 256, lookback + (size_t)p * 256 * ntiles, counters + p);
+            kin, vin, kout, vout, n, begin_bit + 8 * p, p == npass - 1 ? last_mask : 255u, ghist + p * 256,
+            lookback + (size_t)p * 256 * ntiles, counters + p);
         GSX_KERNEL_CHECK();
         uint64_t* tk = kin;
         kin = kout;
@@ -444,11 +451,13 @@ int radix_sort_pairs(uint64_t* keys0, uint64_t* keys1, int32_t* vals0, int32_t* 
     uint64_t *kin = keys0, *kout = keys1;
     int32_t *vin = vals0, *vout = vals1;
     for (int shift = begin_bit; shift < end_bit; shift += 8) {
-        k_rs_hist<<<(unsigned)ntiles, kRsThreads, 0, st>>>(kin, n, shift, ntiles, hist);
+        const uint32_t dmask = digit_mask(shift, end_bit);
+        k_rs_hist<<<(unsigned)ntiles, kRsThreads, 0, st>>>(kin, n, shift, dmask, ntiles, hist);
         GSX_KERNEL_CHECK();
         int rc = exclusive_scan_u32(hist, (int64_t)256 * ntiles, scan_ws, st);
         if (rc) return rc;
-        k_rs_scatter<<<(unsigned)ntiles, kRsThreads, kRsScatterSmem, st>>>(kin, vin, kout, vout, n, shift, ntiles, hist);
+        k_rs_scatter<<<(unsigned)ntiles, kRsThreads, kRsScatterSmem, st>>>(kin, vin, kout, vout, n, shift, dmask, ntiles,
+                                                                          hist);
         GSX_KERNEL_CHECK();
         uint64_t* tk = kin;
         kin = kout;

@@ -5,7 +5,8 @@
 //
 // lexsort: stable LSD over the three float32 keys with our radix sort -- first by z (32 bits), then by the
 // 64-bit key x:y -- after mapping floats to order-preserving unsigned ints (-0.0 is folded into +0.0 because
-// NumPy compares them equal).  quantize: lower_bound in the (<= 4096-entry) codebook held in shared memory,
+// NumPy compares them equal; every NaN, whatever its sign and payload, gets one key above +inf because NumPy sorts
+// NaN last and treats NaNs as equal, so they keep index order).  quantize: lower_bound in the (<= 4096-entry) codebook held in shared memory,
 // clip, then the reference's left-neighbour test |v - cb[left]| < |v - cb[idx]| in float32.
 #include "gsx_common.cuh"
 #include "gsx_sh_mask.cuh"
@@ -15,6 +16,7 @@
 namespace gsx {
 
 __device__ __forceinline__ uint32_t float_key(float f) {
+    if (f != f) return 0xffffffffu;  // NaN: after +inf (0xff800000), all NaNs equal
     f = f + 0.0f;  // -0.0 -> +0.0 (equal keys in NumPy)
     uint32_t u = __float_as_uint(f);
     return (u & 0x80000000u) ? ~u : (u | 0x80000000u);

@@ -213,7 +213,8 @@ int gsx_density_grid_dense(const int32_t* grid_dev, const int64_t* q0, const int
 
 /* ---- SOG writer helpers, the steps either side of K-Means (SURVEY 8(f) item 1) ------------------- */
 /* formats/sog.py:264  np.lexsort((z, y, x)): order_dev[j] = index of the j-th splat in (x, then y, then z) order,
- * stable; -0.0 == +0.0 as in NumPy.  (NaN coordinates are not supported.) */
+ * stable; -0.0 == +0.0 as in NumPy; every NaN (either sign, any payload) sorts after +inf and NaNs compare equal,
+ * as in NumPy. */
 int64_t gsx_lexsort_workspace_bytes(int64_t n);
 int gsx_lexsort_zyx(const float* xyz_dev, int64_t n, int32_t* order_dev, void* ws, int64_t ws_bytes, void* stream);
 /* formats/sog.py:408-419 quantize_to_codebook: index of the nearest entry of an ascending float32 codebook
@@ -326,14 +327,18 @@ int gsx_records_scale_exp(const float* rows_dev, int64_t n, int32_t F, int32_t s
  * 3 x 10-bit Morton order (codes relative to the bounding box of the group; every run of equal codes longer than
  * run_limit (the reference: 256) is re-normalised to its own box and sorted again, until it is short or has no
  * extent).  Equal codes inside a finished run come out in ascending original index (the reference's unstable
- * np.argsort leaves that order unspecified).  *levels_out = number of levels that ran. */
+ * np.argsort leaves that order unspecified).  The levels run until no run is left; *levels_out = number of levels that
+ * ran (the reference's recursion depth + 1).  A NaN position makes its run's box NaN on that axis, as cx.min() does.
+ * Returns GSX_ERR_UNSUPPORTED when a run longer than run_limit does not split (zero, infinite or NaN extent on every
+ * axis, not all zero): the reference recurses into it for ever. */
 int64_t gsx_morton_workspace_bytes(int64_t n);
 int gsx_morton_order(const float* xyz_dev, int64_t n, int32_t* order_dev, int32_t run_limit, int32_t* levels_out, void* ws,
                      int64_t ws_bytes, void* stream);
 /* compressed_ply.py:206-246 (per-256-splat chunk bounds) / ksplat.py:426-441 (np.minimum/maximum.reduceat per
  * bucket): min and max of ncol (<= 8) columns cols_host[] of the row-major float32 matrix rows_dev [n,F] over
  * consecutive chunks of `chunk` rows taken in the order order_dev (NULL = identity); values are clipped to
- * [clip_lo, clip_hi] first (np.clip(scale, -20, 20) of compressed_ply.py:213-215; pass -inf/+inf for none).
+ * [clip_lo, clip_hi] first (np.clip(scale, -20, 20) of compressed_ply.py:213-215; pass -inf/+inf for none).  A NaN
+ * (kept by the clip, as np.clip does) makes its chunk's min and max NaN; of -0.0 and +0.0 the min is -0.0, the max +0.0.
  * lo_dev / hi_dev: float32 [ceil(n/chunk), ncol].  ws >= 64 bytes. */
 int gsx_chunk_minmax(const float* rows_dev, int64_t n, int32_t F, const int32_t* order_dev, int32_t chunk,
                      const int32_t* cols_host, int32_t ncol, float clip_lo, float clip_hi, float* lo_dev, float* hi_dev,
@@ -349,7 +354,8 @@ int gsx_chunk_minmax(const float* rows_dev, int64_t n, int32_t F, const int32_t*
  * (may be NULL when n_rest == 0), *rest_nonzero_dev (device uint64, zeroed here) = bit k set iff packed SH column k holds
  * a value != 0 -- the input of the SH-degree rule of :141-169, which the caller applies (gsx_cply_narrow_sh).
  * NumPy-2 float32 arithmetic, bit-exact except the alpha byte (expf: one count on ~1e-5 of the splats).  vertex_dev and
- * sh_dev 16-byte aligned; n < 2^31; n = 0 launches nothing.  (NaN inputs are not supported.) */
+ * sh_dev 16-byte aligned; n < 2^31; n = 0 launches nothing.  A NaN field packs as NumPy's x86 cast gives it,
+ * 0x80000000 shifted into the word (DESIGN §4.5); a quaternion's first NaN component is its largest. */
 int gsx_cply_pack(const float* rows_dev, int64_t n, int32_t F, const int32_t* order_dev, const int32_t* cols14_host,
                   const int32_t* rest_cols_host, int32_t n_rest, const float* lo_pos_dc_dev, const float* hi_pos_dc_dev,
                   const float* lo_scale_dev, const float* hi_scale_dev, float* chunk_dev, uint32_t* vertex_dev,
