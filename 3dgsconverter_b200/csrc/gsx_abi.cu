@@ -18,6 +18,7 @@
 #include "gsx_records.cuh"
 #include "gsx_sog.cuh"
 #include "gsx_sor.cuh"
+#include "gsx_splat_codecs.cuh"
 
 #include <atomic>
 #include <math.h>
@@ -632,6 +633,37 @@ int gsx_cply_pack(const float* rows_dev, int64_t n, int32_t F, const int32_t* or
 }
 int gsx_cply_narrow_sh(const uint8_t* sh_dev, int64_t n, int32_t width, int32_t keep, uint8_t* out_dev, void* stream) {
     return cply_narrow_sh(sh_dev, n, width, keep, out_dev, (cudaStream_t)stream);
+}
+
+int gsx_codec_sh_mask(const float* rows_dev, int64_t n, int32_t F, const int32_t* sh_cols_host, int32_t nsh,
+                      uint64_t* mask_dev, void* stream) {
+    return codec_sh_mask(rows_dev, n, F, sh_cols_host, nsh, (unsigned long long*)mask_dev, (cudaStream_t)stream);
+}
+int32_t gsx_ksplat_record_bytes(int32_t level, int32_t sh_count) { return ksplat_record_bytes(level, sh_count); }
+int gsx_ksplat_centres(const float* lo_dev, const float* hi_dev, int64_t nbucket, float* centres_dev, void* stream) {
+    return ksplat_centres(lo_dev, hi_dev, nbucket, centres_dev, (cudaStream_t)stream);
+}
+int gsx_ksplat_pack(const float* rows_dev, int64_t n, int32_t F, const int32_t* cols14_host, const int32_t* sh_cols_host,
+                    int32_t sh_count, int32_t level, int64_t bucket_size, float sf_inv, const float* centres_dev,
+                    uint8_t* out_dev, void* stream) {
+    return ksplat_pack(rows_dev, n, F, cols14_host, sh_cols_host, sh_count, level, bucket_size, sf_inv, centres_dev,
+                       out_dev, (cudaStream_t)stream);
+}
+int gsx_spz_pack(const float* rows_dev, int64_t n, int32_t F, const int32_t* cols14_host, const int32_t* sh_cols_host,
+                 int32_t sh_dim, uint8_t* body_dev, void* stream) {
+    return spz_pack(rows_dev, n, F, cols14_host, sh_cols_host, sh_dim, body_dev, (cudaStream_t)stream);
+}
+int gsx_splat_sort_keys(const float* rows_dev, int64_t n, int32_t F, const int32_t* cols4_host, uint64_t* keys_dev,
+                        int32_t* vals_dev, void* stream) {
+    return splat_sort_keys(rows_dev, n, F, cols4_host, keys_dev, vals_dev, (cudaStream_t)stream);
+}
+int gsx_splat_pack(const float* rows_dev, int64_t n, int32_t F, const int32_t* order_dev, const int32_t* cols14_host,
+                   uint8_t* out_dev, void* stream) {
+    return splat_pack(rows_dev, n, F, order_dev, cols14_host, out_dev, (cudaStream_t)stream);
+}
+int gsx_records_from_bytes(const uint8_t* src_dev, int64_t n, int64_t row_bytes, const int32_t* offsets_host, int32_t nf,
+                           float* out_dev, void* stream) {
+    return records_from_bytes(src_dev, n, row_bytes, offsets_host, nf, out_dev, (cudaStream_t)stream);
 }
 
 /* free / total device memory of the current device (sizing decisions of the host-buffer entry points) */

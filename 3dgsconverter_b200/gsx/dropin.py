@@ -11,7 +11,9 @@ and, when ``gsconverter.formats.compressed_ply`` imports, ``CompressedPlyFormat.
 and packing on the device, the file still written by the class's own ``_write_ply_file``; records gsx refuses go to
 the original ``write``).  With ``patch(sog="device")`` also ``SogFormat.write`` (gsx.sog.encode: every texture,
 codebook and the chunked SH palette built on the device; opt-in because its position bytes can differ from NumPy's
-log by one count on a small fraction of the splats).
+log by one count on a small fraction of the splats).  With ``patch(codecs="device")`` also ``SplatFormat.write``,
+``KSplatFormat.write`` and ``SpzFormat.write`` (gsx.splat / gsx.ksplat / gsx.spz: sort, bucket bounds and packing on the
+device, gzip and the file on the host; records gsx refuses go to the original ``write``).
 Host-only helpers and everything else of the reference stay as they are.
 """
 from __future__ import annotations
@@ -52,13 +54,17 @@ class _GsxCodebookKMeans:
 
 
 def patch(verbose: bool = False, defer: bool = True, codebook: str = "sklearn", require_cuda: bool = True,
-          sog: str = "host"):
+          sog: str = "host", codecs: str = "host"):
     """require_cuda: refuse (return False, leave the reference untouched) when no CUDA device is usable, so that a
     CPU-only host keeps the reference's own SciPy / scikit-learn paths (there is no CPU fallback inside gsx).
     sog: "host" keeps the reference's SogFormat.write (with the patched gpu_ops.kmeans and its batch-ahead);
-    "device" replaces it with gsx.sog's device encoder (records gsx refuses go to the original write)."""
+    "device" replaces it with gsx.sog's device encoder (records gsx refuses go to the original write).
+    codecs: "host" keeps the reference's .splat / .ksplat / .spz writers; "device" installs gsx's device writers on
+    them (records gsx refuses go to the original write)."""
     if sog not in ("host", "device"):
         raise ValueError(f"sog must be 'host' or 'device', not {sog!r}")
+    if codecs not in ("host", "device"):
+        raise ValueError(f"codecs must be 'host' or 'device', not {codecs!r}")
     if require_cuda:
         from . import backend_available
         if not backend_available():
@@ -118,6 +124,18 @@ def patch(verbose: bool = False, defer: bool = True, codebook: str = "sklearn", 
     if cply is not None and hasattr(cply, "CompressedPlyFormat"):
         from .compressed_ply import install
         install(cply.CompressedPlyFormat)             # compressed_ply.py:126-250 -> packing on the GPU
+    if codecs == "device":
+        from . import ksplat, splat, spz
+        for modname, clsname, ours in (("splat", "SplatFormat", splat), ("ksplat", "KSplatFormat", ksplat),
+                                       ("spz", "SpzFormat", spz)):
+            fmt = sys.modules.get(f"gsconverter.formats.{modname}")
+            if fmt is None:
+                try:
+                    fmt = importlib.import_module(f"gsconverter.formats.{modname}")
+                except Exception:  # noqa: BLE001  (writer not importable: nothing to patch there)
+                    continue
+            if hasattr(fmt, clsname):
+                ours.install(getattr(fmt, clsname))   # splat.py:82-166, ksplat.py:319-544, spz.py:49-173
     if verbose:
         print("[gsx] gsconverter.processing patched: SOR / density / bbox / alpha / K-Means / compressed PLY packing "
               "run on libgsx.so")

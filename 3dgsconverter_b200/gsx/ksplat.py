@@ -1,0 +1,132 @@
+"""The .ksplat writer on the device: formats/ksplat.py:319-544 (KSplatFormat.write) over DeviceRecords.  The SH degree
+rule reads one non-zero mask of the f_rest columns (gsx_codec_sh_mask); the bucket bounds (gsx_chunk_minmax), their
+centres and the interleaved records are computed on the GPU; the host builds the two headers.
+
+    enc = encode(records, compression_level=1)     # DeviceRecords -> KSplat (device tensors)
+    write_ksplat("out.ksplat", enc)                 # or enc.to_host(): the file's bytes
+"""
+from __future__ import annotations
+
+import ctypes as C
+import struct
+from dataclasses import dataclass
+
+import numpy as np
+import torch
+
+from ._abi import lib, check
+from .compressed_ply import PACK_FIELDS
+from .sor import _ptr, _stream
+
+HEADER_SIZE, SECTION_HEADER_SIZE = 4096, 1024
+MAGIC_MAJOR, MAGIC_MINOR = 0, 1
+MIN_SH, MAX_SH = -2.0, 2.0
+SCALE_RANGE = 32767
+
+
+@dataclass
+class KSplat:
+    head: bytes                     # file header, section header and the partial-bucket length word (if any)
+    centres: torch.Tensor | None    # float32 [B, 3]: bucket centres (levels >= 1)
+    records: torch.Tensor           # uint8 [N, record bytes]: the interleaved splats
+    sh_degree: int
+
+    def to_host(self) -> bytes:
+        """The whole .ksplat file."""
+        from .hostcopy import to_host
+        parts = [self.head] + ([to_host(self.centres).data] if self.centres is not None else [])
+        return b"".join(parts + [to_host(self.records).data])
+
+
+def _headers(n: int, level: int, sh_degree: int, sh_count: int, bucket_size: int, block_size: float) -> bytes:
+    """ksplat.py:370-417, field for field."""
+    header = bytearray(HEADER_SIZE)
+    header[0], header[1] = MAGIC_MAJOR, MAGIC_MINOR
+    struct.pack_into("<IIII", header, 4, 1, 1, n, n)
+    struct.pack_into("<H", header, 20, level)
+    struct.pack_into("<ff", header, 36, MIN_SH, MAX_SH)
+    section = bytearray(SECTION_HEADER_SIZE)
+    struct.pack_into("<II", section, 0, n, n)
+    if level >= 1:
+        struct.pack_into("<II", section, 8, bucket_size, (n + bucket_size - 1) // bucket_size)
+        struct.pack_into("<f", section, 16, block_size)
+        struct.pack_into("<H", section, 20, 12)
+        struct.pack_into("<I", section, 24, SCALE_RANGE)
+    per_splat = 44 + 4 * sh_count if level == 0 else 24 + (2 if level == 1 else 1) * sh_count
+    full, partial = n // bucket_size, 1 if n % bucket_size else 0
+    storage = partial * 4 + ((full + partial) * 12 if level >= 1 else 0) + n * per_splat
+    struct.pack_into("<III", section, 28, storage, full, partial)
+    struct.pack_into("<H", section, 40, sh_degree)
+    return bytes(header) + bytes(section) + (struct.pack("<I", n % bucket_size) if partial else b"")
+
+
+def encode(records, compression_level=0, sh_level=None, bucket_size=256, block_size=5.0) -> KSplat:
+    """Pack `records` (DeviceRecords) as KSplatFormat.write(data, path, compression_level, sh_level=...,
+    bucket_size=..., block_size=...) does.  None takes the reference's default for any argument but the level."""
+    level = int(compression_level)
+    sh_level = None if sh_level is None else int(sh_level)
+    bucket_size = 256 if bucket_size is None else int(bucket_size)
+    block_size = 5.0 if block_size is None else float(block_size)
+    if not 0 <= level <= 65535 or bucket_size < 1:
+        raise ValueError(f"compression_level {level} / bucket_size {bucket_size} out of range")
+    missing = [f for f in PACK_FIELDS if f not in records.col]
+    if missing:
+        raise ValueError(f".ksplat needs the fields {missing}")
+    nz = records.nonzero_columns([f"f_rest_{j}" for j in range(24)])
+    degree = 0
+    if any(f"f_rest_{j}" in nz for j in range(9)):
+        degree = 2 if any(f"f_rest_{j}" in nz for j in range(9, 24)) else 1
+    if sh_level is not None and sh_level < degree:
+        degree = sh_level
+    if degree < 0:
+        raise ValueError(f"sh_level {sh_level} < 0")
+    sh_count = {1: 9, 2: 24}.get(degree, 0)
+    sh_names = [f"f_rest_{j}" for j in range(sh_count)]
+    if any(f not in records.col for f in sh_names):
+        raise ValueError(f"SH degree {degree} needs the fields f_rest_0 .. f_rest_{sh_count - 1}")
+    n, dev = len(records), records.rows.device
+    head = _headers(n, level, degree, sh_count, bucket_size, block_size)
+    centres = None
+    sf_inv = 0.0
+    if level >= 1:
+        from .morton import chunk_minmax
+        nb = (n + bucket_size - 1) // bucket_size
+        centres = torch.empty((nb, 3), dtype=torch.float32, device=dev)
+        if n:
+            lo, hi = chunk_minmax(records.rows, [records.col[f] for f in ("x", "y", "z")], None, bucket_size)
+            check(lib.gsx_ksplat_centres(_ptr(lo), _ptr(hi), nb, _ptr(centres), _stream()), "gsx_ksplat_centres")
+        sf_inv = float(np.float32(SCALE_RANGE / (block_size / 2.0)))
+    rec = lib.gsx_ksplat_record_bytes(min(level, 3), sh_count)
+    out = torch.empty((n, rec), dtype=torch.uint8, device=dev)
+    c14 = (C.c_int32 * 14)(*[records.col[f] for f in PACK_FIELDS])
+    csh = (C.c_int32 * max(sh_count, 1))(*[records.col[f] for f in sh_names])
+    check(lib.gsx_ksplat_pack(_ptr(records.rows), n, records.F, c14, csh, sh_count, level, bucket_size, sf_inv,
+                              _ptr(centres), _ptr(out), _stream()), "gsx_ksplat_pack")
+    return KSplat(head, centres, out, degree)
+
+
+def write_ksplat(path, enc: KSplat) -> None:
+    with open(path, "wb") as fh:
+        fh.write(enc.to_host())
+
+
+def dropin_write(self, data: np.ndarray, path, *args, **kwargs) -> None:
+    """Replacement for KSplatFormat.write(data, path, compression_level=0, **kwargs): the file is packed on the
+    device; anything gsx refuses or fails on goes to the original write with the original arguments."""
+    from .records import DeviceRecords
+    try:
+        level = args[0] if args else kwargs.get("compression_level", 0)
+        enc = encode(DeviceRecords.from_writer_input(data), level, kwargs.get("sh_level"), kwargs.get("bucket_size"),
+                     kwargs.get("block_size"))
+        blob = enc.to_host()
+    except Exception:  # noqa: BLE001  (the reference's convention: exception => CPU path)
+        return self._gsx_reference_write(data, path, *args, **kwargs)
+    with open(path, "wb") as fh:
+        fh.write(blob)
+
+
+def install(cls) -> None:
+    """Make cls.write the device writer, keeping the original as cls._gsx_reference_write (idempotent)."""
+    if "_gsx_reference_write" not in cls.__dict__:
+        cls._gsx_reference_write = cls.write
+        cls.write = dropin_write

@@ -3,6 +3,8 @@ all-float32 fields) as one row-major float32 matrix in HBM.  Upload once, extrac
 gather the survivors on the device, one D2H at the end; plus the writers' elementwise attribute transforms."""
 from __future__ import annotations
 
+import ctypes as C
+
 import numpy as np
 import torch
 
@@ -32,6 +34,28 @@ class DeviceRecords:
         flat = np.ascontiguousarray(a).view(np.float32).reshape(len(a), len(a.dtype.names))
         from .hostcopy import to_device
         return cls(to_device(flat, device), a.dtype.names, a.dtype)
+
+    @classmethod
+    def from_writer_input(cls, a: np.ndarray, device="cuda"):
+        """Every float32 field of a writer's input `a`, whatever other fields it also carries (the converter adds
+        red/green/blue u1 before the .splat / .ksplat / SOG writers, converter.py:244-253); the other fields are
+        dropped.  Packed float32 records go up as from_structured does; any other layout is uploaded as raw rows once
+        and its float32 fields gathered on the device (gsx_records_from_bytes)."""
+        if is_packed_f32(a):
+            return cls.from_structured(a, device)
+        dt = a.dtype
+        names = [n for n in (dt.names or ()) if dt.fields[n][0] == np.dtype("<f4")]
+        if a.ndim != 1 or not names:
+            raise ValueError("DeviceRecords needs a 1-D structured array with float32 fields")
+        from .hostcopy import to_device
+        a = np.ascontiguousarray(a)
+        raw = to_device(a.view(np.uint8).reshape(-1), device)
+        rows = torch.empty((len(a), len(names)), dtype=torch.float32, device=raw.device)
+        offs = (C.c_int32 * len(names))(*[dt.fields[n][1] for n in names])
+        with torch.cuda.device(raw.device):
+            check(lib.gsx_records_from_bytes(_ptr(raw), len(a), dt.itemsize, offs, len(names), _ptr(rows), _stream()),
+                  "gsx_records_from_bytes")
+        return cls(rows, names, np.dtype([(n, "<f4") for n in names]))
 
     def __len__(self):
         return self.rows.shape[0]
@@ -83,3 +107,17 @@ class DeviceRecords:
         check(lib.gsx_records_scale_exp(_ptr(self.rows), n, self.F, self.col["scale_0"], self.col["scale_1"],
                                         self.col["scale_2"], _ptr(out), _stream()), "gsx_records_scale_exp")
         return out
+
+    def nonzero_columns(self, names) -> set:
+        """The fields among `names` (at most 45) that hold a value != 0, NaN included: np.any(a[f] != 0) for each, in
+        one pass over the rows (the input of the writers' SH-degree rules)."""
+        names = [f for f in names if f in self.col]
+        if not names or len(self) == 0:
+            return set()
+        from .hostcopy import to_host
+        mask = torch.empty(1, dtype=torch.int64, device=self.rows.device)
+        cols = (C.c_int32 * len(names))(*[self.col[f] for f in names])
+        check(lib.gsx_codec_sh_mask(_ptr(self.rows), len(self), self.F, cols, len(names), _ptr(mask), _stream()),
+              "gsx_codec_sh_mask")
+        m = int(to_host(mask).view(np.uint64)[0])
+        return {f for k, f in enumerate(names) if m >> k & 1}

@@ -1,0 +1,97 @@
+"""The .spz writer on the device: formats/spz.py:49-173 (SpzFormat.write, _pack_v3) over DeviceRecords.  The SH degree
+rule reads one non-zero mask of the f_rest columns (gsx_codec_sh_mask); the planar body is packed on the GPU
+(gsx_spz_pack) behind the 16-byte header; the host runs gzip.
+
+    enc = encode(records)                           # DeviceRecords -> Spz (device payload: header + body)
+    write_spz("out.spz", enc, compression_level=0)
+"""
+from __future__ import annotations
+
+import ctypes as C
+import gzip
+import struct
+from dataclasses import dataclass
+
+import numpy as np
+import torch
+
+from ._abi import lib, check
+from .compressed_ply import PACK_FIELDS
+from .sor import _ptr, _stream
+
+MAGIC, VERSION, FRACTIONAL_BITS, FLAG_ANTIALIASED = 0x5053474E, 3, 12, 1
+SH_DIM = {0: 0, 1: 3, 2: 8, 3: 15}
+
+
+@dataclass
+class Spz:
+    payload: torch.Tensor   # uint8 [16 + N * (20 + 3 * sh_dim)]: the uncompressed file, header included
+    sh_degree: int
+
+    def to_host(self) -> bytes:
+        """The payload the reference hands to gzip.compress."""
+        from .hostcopy import to_host
+        return to_host(self.payload).tobytes()
+
+
+def sh_degree(records) -> int:
+    """spz.py:50-77: the degree the field names allow, lowered to that of the last f_rest column with a value != 0."""
+    col = records.col
+    degree = 0
+    if "f_rest_0" in col:
+        degree = 3 if "f_rest_44" in col else 2 if "f_rest_23" in col else 1 if "f_rest_8" in col else 0
+    if degree == 0:
+        return 0
+    top = {3: 44, 2: 23, 1: 8}[degree]
+    nz = records.nonzero_columns([f"f_rest_{i}" for i in range(top + 1)])
+    last = max((i for i in range(top + 1) if f"f_rest_{i}" in nz), default=-1)
+    return 3 if last >= 24 else 2 if last >= 9 else 1 if last >= 0 else 0
+
+
+def encode(records) -> Spz:
+    """Pack `records` (DeviceRecords) as SpzFormat.write does, up to the gzip step."""
+    missing = [f for f in PACK_FIELDS if f not in records.col]
+    if missing:
+        raise ValueError(f".spz needs the fields {missing}")
+    degree = sh_degree(records)
+    dim = SH_DIM[degree]
+    sh_names = [f"f_rest_{i + 15 * c}" for i in range(dim) for c in range(3)]
+    absent = [f for f in sh_names if f not in records.col]
+    if absent:   # the reference raises a KeyError here
+        raise ValueError(f"SH degree {degree} of the SPZ layout needs the fields {absent}")
+    n, dev = len(records), records.rows.device
+    from .hostcopy import to_device
+    head = struct.pack("<IIIBBBB", MAGIC, VERSION, n, degree, FRACTIONAL_BITS, FLAG_ANTIALIASED, 0)
+    payload = torch.empty(16 + n * (20 + 3 * dim), dtype=torch.uint8, device=dev)
+    payload[:16].copy_(to_device(np.frombuffer(head, np.uint8), dev))
+    c14 = (C.c_int32 * 14)(*[records.col[f] for f in PACK_FIELDS])
+    csh = (C.c_int32 * max(len(sh_names), 1))(*[records.col[f] for f in sh_names])
+    check(lib.gsx_spz_pack(_ptr(records.rows), n, records.F, c14, csh, dim, _ptr(payload[16:]), _stream()),
+          "gsx_spz_pack")
+    return Spz(payload, degree)
+
+
+def write_spz(path, enc: Spz, compression_level=0) -> None:
+    """gzip at `compression_level` (0 = stored), as spz.py:97-102."""
+    with open(path, "wb") as fh:
+        fh.write(gzip.compress(enc.to_host(), compresslevel=compression_level))
+
+
+def dropin_write(self, data: np.ndarray, path, **kwargs) -> None:
+    """Replacement for SpzFormat.write: the payload is packed on the device and gzipped on the host; anything gsx
+    refuses or fails on goes to the original write with the original arguments."""
+    from .records import DeviceRecords
+    try:
+        payload = encode(DeviceRecords.from_writer_input(data)).to_host()
+        blob = gzip.compress(payload, compresslevel=kwargs.get("compression_level", 0))
+    except Exception:  # noqa: BLE001  (the reference's convention: exception => CPU path)
+        return self._gsx_reference_write(data, path, **kwargs)
+    with open(path, "wb") as fh:
+        fh.write(blob)
+
+
+def install(cls) -> None:
+    """Make cls.write the device writer, keeping the original as cls._gsx_reference_write (idempotent)."""
+    if "_gsx_reference_write" not in cls.__dict__:
+        cls._gsx_reference_write = cls.write
+        cls.write = dropin_write

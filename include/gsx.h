@@ -364,6 +364,54 @@ int gsx_cply_pack(const float* rows_dev, int64_t n, int32_t F, const int32_t* or
  * the detected SH degree keeps fewer columns than were packed.  0 <= keep <= width <= 45. */
 int gsx_cply_narrow_sh(const uint8_t* sh_dev, int64_t n, int32_t width, int32_t keep, uint8_t* out_dev, void* stream);
 
+/* The .ksplat / .spz / .splat writers (formats/ksplat.py:319-544, spz.py:49-173, splat.py:82-166) over device-resident
+ * float32 records [n, F].  cols14_host: the columns of x y z f_dc_0 f_dc_1 f_dc_2 opacity scale_0 scale_1 scale_2
+ * rot_0 rot_1 rot_2 rot_3.  NumPy-2 float32 arithmetic in the reference's order, NumPy's SIMD float32 exp restated
+ * exactly, NumPy's x86-64 casts (NaN -> 0 in uint8 / uint16, INT32_MIN in int32, 0x80000000 in a SIMD uint32 cast;
+ * float16 NaN = sign | 0x7c00 | mantissa >> 13).  n >= 2^31 is refused with GSX_ERR_UNSUPPORTED (int32 row indices,
+ * uint32 counts in the ksplat header); n = 0 launches nothing.
+ *
+ * ksplat.py:340-368 / spz.py:53-77 (np.all(x == 0) / np.any(x != 0) per f_rest column): *mask_dev (zeroed here) gets
+ * bit k iff column sh_cols_host[k] holds a value != 0 (NaN included, -0.0 excluded).  nsh <= 45.  The degree rules
+ * run on the host from this mask. */
+int gsx_codec_sh_mask(const float* rows_dev, int64_t n, int32_t F, const int32_t* sh_cols_host, int32_t nsh,
+                      uint64_t* mask_dev, void* stream);
+/* ksplat.py:396-403: bytes of one interleaved record at `level` (0: float32; 1: float16; >= 2: float16 with uint8 SH)
+ * for sh_count = 0, 9 or 24 SH values. */
+int32_t gsx_ksplat_record_bytes(int32_t level, int32_t sh_count);
+/* ksplat.py:439-445: centres_dev[b, a] = (lo_dev[b, a] + hi_dev[b, a]) / 2.0 in float32, for the bucket bounds
+ * [nbucket, 3] of gsx_chunk_minmax(x, y, z; chunk = bucket_size). */
+int gsx_ksplat_centres(const float* lo_dev, const float* hi_dev, int64_t nbucket, float* centres_dev, void* stream);
+/* ksplat.py:419-536: the interleaved records, n * gsx_ksplat_record_bytes(level, sh_count) bytes into out_dev, rows in
+ * stored order.  sh_cols_host: the columns of f_rest_0 .. f_rest_{sh_count-1}.  Level 0 writes the float32 position,
+ * exp(scale) and rotation bits; levels >= 1 write clip(rint((x - centre) * sf_inv) + 32767, 0, 65535) as uint16
+ * (centre = centres_dev row j / bucket_size) and float16 exp(scale), rotation and SH; level 2 stores the SH as
+ * uint8 clip((v + 2) / 4 * 255, 0, 255), and levels >= 3, as the reference does, the raw uint8 cast of v. */
+int gsx_ksplat_pack(const float* rows_dev, int64_t n, int32_t F, const int32_t* cols14_host, const int32_t* sh_cols_host,
+                    int32_t sh_count, int32_t level, int64_t bucket_size, float sf_inv, const float* centres_dev,
+                    uint8_t* out_dev, void* stream);
+/* spz.py:106-173 (_pack_v3): the planar SPZ body of n * (20 + 3 * sh_dim) bytes into body_dev: 24-bit positions
+ * (rint(x * 4096) as int32, low three bytes), alpha, colour, scales, smallest-three rotations (spz.py:298-343), then the
+ * SH bytes.  sh_dim = 0, 3, 8 or 15; sh_cols_host[3 * sh_dim] holds the columns of f_rest_i, f_rest_{i+15},
+ * f_rest_{i+30} for i < sh_dim, interleaved in that order. */
+int gsx_spz_pack(const float* rows_dev, int64_t n, int32_t F, const int32_t* cols14_host, const int32_t* sh_cols_host,
+                 int32_t sh_dim, uint8_t* body_dev, void* stream);
+/* splat.py:92-98: keys_dev[i] = an order-preserving uint32 key (bits 0..31 of the uint64 word) of
+ * -(exp(scale_0 + scale_1 + scale_2) * (1 / (1 + exp(-opacity)))), -0.0 sorted as +0.0 and every NaN above +inf, and
+ * vals_dev[i] = i.  cols4_host: scale_0 scale_1 scale_2 opacity.  gsx_sort_pairs on bits [0, 32) then gives NumPy's
+ * stable argsort of -metric. */
+int gsx_splat_sort_keys(const float* rows_dev, int64_t n, int32_t F, const int32_t* cols4_host, uint64_t* keys_dev,
+                        int32_t* vals_dev, void* stream);
+/* splat.py:100-164: the 32-byte .splat records of rows order_dev[0 .. n) into out_dev: float32 position,
+ * float32 exp(scale), RGBA8, and uint8 clip(r / |r| * 128 + 128, 0, 255) of the rotation. */
+int gsx_splat_pack(const float* rows_dev, int64_t n, int32_t F, const int32_t* order_dev, const int32_t* cols14_host,
+                   uint8_t* out_dev, void* stream);
+/* out_dev[j, k] = the float32 at byte offsets_host[k] of row j of src_dev (n rows of row_bytes bytes, any alignment):
+ * the float32 fields of a structured array that also holds other fields (the converter's red/green/blue u1), as the
+ * packed float32 rows the writers read.  1 <= nf <= 256. */
+int gsx_records_from_bytes(const uint8_t* src_dev, int64_t n, int64_t row_bytes, const int32_t* offsets_host, int32_t nf,
+                           float* out_dev, void* stream);
+
 /* The SOG shN schedule (formats/sog.py:536-549: up to 64 chunks of one SH block, each clustered by its own
  * gpu_ops.kmeans call) in ONE call on HOST buffers: one upload of the block, one batched launch per phase.
  * nprob problems back to back in X_host (rows row_off[p] .. row_off[p+1]), K centroids each;
