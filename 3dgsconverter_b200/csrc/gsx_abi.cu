@@ -15,6 +15,7 @@
 #include "gsx_masks.cuh"
 #include "gsx_morton.cuh"
 #include "gsx_radix.cuh"
+#include "gsx_readers.cuh"
 #include "gsx_records.cuh"
 #include "gsx_sog.cuh"
 #include "gsx_sor.cuh"
@@ -664,6 +665,29 @@ int gsx_splat_pack(const float* rows_dev, int64_t n, int32_t F, const int32_t* o
 int gsx_records_from_bytes(const uint8_t* src_dev, int64_t n, int64_t row_bytes, const int32_t* offsets_host, int32_t nf,
                            float* out_dev, void* stream) {
     return records_from_bytes(src_dev, n, row_bytes, offsets_host, nf, out_dev, (cudaStream_t)stream);
+}
+
+int gsx_splat_decode(const uint8_t* data_dev, int64_t n, const float* tables_dev, uint8_t* rows_dev, void* stream) {
+    return splat_decode(data_dev, n, tables_dev, rows_dev, (cudaStream_t)stream);
+}
+int gsx_ksplat_decode_section(const uint8_t* records_dev, int64_t n, int32_t level, int32_t sh_count, float scale_range,
+                              float scale_factor, const uint8_t* centres_dev, int64_t ncentres, int64_t full_buckets,
+                              int64_t bucket_size, const int64_t* partial_end_dev, int32_t npartial,
+                              const float* tables_dev, int32_t row_bytes, uint8_t* rows_dev, void* stream) {
+    return ksplat_decode_section(records_dev, n, level, sh_count, scale_range, scale_factor, centres_dev, ncentres,
+                                 full_buckets, bucket_size, partial_end_dev, npartial, tables_dev, row_bytes, rows_dev,
+                                 (cudaStream_t)stream);
+}
+int gsx_spz_decode(const uint8_t* body_dev, int64_t n, int32_t version, int32_t sh_dim, int32_t frac_bits,
+                   const float* tables_dev, int32_t row_bytes, uint8_t* rows_dev, void* stream) {
+    return spz_decode(body_dev, n, version, sh_dim, frac_bits, tables_dev, row_bytes, rows_dev, (cudaStream_t)stream);
+}
+int gsx_cply_decode(const uint8_t* chunk_dev, int64_t nchunk, int32_t chunk_row, const int32_t* chunk_offs_host,
+                    const uint8_t* vertex_dev, int64_t n, int32_t vertex_row, const int32_t* vertex_offs_host,
+                    const uint8_t* sh_dev, int32_t sh_row, const int32_t* sh_offs_host, int32_t nsh,
+                    const float* tables_dev, uint8_t* rows_dev, void* stream) {
+    return cply_decode(chunk_dev, nchunk, chunk_row, chunk_offs_host, vertex_dev, n, vertex_row, vertex_offs_host, sh_dev,
+                       sh_row, sh_offs_host, nsh, tables_dev, rows_dev, (cudaStream_t)stream);
 }
 
 /* free / total device memory of the current device (sizing decisions of the host-buffer entry points) */

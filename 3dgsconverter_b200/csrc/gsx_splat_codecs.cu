@@ -24,6 +24,7 @@
 #include "gsx_numpy_scalar.cuh"
 #include "gsx_sh_mask.cuh"
 #include "gsx_splat_codecs.cuh"
+#include "gsx_staged.cuh"
 
 namespace gsx {
 
@@ -72,25 +73,6 @@ __device__ __forceinline__ void load_tile(const float* __restrict__ rows, int F,
 __device__ __forceinline__ void load_cols(const CodecCols& cols, int32_t* scols) {
     for (int k = threadIdx.x; k < cols.ncol; k += blockDim.x) scols[k] = cols.c[k];
     __syncthreads();
-}
-
-// dst[0, nbytes) = s[0, nbytes), block-cooperative: a byte head up to dst's 16-byte boundary, 16-byte words realigned
-// from s's 32-bit words with funnel shifts, a byte tail.  s is 4-byte aligned with 4 readable bytes past nbytes.
-__device__ __forceinline__ void store_staged(uint8_t* __restrict__ dst, const uint8_t* s, int nbytes) {
-    const int a = (int)((uintptr_t)dst & 15);
-    const int h = a ? (16 - a < nbytes ? 16 - a : nbytes) : 0;
-    for (int i = threadIdx.x; i < h; i += blockDim.x) dst[i] = s[i];
-    const int nvec = (nbytes - h) >> 4;
-    const uint32_t* s32 = reinterpret_cast<const uint32_t*>(s) + (h >> 2);
-    const uint32_t sh = (uint32_t)(h & 3) * 8;
-    uint4* d4 = reinterpret_cast<uint4*>(dst + h);
-    for (int v = threadIdx.x; v < nvec; v += blockDim.x) {
-        const uint32_t* p = s32 + 4 * v;
-        const uint32_t x0 = p[0], x1 = p[1], x2 = p[2], x3 = p[3], x4 = p[4];
-        d4[v] = make_uint4(__funnelshift_r(x0, x1, sh), __funnelshift_r(x1, x2, sh), __funnelshift_r(x2, x3, sh),
-                           __funnelshift_r(x3, x4, sh));
-    }
-    for (int i = h + (nvec << 4) + threadIdx.x; i < nbytes; i += blockDim.x) dst[i] = s[i];
 }
 
 // np.clip((0.5 + C0 * f) * 255, 0, 255).astype(np.uint8)  (splat.py:135-137, ksplat.py:479-481)

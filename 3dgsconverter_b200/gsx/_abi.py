@@ -112,6 +112,12 @@ _SIGS = {
     "gsx_splat_sort_keys": (C.c_int, [_vp, _i64, _i32, C.POINTER(_i32), _vp, _vp, _vp]),
     "gsx_splat_pack": (C.c_int, [_vp, _i64, _i32, _vp, C.POINTER(_i32), _vp, _vp]),
     "gsx_records_from_bytes": (C.c_int, [_vp, _i64, _i64, C.POINTER(_i32), _i32, _vp, _vp]),
+    "gsx_splat_decode": (C.c_int, [_vp, _i64, _vp, _vp, _vp]),
+    "gsx_ksplat_decode_section": (C.c_int, [_vp, _i64, _i32, _i32, C.c_float, C.c_float, _vp, _i64, _i64, _i64, _vp, _i32,
+                                            _vp, _i32, _vp, _vp]),
+    "gsx_spz_decode": (C.c_int, [_vp, _i64, _i32, _i32, _i32, _vp, _i32, _vp, _vp]),
+    "gsx_cply_decode": (C.c_int, [_vp, _i64, _i32, C.POINTER(_i32), _vp, _i64, _i32, C.POINTER(_i32), _vp, _i32,
+                                  C.POINTER(_i32), _i32, _vp, _vp, _vp]),
     "gsx_copy_h2d": (C.c_int, [_vp, _vp, _i64, _vp]),
     "gsx_copy_d2h": (C.c_int, [_vp, _vp, _i64, _vp]),
     "gsx_host_gather_rows": (C.c_int, [_vp, _i64, _i64, _vp, _i64, _vp]),

@@ -1,10 +1,12 @@
-"""PlayCanvas compressed PLY export on the device: formats/compressed_ply.py:126-250 (CompressedPlyFormat.write) over
-DeviceRecords.  The Morton order (gsx_morton_order), the chunk bounds (gsx_chunk_minmax) and the per-splat packing
+"""PlayCanvas compressed PLY on the device.  decode: formats/compressed_ply.py:14-123 (CompressedPlyFormat.read): the
+PLY header parsed on the host, every splat de-normalised on the GPU (gsx_cply_decode).  encode / export:
+formats/compressed_ply.py:126-250 (CompressedPlyFormat.write) over DeviceRecords.  The Morton order (gsx_morton_order), the chunk bounds (gsx_chunk_minmax) and the per-splat packing
 (gsx_cply_pack) run on the GPU; only the packed 16 B per splat plus the SH bytes come back to the host.
 
     enc = encode(records)                       # DeviceRecords -> CompressedPly (device tensors)
     chunk_data, vertex_data, sh_data = enc.to_host()
     write_ply("out.compressed.ply", chunk_data, vertex_data, sh_data)
+    dec = decode("in.compressed.ply")           # -> readers.Decoded (rows, dtype, metadata)
 """
 from __future__ import annotations
 
@@ -145,3 +147,72 @@ def install(cls) -> None:
     if "_gsx_reference_write" not in cls.__dict__:
         cls._gsx_reference_write = cls.write
         cls.write = dropin_write
+
+
+FIXED_FIELDS = ("x", "y", "z", "nx", "ny", "nz", "f_dc_0", "f_dc_1", "f_dc_2", "opacity", "scale_0", "scale_1",
+                "scale_2", "rot_0", "rot_1", "rot_2", "rot_3")
+
+
+def read_tables():
+    """The byte-indexed maps of compressed_ply.py:113-122 (opacity logit, SH), float64 as NumPy promotes them and
+    rounded to float32 as the reader stores them."""
+    b = np.arange(256, dtype=np.uint8)
+    a = np.clip(b / 255.0, 1e-6, 1.0 - 1e-6)
+    return np.log(a / (1.0 - a)).astype(np.float32), ((b / 256.0 - 0.5) * 8.0).astype(np.float32)
+
+
+def _offsets(el, names, want):
+    """Byte offsets of `names` in element `el`, each of NumPy type `want`."""
+    out = []
+    for f in names:
+        if f not in (el.dtype.names or ()) or el.dtype.fields[f][0] != np.dtype(want):
+            raise ValueError(f"compressed PLY: {el.name}.{f} missing or not {want}")
+        out.append(el.dtype.fields[f][1])
+    return out
+
+
+def decode(data, device="cuda"):
+    """CompressedPlyFormat.read on the device, `data` the file's bytes or its path.  Binary little-endian PLY with the
+    elements chunk (float32 bounds), vertex (uint32 packed words) and optionally sh (uchar); property types may use
+    either PLY name (float / float32, uint / uint32, uchar / uint8) and come in any order.  Refused (ValueError): no
+    chunk element (the reference reads such a file as a plain 3DGS PLY), anything parse_ply_header refuses, a body cut
+    short, an sh element shorter than vertex or with more than 64 properties, SH names that repeat a fixed field."""
+    from . import readers
+    buf = readers.file_bytes(data)
+    els, end = readers.parse_ply_header(buf)
+    if "chunk" not in els or "vertex" not in els:
+        raise ValueError("compressed PLY: no chunk or vertex element")
+    if end > len(buf):
+        raise ValueError("compressed PLY: body cut short")
+    ch, vx, sh = els["chunk"], els["vertex"], els.get("sh")
+    coffs = _offsets(ch, CHUNK_DTYPE.names, "<f4")
+    voffs = _offsets(vx, VERTEX_DTYPE.names, "<u4")
+    names = list(sh.dtype.names or ()) if sh is not None else []
+    soffs = _offsets(sh, names, "u1") if names else []
+    n = vx.count
+    if sh is not None and sh.count < n:
+        raise ValueError("compressed PLY: sh element shorter than vertex")
+    if len(names) > 64 or set(names) & set(FIXED_FIELDS):
+        raise ValueError("compressed PLY: sh properties not read on the device")
+    if n >= 1 << 31:
+        raise ValueError("compressed PLY: 2^31 splats or more")
+    degree = 3 if len(names) >= 45 else 2 if len(names) >= 24 else 1 if len(names) >= 9 else 0
+    metadata = {"count": n, "sh_degree": degree, "chunks": ch.count}
+    dtype = np.dtype([(f, "<f4") for f in FIXED_FIELDS + tuple(names)])
+    raw = readers.upload(buf, device)
+    dev, base = raw.device, raw.data_ptr()
+    rows = torch.empty((n, dtype.itemsize), dtype=torch.uint8, device=dev)
+    tabs = readers.tables_on(dev, *read_tables())
+    i32 = lambda v: (C.c_int32 * max(len(v), 1))(*v)  # noqa: E731
+    with torch.cuda.device(dev):
+        check(lib.gsx_cply_decode(C.c_void_p(base + ch.offset), ch.count, max(ch.dtype.itemsize, 1), i32(coffs),
+                                  C.c_void_p(base + vx.offset), n, vx.dtype.itemsize, i32(voffs),
+                                  C.c_void_p(base + sh.offset) if names else None, sh.dtype.itemsize if names else 0,
+                                  i32(soffs), len(names), _ptr(tabs), _ptr(rows), _stream()), "gsx_cply_decode")
+    return readers.Decoded(rows, dtype, metadata)
+
+
+def install_reader(cls) -> None:
+    """Make cls.read the device reader, keeping the original as cls._gsx_reference_read (idempotent)."""
+    from . import readers
+    readers.install(cls, decode)

@@ -13,7 +13,11 @@ the original ``write``).  With ``patch(sog="device")`` also ``SogFormat.write`` 
 codebook and the chunked SH palette built on the device; opt-in because its position bytes can differ from NumPy's
 log by one count on a small fraction of the splats).  With ``patch(codecs="device")`` also ``SplatFormat.write``,
 ``KSplatFormat.write`` and ``SpzFormat.write`` (gsx.splat / gsx.ksplat / gsx.spz: sort, bucket bounds and packing on the
-device, gzip and the file on the host; records gsx refuses go to the original ``write``).
+device, gzip and the file on the host; records gsx refuses go to the original ``write``).  With
+``patch(readers="device")`` also the ``read`` of ``SplatFormat``, ``KSplatFormat``, ``SpzFormat`` and
+``CompressedPlyFormat`` (gsx.splat / gsx.ksplat / gsx.spz / gsx.compressed_ply ``decode``: headers and gunzip on the
+host, every splat decoded on the device, byte for byte as the reference readers; files gsx refuses go to the original
+``read``).  The SOG, parquet and plain PLY readers stay on the host.
 Host-only helpers and everything else of the reference stay as they are.
 """
 from __future__ import annotations
@@ -54,17 +58,21 @@ class _GsxCodebookKMeans:
 
 
 def patch(verbose: bool = False, defer: bool = True, codebook: str = "sklearn", require_cuda: bool = True,
-          sog: str = "host", codecs: str = "host"):
+          sog: str = "host", codecs: str = "host", readers: str = "host"):
     """require_cuda: refuse (return False, leave the reference untouched) when no CUDA device is usable, so that a
     CPU-only host keeps the reference's own SciPy / scikit-learn paths (there is no CPU fallback inside gsx).
     sog: "host" keeps the reference's SogFormat.write (with the patched gpu_ops.kmeans and its batch-ahead);
     "device" replaces it with gsx.sog's device encoder (records gsx refuses go to the original write).
     codecs: "host" keeps the reference's .splat / .ksplat / .spz writers; "device" installs gsx's device writers on
-    them (records gsx refuses go to the original write)."""
+    them (records gsx refuses go to the original write).
+    readers: "host" keeps the reference's .splat / .ksplat / .spz / compressed PLY readers; "device" installs gsx's
+    device readers on them (files gsx refuses go to the original read)."""
     if sog not in ("host", "device"):
         raise ValueError(f"sog must be 'host' or 'device', not {sog!r}")
     if codecs not in ("host", "device"):
         raise ValueError(f"codecs must be 'host' or 'device', not {codecs!r}")
+    if readers not in ("host", "device"):
+        raise ValueError(f"readers must be 'host' or 'device', not {readers!r}")
     if require_cuda:
         from . import backend_available
         if not backend_available():
@@ -136,6 +144,20 @@ def patch(verbose: bool = False, defer: bool = True, codebook: str = "sklearn", 
                     continue
             if hasattr(fmt, clsname):
                 ours.install(getattr(fmt, clsname))   # splat.py:82-166, ksplat.py:319-544, spz.py:49-173
+    if readers == "device":
+        from . import compressed_ply, ksplat, splat, spz
+        for modname, clsname, ours in (("splat", "SplatFormat", splat), ("ksplat", "KSplatFormat", ksplat),
+                                       ("spz", "SpzFormat", spz), ("compressed_ply", "CompressedPlyFormat",
+                                                                   compressed_ply)):
+            fmt = sys.modules.get(f"gsconverter.formats.{modname}")
+            if fmt is None:
+                try:
+                    fmt = importlib.import_module(f"gsconverter.formats.{modname}")
+                except Exception:  # noqa: BLE001  (reader not importable: nothing to patch there)
+                    continue
+            if hasattr(fmt, clsname):
+                ours.install_reader(getattr(fmt, clsname))   # splat.py:9-80, ksplat.py:29-317, spz.py:18-296,
+                #                                               compressed_ply.py:14-123
     if verbose:
         print("[gsx] gsconverter.processing patched: SOR / density / bbox / alpha / K-Means / compressed PLY packing "
               "run on libgsx.so")

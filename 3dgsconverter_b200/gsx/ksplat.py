@@ -1,9 +1,12 @@
-"""The .ksplat writer on the device: formats/ksplat.py:319-544 (KSplatFormat.write) over DeviceRecords.  The SH degree
+"""The .ksplat reader and writer on the device.  decode: formats/ksplat.py:29-317 (KSplatFormat.read): the headers are
+parsed on the host, every section's records decoded on the GPU (gsx_ksplat_decode_section).  encode:
+formats/ksplat.py:319-544 (KSplatFormat.write) over DeviceRecords.  The SH degree
 rule reads one non-zero mask of the f_rest columns (gsx_codec_sh_mask); the bucket bounds (gsx_chunk_minmax), their
 centres and the interleaved records are computed on the GPU; the host builds the two headers.
 
     enc = encode(records, compression_level=1)     # DeviceRecords -> KSplat (device tensors)
     write_ksplat("out.ksplat", enc)                 # or enc.to_host(): the file's bytes
+    dec = decode("in.ksplat")                       # -> readers.Decoded (rows, dtype, metadata)
 """
 from __future__ import annotations
 
@@ -14,6 +17,7 @@ from dataclasses import dataclass
 import numpy as np
 import torch
 
+from . import readers
 from ._abi import lib, check
 from .compressed_ply import PACK_FIELDS
 from .sor import _ptr, _stream
@@ -130,3 +134,102 @@ def install(cls) -> None:
     if "_gsx_reference_write" not in cls.__dict__:
         cls._gsx_reference_write = cls.write
         cls.write = dropin_write
+
+
+def read_tables():
+    """The byte-indexed maps of ksplat.py:24-27, 229-234, 257-258 (DC, opacity logit, level-2 SH), with the reference's
+    expressions and dtypes."""
+    b = np.arange(256, dtype=np.uint8)
+    dc = (b.astype(np.float32) / 255.0 - 0.5) / 0.28209479177387814
+    alpha = np.clip(b.astype(np.float32) / 255.0, 1e-7, 1.0 - 1e-7)
+    return dc, np.log(alpha / (1.0 - alpha)), (b.astype(np.float32) - 128.0) / 128.0
+
+
+_SECTION_KEYS = ("splatCount", "maxSplatCount", "bucketSize", "bucketCount", "bucketBlockSize", "bucketStorageSizeBytes",
+                 "compressionScaleRange", "storageSizeBytes", "fullBucketCount", "partiallyFilledBucketCount",
+                 "shDegree")
+
+
+def decode(data, device="cuda") -> readers.Decoded:
+    """KSplatFormat.read on the device, `data` the file's bytes or its path.  Refused (ValueError) where the reference
+    raises or does not read the file as written: a version other than 0.1, headers or sections cut short, levels >= 1
+    without bucket centres or with partial-bucket lengths that leave splats without a bucket or reach a bucket past the
+    centres, SH degrees above 255."""
+    buf = readers.file_bytes(data)
+    if len(buf) < HEADER_SIZE:
+        raise ValueError("ksplat: file shorter than its header")
+    if (buf[0], buf[1]) != (MAGIC_MAJOR, MAGIC_MINOR):
+        raise ValueError(f"ksplat: version {buf[0]}.{buf[1]}, not {MAGIC_MAJOR}.{MAGIC_MINOR}")
+    max_sections, _, _, splat_count = struct.unpack_from("<IIII", buf, 4)
+    level = struct.unpack_from("<H", buf, 20)[0]
+    min_sh, max_sh = struct.unpack_from("<ff", buf, 36)
+    payload = HEADER_SIZE + max_sections * SECTION_HEADER_SIZE
+    if payload > len(buf):
+        raise ValueError("ksplat: section headers cut short")
+    sections = []
+    for i in range(max_sections):
+        vals = struct.unpack_from("<IIIIfHxxIIIIH", buf, HEADER_SIZE + i * SECTION_HEADER_SIZE)
+        sec = dict(zip(_SECTION_KEYS, vals))
+        if sec["compressionScaleRange"] == 0 and level >= 1:
+            sec["compressionScaleRange"] = 32767
+        sections.append(sec)
+    metadata = {"v_major": buf[0], "v_minor": buf[1], "splat_count": splat_count, "compression_level": level,
+                "min_sh": min_sh, "max_sh": max_sh, "sections": sections}
+    degree = max((s["shDegree"] for s in sections), default=3)
+    if degree > 255:
+        raise ValueError(f"ksplat: SH degree {degree}")
+    dtype = readers.gaussian_dtype(sh_degree=degree)
+    lv = min(level, 2)
+    plan, off, total = [], payload, 0
+    for sec in sections:   # ksplat.py:109-145: where each section's arrays lie, checked before any upload
+        n, npart, nb = sec["splatCount"], sec["partiallyFilledBucketCount"], sec["bucketCount"]
+        sh_count = {1: 9, 2: 24}.get(sec["shDegree"], 0)
+        per = 44 + 4 * sh_count if lv == 0 else 24 + (2 if lv == 1 else 1) * sh_count
+        lengths_at, centres_at, rec_at = off, off + 4 * npart, off + 4 * npart + 12 * nb
+        if rec_at + n * per > len(buf):
+            raise ValueError("ksplat: section cut short")
+        ends = None
+        if lv >= 1:
+            if nb == 0:
+                raise ValueError("ksplat: no bucket centres")
+            full = sec["fullBucketCount"] * sec["bucketSize"]
+            ends = np.cumsum(np.frombuffer(buf, "<u4", npart, lengths_at), dtype=np.int64)
+            if full + (int(ends[-1]) if npart else 0) < n:
+                raise ValueError("ksplat: the bucket lengths leave splats without a bucket")
+            if n:
+                last = (n - 1) // sec["bucketSize"] if n <= full else \
+                    sec["fullBucketCount"] + int(np.searchsorted(ends, n - 1 - full, side="right"))
+                if last >= nb:
+                    raise ValueError("ksplat: a splat's bucket has no centre")
+        plan.append((sec, n, sh_count, centres_at, rec_at, ends))
+        off += 4 * npart + 12 * nb + sec["maxSplatCount"] * per
+        total += n
+    if total >= 1 << 31:
+        raise ValueError("ksplat: 2^31 splats or more")
+    raw = readers.upload(buf, device)
+    dev = raw.device
+    rows = torch.empty((total, dtype.itemsize), dtype=torch.uint8, device=dev)
+    tabs = readers.tables_on(dev, *read_tables())
+    base, row = raw.data_ptr(), 0
+    with torch.cuda.device(dev):
+        for sec, n, sh_count, centres_at, rec_at, ends in plan:
+            if n == 0:
+                continue
+            sr = sec["compressionScaleRange"]
+            sf = (sec["bucketBlockSize"] / 2.0) / sr if lv >= 1 else 0.0
+            ends_dev = None
+            if ends is not None and len(ends):
+                from .hostcopy import to_device
+                ends_dev = to_device(ends, dev)
+            check(lib.gsx_ksplat_decode_section(
+                C.c_void_p(base + rec_at), n, lv, sh_count, float(np.float32(sr)), float(np.float32(sf)),
+                C.c_void_p(base + centres_at), sec["bucketCount"], sec["fullBucketCount"], sec["bucketSize"],
+                _ptr(ends_dev), 0 if ends is None else len(ends), _ptr(tabs), dtype.itemsize,
+                _ptr(rows[row:row + n]), _stream()), "gsx_ksplat_decode_section")
+            row += n
+    return readers.Decoded(rows, dtype, metadata)
+
+
+def install_reader(cls) -> None:
+    """Make cls.read the device reader, keeping the original as cls._gsx_reference_read (idempotent)."""
+    readers.install(cls, decode)

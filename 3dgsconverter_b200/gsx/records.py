@@ -49,13 +49,22 @@ class DeviceRecords:
             raise ValueError("DeviceRecords needs a 1-D structured array with float32 fields")
         from .hostcopy import to_device
         a = np.ascontiguousarray(a)
-        raw = to_device(a.view(np.uint8).reshape(-1), device)
-        rows = torch.empty((len(a), len(names)), dtype=torch.float32, device=raw.device)
-        offs = (C.c_int32 * len(names))(*[dt.fields[n][1] for n in names])
+        return cls.from_device_bytes(to_device(a.view(np.uint8).reshape(-1), device), dt)
+
+    @classmethod
+    def from_device_bytes(cls, raw: torch.Tensor, dt: np.dtype):
+        """The float32 fields of structured rows of dtype `dt` already on the device (`raw`: their bytes, contiguous),
+        gathered on the device (gsx_records_from_bytes); the other fields are dropped."""
+        names = [n for n in (dt.names or ()) if dt.fields[n][0] == np.dtype("<f4")]
+        if not names:
+            raise ValueError("DeviceRecords needs a structured dtype with float32 fields")
+        n = raw.numel() // dt.itemsize
+        rows = torch.empty((n, len(names)), dtype=torch.float32, device=raw.device)
+        offs = (C.c_int32 * len(names))(*[dt.fields[f][1] for f in names])
         with torch.cuda.device(raw.device):
-            check(lib.gsx_records_from_bytes(_ptr(raw), len(a), dt.itemsize, offs, len(names), _ptr(rows), _stream()),
+            check(lib.gsx_records_from_bytes(_ptr(raw), n, dt.itemsize, offs, len(names), _ptr(rows), _stream()),
                   "gsx_records_from_bytes")
-        return cls(rows, names, np.dtype([(n, "<f4") for n in names]))
+        return cls(rows, names, np.dtype([(f, "<f4") for f in names]))
 
     def __len__(self):
         return self.rows.shape[0]

@@ -1,10 +1,12 @@
-"""The .splat writer on the device: formats/splat.py:82-166 (SplatFormat.write) over DeviceRecords.  The sort metric
+"""The .splat reader and writer on the device.  decode: formats/splat.py:9-80 (SplatFormat.read) from the file's bytes
+(gsx_splat_decode).  encode: formats/splat.py:82-166 (SplatFormat.write) over DeviceRecords.  The sort metric
 and its keys (gsx_splat_sort_keys), the stable radix sort (gsx_sort_pairs) and the 32-byte records (gsx_splat_pack)
 run on the GPU.  Equal metrics keep ascending index (NumPy's stable argsort; the reference's default argsort leaves
 their order unspecified).
 
     enc = encode(records)                           # DeviceRecords -> Splat (device tensors)
     write_splat("out.splat", enc)
+    dec = decode("in.splat")                        # -> readers.Decoded: dec.to_host() is what SplatFormat.read returns
 """
 from __future__ import annotations
 
@@ -14,6 +16,7 @@ from dataclasses import dataclass
 import numpy as np
 import torch
 
+from . import readers
 from ._abi import lib, check
 from .compressed_ply import PACK_FIELDS
 from .sor import _ptr, _stream, sort_pairs
@@ -70,3 +73,30 @@ def install(cls) -> None:
     if "_gsx_reference_write" not in cls.__dict__:
         cls._gsx_reference_write = cls.write
         cls.write = dropin_write
+
+
+def read_tables():
+    """The byte-indexed maps of splat.py:67-77 (DC, opacity logit), with the reference's expressions and dtypes."""
+    b = np.arange(256, dtype=np.uint8)
+    dc = (b.astype(np.float32) / 255.0 - 0.5) / readers.SH_C0
+    linear_alpha = np.clip(b.astype(np.float32) / 255.0, 1.0 / 255.0, 0.9999)
+    return dc, -np.log((1.0 / linear_alpha) - 1.0)
+
+
+def decode(data, device="cuda") -> readers.Decoded:
+    """SplatFormat.read on the device: every whole 32-byte record of `data` (bytes or a path), trailing bytes ignored
+    as np.fromfile ignores them."""
+    buf = readers.file_bytes(data)
+    n = len(buf) // 32
+    dtype = readers.gaussian_dtype(has_rgb=True, sh_degree=0)
+    raw = readers.upload(buf[:n * 32], device)
+    rows = torch.empty((n, dtype.itemsize), dtype=torch.uint8, device=raw.device)
+    tabs = readers.tables_on(raw.device, *read_tables())
+    with torch.cuda.device(raw.device):
+        check(lib.gsx_splat_decode(_ptr(raw), n, _ptr(tabs), _ptr(rows), _stream()), "gsx_splat_decode")
+    return readers.Decoded(rows, dtype, None)
+
+
+def install_reader(cls) -> None:
+    """Make cls.read the device reader, keeping the original as cls._gsx_reference_read (idempotent)."""
+    readers.install(cls, decode)

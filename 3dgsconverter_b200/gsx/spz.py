@@ -1,9 +1,12 @@
-"""The .spz writer on the device: formats/spz.py:49-173 (SpzFormat.write, _pack_v3) over DeviceRecords.  The SH degree
+"""The .spz reader and writer on the device.  decode: formats/spz.py:18-47, 175-296 (SpzFormat.read, _read_body): gunzip
+and the 16-byte header on the host, the planar body on the GPU (gsx_spz_decode).  encode: formats/spz.py:49-173
+(SpzFormat.write, _pack_v3) over DeviceRecords.  The SH degree
 rule reads one non-zero mask of the f_rest columns (gsx_codec_sh_mask); the planar body is packed on the GPU
 (gsx_spz_pack) behind the 16-byte header; the host runs gzip.
 
     enc = encode(records)                           # DeviceRecords -> Spz (device payload: header + body)
     write_spz("out.spz", enc, compression_level=0)
+    dec = decode("in.spz")                          # -> readers.Decoded: dec.to_host() is what SpzFormat.read returns
 """
 from __future__ import annotations
 
@@ -15,6 +18,7 @@ from dataclasses import dataclass
 import numpy as np
 import torch
 
+from . import readers
 from ._abi import lib, check
 from .compressed_ply import PACK_FIELDS
 from .sor import _ptr, _stream
@@ -95,3 +99,49 @@ def install(cls) -> None:
     if "_gsx_reference_write" not in cls.__dict__:
         cls._gsx_reference_write = cls.write
         cls.write = dropin_write
+
+
+def read_tables():
+    """The byte-indexed maps of spz.py:200-222, 243, 345-348 (opacity logit, DC, red/green/blue, scale, SH), with the
+    reference's expressions and dtypes; the scale map is float64 (u8 / 16.0), stored as float32 as the reader stores
+    it."""
+    b = np.arange(256, dtype=np.uint8)
+    v = np.clip(b.astype(np.float32) / 255.0, 1e-7, 1.0 - 1e-7)
+    dc = (b.astype(np.float32) / 255.0 - 0.5) / 0.15
+    rgb = np.clip((0.5 + readers.SH_C0 * dc) * 255.0, 0, 255).astype(np.uint8)
+    return np.log(v / (1.0 - v)), dc, rgb, (b / 16.0 - 10.0).astype(np.float32), (b.astype(np.float32) - 128.0) / 128.0
+
+
+def decode(data, device="cuda") -> readers.Decoded:
+    """SpzFormat.read on the device, `data` the file's bytes or its path (gunzipped on the host when it starts with
+    1f 8b).  Refused (ValueError) where the reference raises or does not read the file as written: a bad magic or
+    version, a body shorter than the header's count needs, 1 << frac_bits beyond float32."""
+    buf = readers.file_bytes(data)
+    if len(buf) > 2 and buf[0] == 0x1F and buf[1] == 0x8B:
+        buf = memoryview(gzip.decompress(buf))
+    if len(buf) < 16:
+        raise ValueError("spz: shorter than its header")
+    magic, version, n, degree, frac_bits, _, _ = struct.unpack_from("<IIIBBBB", buf, 0)
+    if magic != MAGIC or not 1 <= version <= 3:
+        raise ValueError(f"spz: magic {magic:#x} / version {version}")
+    if frac_bits > 127:
+        raise ValueError(f"spz: 1 << {frac_bits} is not a float32")
+    if n >= 1 << 31:
+        raise ValueError("spz: 2^31 splats or more")
+    dim = SH_DIM.get(degree, 0)
+    need = n * ((6 if version == 1 else 9) + 7 + (4 if version >= 3 else 3) + 3 * dim)
+    if len(buf) - 16 < need:
+        raise ValueError("spz: body cut short")
+    dtype = readers.gaussian_dtype(has_rgb=True, sh_degree=degree)
+    raw = readers.upload(buf[16:16 + need], device)
+    rows = torch.empty((n, dtype.itemsize), dtype=torch.uint8, device=raw.device)
+    tabs = readers.tables_on(raw.device, *read_tables())
+    with torch.cuda.device(raw.device):
+        check(lib.gsx_spz_decode(_ptr(raw), n, version, dim, frac_bits, _ptr(tabs), dtype.itemsize, _ptr(rows),
+                                 _stream()), "gsx_spz_decode")
+    return readers.Decoded(rows, dtype, None)
+
+
+def install_reader(cls) -> None:
+    """Make cls.read the device reader, keeping the original as cls._gsx_reference_read (idempotent)."""
+    readers.install(cls, decode)

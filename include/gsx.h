@@ -412,6 +412,43 @@ int gsx_splat_pack(const float* rows_dev, int64_t n, int32_t F, const int32_t* o
 int gsx_records_from_bytes(const uint8_t* src_dev, int64_t n, int64_t row_bytes, const int32_t* offsets_host, int32_t nf,
                            float* out_dev, void* stream);
 
+/* Readers: the file's bytes on the device -> rows in the exact byte layout of the structured array the reference
+ * reader returns (row_bytes = that dtype's itemsize; red/green/blue u1 fields included).  tables_dev holds 256-entry
+ * float32 tables, one per map of a single input byte, which the caller builds with the reference's own NumPy expression
+ * (gsx.splat / gsx.ksplat / gsx.spz / gsx.compressed_ply build them): NumPy's float32 and float64 log come out as the
+ * host computes them.  Input buffers may start at any byte.  n < 2^31.
+ * gsx_splat_decode (splat.py:9-80): n 32-byte records -> n rows of 71 bytes (define_dtype(has_rgb=True, sh_degree=0));
+ *   scales log(max(s, 1e-6)) with NumPy's float32 log, rotations (b - 128) / 128 renormalised by max(norm, 1e-6);
+ *   nx/ny/nz and red/green/blue stay 0.  tables: DC, opacity logit. */
+int gsx_splat_decode(const uint8_t* data_dev, int64_t n, const float* tables_dev, uint8_t* rows_dev, void* stream);
+/* gsx_ksplat_decode_section (ksplat.py:109-264): one section's n records of level 0, 1 or 2 (any stored level >= 2)
+ * into rows of row_bytes bytes (define_dtype(sh_degree = the file's largest section degree)); the section's sh_count
+ * (0, 9 or 24) values fill f_rest_0 .., the other f_rest columns stay 0.  Levels >= 1: splat i lies in bucket
+ * i / bucket_size below full_buckets * bucket_size, past it in partial bucket full_buckets + k for the first k with
+ * partial_end_dev[k] (the prefix sums of the partially-filled bucket lengths) > i - full_buckets * bucket_size;
+ * positions are (float32(u16) - scale_range) * scale_factor + centre in float32.  Every splat's bucket must have a
+ * centre among the ncentres of centres_dev (checked from the last splat's).  tables: DC, opacity logit, level-2 SH. */
+int gsx_ksplat_decode_section(const uint8_t* records_dev, int64_t n, int32_t level, int32_t sh_count, float scale_range,
+                              float scale_factor, const uint8_t* centres_dev, int64_t ncentres, int64_t full_buckets,
+                              int64_t bucket_size, const int64_t* partial_end_dev, int32_t npartial,
+                              const float* tables_dev, int32_t row_bytes, uint8_t* rows_dev, void* stream);
+/* gsx_spz_decode (spz.py:175-296): the gunzipped body after the 16-byte header of version 1, 2 or 3 -> rows of
+ * row_bytes bytes (define_dtype(has_rgb=True, sh_degree = the header's degree)).  sh_dim = 0, 3, 8 or 15 (0 for
+ * degrees above 3, whose f_rest columns stay 0); positions float16 (v1) or int24 / 2^frac_bits (frac_bits <= 127);
+ * rotations first-three (v1, v2) or smallest-three in float64 (v3).  tables: opacity logit, DC, RGB, scale, SH. */
+int gsx_spz_decode(const uint8_t* body_dev, int64_t n, int32_t version, int32_t sh_dim, int32_t frac_bits,
+                   const float* tables_dev, int32_t row_bytes, uint8_t* rows_dev, void* stream);
+/* gsx_cply_decode (compressed_ply.py:14-123, 342-378): a binary little-endian compressed PLY's elements chunk (nchunk
+ * rows of chunk_row bytes; chunk_offs_host[18]: byte offsets of min_x .. max_b in gsx.compressed_ply.CHUNK_DTYPE
+ * order, float32), vertex (n rows of vertex_row bytes; vertex_offs_host[4]: packed_position, packed_rotation,
+ * packed_scale, packed_color, uint32) and sh (sh_row bytes; sh_offs_host[nsh]: its uchar properties in file order,
+ * nsh <= 64) -> n rows of 4 * (17 + nsh) bytes.  Bounds and de-normalisation in float64 as NumPy promotes them, rounded
+ * once on store; rows past nchunk * 256 stay 0.  tables: opacity logit, SH. */
+int gsx_cply_decode(const uint8_t* chunk_dev, int64_t nchunk, int32_t chunk_row, const int32_t* chunk_offs_host,
+                    const uint8_t* vertex_dev, int64_t n, int32_t vertex_row, const int32_t* vertex_offs_host,
+                    const uint8_t* sh_dev, int32_t sh_row, const int32_t* sh_offs_host, int32_t nsh,
+                    const float* tables_dev, uint8_t* rows_dev, void* stream);
+
 /* The SOG shN schedule (formats/sog.py:536-549: up to 64 chunks of one SH block, each clustered by its own
  * gpu_ops.kmeans call) in ONE call on HOST buffers: one upload of the block, one batched launch per phase.
  * nprob problems back to back in X_host (rows row_off[p] .. row_off[p+1]), K centroids each;
