@@ -171,12 +171,26 @@ def _offsets(el, names, want):
     return out
 
 
+DECODE_ROWS = 128                  # rows per CTA of gsx_cply_decode
+DECODE_ROW_MAX = 1024              # the widest chunk, vertex or sh row it stages
+DECODE_SMEM_MAX = 200 * 1024       # dynamic shared memory per CTA it accepts
+
+
+def decode_smem_bytes(vertex_row: int, sh_row: int, nsh: int) -> int:
+    """Dynamic shared memory per CTA of gsx_cply_decode (cply_decode in gsx_readers.cu): the staged vertex and sh rows,
+    each rounded up to 16 bytes with 16 bytes of slack, then the output rows."""
+    up16 = lambda x: (x + 15) & ~15  # noqa: E731
+    return (up16(DECODE_ROWS * vertex_row + 16) + (up16(DECODE_ROWS * sh_row + 16) if nsh else 0) +
+            DECODE_ROWS * 4 * (len(FIXED_FIELDS) + nsh) + 16)
+
+
 def decode(data, device="cuda"):
     """CompressedPlyFormat.read on the device, `data` the file's bytes or its path.  Binary little-endian PLY with the
     elements chunk (float32 bounds), vertex (uint32 packed words) and optionally sh (uchar); property types may use
     either PLY name (float / float32, uint / uint32, uchar / uint8) and come in any order.  Refused (ValueError): no
     chunk element (the reference reads such a file as a plain 3DGS PLY), anything parse_ply_header refuses, a body cut
-    short, an sh element shorter than vertex or with more than 64 properties, SH names that repeat a fixed field."""
+    short, an sh element shorter than vertex or with more than 64 properties, SH names that repeat a fixed field, a
+    chunk, vertex or sh row wider than 1024 bytes, rows that need more than 200 KB of shared memory per CTA."""
     from . import readers
     buf = readers.file_bytes(data)
     els, end = readers.parse_ply_header(buf)
@@ -196,6 +210,15 @@ def decode(data, device="cuda"):
         raise ValueError("compressed PLY: sh properties not read on the device")
     if n >= 1 << 31:
         raise ValueError("compressed PLY: 2^31 splats or more")
+    # the kernel refuses these too, but as a GsxError after the upload; the caller is promised a ValueError
+    srow = sh.dtype.itemsize if names else 0
+    if max(ch.dtype.itemsize, vx.dtype.itemsize, srow) > DECODE_ROW_MAX:
+        raise ValueError(f"compressed PLY: rows of {ch.dtype.itemsize} / {vx.dtype.itemsize} / {srow} bytes (chunk / "
+                         f"vertex / sh); at most {DECODE_ROW_MAX} are read on the device")
+    smem = decode_smem_bytes(vx.dtype.itemsize, srow, len(names))
+    if smem > DECODE_SMEM_MAX:
+        raise ValueError(f"compressed PLY: these rows need {smem} bytes of shared memory per CTA, more than "
+                         f"{DECODE_SMEM_MAX}")
     degree = 3 if len(names) >= 45 else 2 if len(names) >= 24 else 1 if len(names) >= 9 else 0
     metadata = {"count": n, "sh_degree": degree, "chunks": ch.count}
     dtype = np.dtype([(f, "<f4") for f in FIXED_FIELDS + tuple(names)])
