@@ -18,6 +18,7 @@
 #include "gsx_readers.cuh"
 #include "gsx_records.cuh"
 #include "gsx_sog.cuh"
+#include "gsx_sog_decode.cuh"
 #include "gsx_sor.cuh"
 #include "gsx_splat_codecs.cuh"
 
@@ -688,6 +689,21 @@ int gsx_cply_decode(const uint8_t* chunk_dev, int64_t nchunk, int32_t chunk_row,
                     const float* tables_dev, uint8_t* rows_dev, void* stream) {
     return cply_decode(chunk_dev, nchunk, chunk_row, chunk_offs_host, vertex_dev, n, vertex_row, vertex_offs_host, sh_dev,
                        sh_row, sh_offs_host, nsh, tables_dev, rows_dev, (cudaStream_t)stream);
+}
+int gsx_sog_decode_palette(const uint8_t* centroids_dev, int64_t palette_size, int32_t coeffs, const float* codebook_dev,
+                           int32_t codebook_len, float* palette_dev, int32_t* error_dev, void* stream) {
+    return sog_decode_palette(centroids_dev, palette_size, coeffs, codebook_dev, codebook_len, palette_dev, error_dev,
+                              (cudaStream_t)stream);
+}
+int gsx_sog_decode(const uint8_t* const* textures_host, int64_t n, const float* position_tables_dev,
+                   const float* tables_dev, int32_t scale_codebook_len, int32_t sh0_codebook_len,
+                   const float* palette_dev, int64_t palette_size, int32_t coeffs, uint8_t* rows_dev, int32_t* error_dev,
+                   void* stream) {
+    GSX_REQUIRE(textures_host, GSX_ERR_ARG, "gsx_sog_decode: no texture table");
+    const SogTextures tx{textures_host[0], textures_host[1], textures_host[2],
+                         textures_host[3], textures_host[4], textures_host[5]};
+    return sog_decode(tx, n, position_tables_dev, tables_dev, scale_codebook_len, sh0_codebook_len, palette_dev,
+                      palette_size, coeffs, rows_dev, error_dev, (cudaStream_t)stream);
 }
 
 /* free / total device memory of the current device (sizing decisions of the host-buffer entry points) */

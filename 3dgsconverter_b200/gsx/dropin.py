@@ -17,7 +17,10 @@ device, gzip and the file on the host; records gsx refuses go to the original ``
 ``patch(readers="device")`` also the ``read`` of ``SplatFormat``, ``KSplatFormat``, ``SpzFormat`` and
 ``CompressedPlyFormat`` (gsx.splat / gsx.ksplat / gsx.spz / gsx.compressed_ply ``decode``: headers and gunzip on the
 host, every splat decoded on the device, byte for byte as the reference readers; files gsx refuses go to the original
-``read``).  The SOG, parquet and plain PLY readers stay on the host.
+``read``).  With ``patch(sog_reader="device")`` also ``SogFormat.read`` (gsx.sog_reader.decode: ZIP, meta.json and
+WebP on the host, the shN palette and every splat decoded on the device, byte for byte as the reference reader, its
+palette indexing included; bundles gsx refuses go to the original ``read``).  The parquet and plain PLY readers stay
+on the host.
 Host-only helpers and everything else of the reference stay as they are.
 """
 from __future__ import annotations
@@ -58,7 +61,7 @@ class _GsxCodebookKMeans:
 
 
 def patch(verbose: bool = False, defer: bool = True, codebook: str = "sklearn", require_cuda: bool = True,
-          sog: str = "host", codecs: str = "host", readers: str = "host"):
+          sog: str = "host", codecs: str = "host", readers: str = "host", sog_reader: str = "host"):
     """require_cuda: refuse (return False, leave the reference untouched) when no CUDA device is usable, so that a
     CPU-only host keeps the reference's own SciPy / scikit-learn paths (there is no CPU fallback inside gsx).
     sog: "host" keeps the reference's SogFormat.write (with the patched gpu_ops.kmeans and its batch-ahead);
@@ -66,13 +69,17 @@ def patch(verbose: bool = False, defer: bool = True, codebook: str = "sklearn", 
     codecs: "host" keeps the reference's .splat / .ksplat / .spz writers; "device" installs gsx's device writers on
     them (records gsx refuses go to the original write).
     readers: "host" keeps the reference's .splat / .ksplat / .spz / compressed PLY readers; "device" installs gsx's
-    device readers on them (files gsx refuses go to the original read)."""
+    device readers on them (files gsx refuses go to the original read).
+    sog_reader: "host" keeps the reference's SogFormat.read; "device" installs gsx.sog_reader's device reader on it
+    (bundles gsx refuses go to the original read)."""
     if sog not in ("host", "device"):
         raise ValueError(f"sog must be 'host' or 'device', not {sog!r}")
     if codecs not in ("host", "device"):
         raise ValueError(f"codecs must be 'host' or 'device', not {codecs!r}")
     if readers not in ("host", "device"):
         raise ValueError(f"readers must be 'host' or 'device', not {readers!r}")
+    if sog_reader not in ("host", "device"):
+        raise ValueError(f"sog_reader must be 'host' or 'device', not {sog_reader!r}")
     if require_cuda:
         from . import backend_available
         if not backend_available():
@@ -123,6 +130,9 @@ def patch(verbose: bool = False, defer: bool = True, codebook: str = "sklearn", 
     if sog_mod is not None and sog == "device" and hasattr(sog_mod, "SogFormat"):
         from .sog import install as install_sog
         install_sog(sog_mod.SogFormat)                # sog.py:249-639 -> textures and palette on the GPU
+    if sog_mod is not None and sog_reader == "device" and hasattr(sog_mod, "SogFormat"):
+        from .sog_reader import install_reader as install_sog_reader
+        install_sog_reader(sog_mod.SogFormat)         # sog.py:23-247 -> palette and rows on the GPU
     cply = sys.modules.get("gsconverter.formats.compressed_ply")
     if cply is None:
         try:

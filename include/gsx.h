@@ -448,6 +448,26 @@ int gsx_cply_decode(const uint8_t* chunk_dev, int64_t nchunk, int32_t chunk_row,
                     const uint8_t* vertex_dev, int64_t n, int32_t vertex_row, const int32_t* vertex_offs_host,
                     const uint8_t* sh_dev, int32_t sh_row, const int32_t* sh_offs_host, int32_t nsh,
                     const float* tables_dev, uint8_t* rows_dev, void* stream);
+/* The SOG reader (formats/sog.py:23-247, SogFormat.read) after the WebP step, in two launches on the same stream.
+ * Textures are the decoded members' RGBA pixels (4 bytes each, 4-byte aligned).  An index the reference rejects with
+ * IndexError ORs a bit into *error_dev (1: scales codebook, 2: sh0 codebook, 4: shN codebook, 8: label >= P); the
+ * caller zeroes the word first and refuses the file if it is non-zero afterwards.
+ * gsx_sog_decode_palette (sog.py:181-211, the palette double loop): palette_dev float32 [palette_size, coeffs]
+ *   (coeffs 0, 9, 24 or 45), entry [i, c * C + j] = codebook_dev[byte c of centroids pixel (i / 64) * 64 * coeffs +
+ *   (i % 64) * C + j], C = coeffs / 3: the reader's index formula, which differs from the writer's layout for entries
+ *   >= 64 (reproduced, not fixed).  codebook_len entries past 256 are never indexed.
+ * gsx_sog_decode (sog.py:60-179, 213-245): textures_host[6] = device pointers to the means_l, means_u, quats, scales,
+ *   sh0 and shN_labels pixels (the last null without shN) -> n rows of 4 * (17 + coeffs) bytes, define_dtype(sh_degree =
+ *   bands).  position_tables_dev float32 [3, 65536]: x, y, z of each u16 code; tables_dev float32 [4, 256]: quaternion
+ *   component (u8 / 255 - 0.5) * 2, opacity logit, scales codebook, sh0 codebook (each padded to 256).  Quaternion:
+ *   max_comp = uint8(alpha - 252), missing = sqrt(max(1 - ((a*a + b*b) + c*c), 0)) in float32, rot_* 0 for max_comp
+ *   > 3; f_rest = palette_dev[R | G << 8 of the labels].  n < 2^31. */
+int gsx_sog_decode_palette(const uint8_t* centroids_dev, int64_t palette_size, int32_t coeffs, const float* codebook_dev,
+                           int32_t codebook_len, float* palette_dev, int32_t* error_dev, void* stream);
+int gsx_sog_decode(const uint8_t* const* textures_host, int64_t n, const float* position_tables_dev,
+                   const float* tables_dev, int32_t scale_codebook_len, int32_t sh0_codebook_len,
+                   const float* palette_dev, int64_t palette_size, int32_t coeffs, uint8_t* rows_dev, int32_t* error_dev,
+                   void* stream);
 
 /* The SOG shN schedule (formats/sog.py:536-549: up to 64 chunks of one SH block, each clustered by its own
  * gpu_ops.kmeans call) in ONE call on HOST buffers: one upload of the block, one batched launch per phase.
