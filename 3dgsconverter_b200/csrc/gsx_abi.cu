@@ -506,37 +506,18 @@ int gsx_kmeans_lloyd_device(const float* X_dev, const int64_t* row_off_host, int
 }
 
 int32_t gsx_kmeans_tensor_core_supported(int32_t K, int32_t D) {
-    return kmeans_tc_supported(K, D) ? (kmeans_tc16_built() ? 3 : 1) : 0;   // bit 0: TF32 kernel, bit 1: split-bf16 build
+    return kmeans_tc_supported(K, D) ? 1 : 0;
 }
 
 int gsx_kmeans_tc_debug_scores(const float* X_dev, int64_t rows, const float* C_dev, int32_t K, int32_t D,
-                               int32_t variant, float* scores_dev, void* ws, int64_t ws_bytes, void* stream) {
-    return kmeans_tc_debug_scores(X_dev, rows, C_dev, K, D, variant, scores_dev, ws, ws_bytes, (cudaStream_t)stream);
+                               float* scores_dev, void* ws, int64_t ws_bytes, void* stream) {
+    return kmeans_tc_debug_scores(X_dev, rows, C_dev, K, D, scores_dev, ws, ws_bytes, (cudaStream_t)stream);
 }
 
 int gsx_kmeans_host(const float* X_host, int64_t n, int32_t K, int32_t D, int32_t max_iter, float* C_host_inout,
                     int32_t* labels_host, int32_t assign_mode) {
-    GSX_REQUIRE(n >= 1 && K >= 1 && D >= 1, GSX_ERR_ARG, "kmeans: bad shape");
-    cudaStream_t st = 0;
-    DevBuf X(st), C(st), L(st), cnt(st), ws(st);
-    int rc;
-    int64_t wsb = kmeans_workspace_bytes(n, 1, K, D);
-    if ((rc = X.alloc((size_t)n * D * 4))) return rc;
-    if ((rc = C.alloc((size_t)K * D * 4))) return rc;
-    if ((rc = L.alloc((size_t)n * 4))) return rc;
-    if ((rc = cnt.alloc((size_t)K * 4))) return rc;
-    if ((rc = ws.alloc((size_t)wsb))) return rc;
-    if ((rc = copy_h2d(X.p, X_host, (size_t)n * D * 4, st))) return rc;
-    GSX_CUDA_CHECK(cudaMemcpyAsync(C.p, C_host_inout, (size_t)K * D * 4, cudaMemcpyHostToDevice, st));
-    GSX_CUDA_CHECK(cudaMemsetAsync(L.p, 0, (size_t)n * 4, st));
-    int64_t off[2] = {0, n};
-    if ((rc = kmeans_lloyd((const float*)X.p, off, 1, K, D, max_iter, (float*)C.p, (int*)L.p, (int*)cnt.p, ws.p, wsb, assign_mode, nullptr, st)))
-        return rc;
-    prefault_host(labels_host, (size_t)n * 4);   // while the Lloyd iterations run
-    GSX_CUDA_CHECK(cudaMemcpyAsync(C_host_inout, C.p, (size_t)K * D * 4, cudaMemcpyDeviceToHost, st));
-    if ((rc = copy_d2h(labels_host, L.p, (size_t)n * 4, st))) return rc;
-    GSX_CUDA_CHECK(cudaStreamSynchronize(st));
-    return GSX_OK;
+    const int64_t off[2] = {0, n};
+    return gsx_kmeans_host_batched(X_host, off, 1, K, D, max_iter, C_host_inout, labels_host, assign_mode);
 }
 
 /* SOG shN schedule in one call on HOST buffers: nprob problems stored back to back in X_host (rows row_off[p] ..

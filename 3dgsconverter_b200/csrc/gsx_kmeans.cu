@@ -11,8 +11,8 @@
 //   * assign: x rows live in registers (D is a template parameter), centroids are staged through
 //     shared memory in tiles and read as broadcast float4; every thread runs P points x 2 centroids
 //     = 2P independent accumulation chains, so the dependent FADD chain of the contract does not
-//     stall the FP32 pipes.  CUDA cores, not tensor cores: the contract's rounding sequence is not
-//     a GEMM (DESIGN.md discusses the GEMM-prefilter idea for a later round).
+//     stall the FP32 pipes.  The contract's rounding sequence is not a GEMM; the tensor-core form
+//     (gsx_kmeans_tc.cu) uses a GEMM score only to pick candidates for this same strict distance.
 //   * update: a stable partition of the point indices by label (per-warp shared-memory counters,
 //     match.any ranks -- O(N)), then one warp per (problem, cluster) walks its member list in index
 //     order with 8 row loads in flight and accumulates lane-per-dimension.  This reproduces the
@@ -124,207 +124,6 @@ __global__ void __launch_bounds__(kAssignThreads)
 #pragma unroll
     for (int p = 0; p < P; ++p)
         if (live[p]) labels[row[p]] = best_k[p];
-}
-
-// ---------------------------------------------------------------------------------------------
-// Exact pre-filter (optional, gsx_kmeans_set_prefilter): the contract's distance costs 3 FP32 instructions
-// per (point, centroid, dim).  Here every centroid is first scored with ONE fma per dim,
-//     s_c = x.c - 0.5*||c||^2        (so that  E_c = ||x||^2 - 2 s_c  is the squared distance),
-// and only the centroids whose score is within a rigorous rounding-error margin of the best score are then
-// evaluated with the strict (sub, mul, add -- no fma, dims ascending) distance of SURVEY A.5, lowest index
-// winning ties.  Let c* be the contract's answer, c' the best-scoring centroid, delta >= |(-2 s_c) - (||c||^2 -
-// 2 x.c)| the fma-chain error bound gamma_{2D} (Cmax^2 + 2 ||x|| Cmax), and g' = 2 gamma_{D+2}/(1-gamma_{D+2})
-// the bound of the strict evaluation.  Then  s_{c*} >= s_{c'} - (delta + g'/2 * E_{c'})  (DESIGN.md §4.6), so a
-// candidate set with margin 2*delta + g' * (||x||^2 - 2 s_max + delta) (twice the bound) always contains c*.
-// Up to kPreCand candidates per point live in shared memory; overflow (many near-ties) or a non-finite margin
-// falls back to the full strict scan, so the labels are bit-identical to k_kmeans_assign in every case.
-constexpr int kPreCand = 8;
-
-template <int D>
-__device__ __forceinline__ float strict_dist(const float* __restrict__ x, const float* __restrict__ c) {
-    float acc = 0.f;
-#pragma unroll
-    for (int d = 0; d < D; ++d) {
-        float df = __fsub_rn(x[d], __ldg(c + d));
-        acc = __fadd_rn(acc, __fmul_rn(df, df));
-    }
-    return acc;
-}
-
-// per problem: an upper bound of max_c ||c|| (input of the error margin)
-__global__ void __launch_bounds__(256) k_kmeans_cmax(const float* __restrict__ C, int K, int D,
-                                                     float* __restrict__ cmax) {
-    const float* Cp = C + (size_t)blockIdx.x * K * D;
-    float m = 0.f;
-    for (int c = threadIdx.x; c < K; c += blockDim.x) {
-        float cn = 0.f;
-        for (int d = 0; d < D; ++d) {
-            float v = Cp[(size_t)c * D + d];
-            cn = __fmaf_rn(v, v, cn);
-        }
-        m = fmaxf(m, cn);
-    }
-    __shared__ float sm[256];
-    sm[threadIdx.x] = m;
-    __syncthreads();
-    for (int o = 128; o > 0; o >>= 1) {
-        if (threadIdx.x < o) sm[threadIdx.x] = fmaxf(sm[threadIdx.x], sm[threadIdx.x + o]);
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) cmax[blockIdx.x] = sqrtf(sm[0]) * 1.0001f;
-}
-
-template <int D, int P>
-__global__ void __launch_bounds__(kAssignThreads)
-    k_kmeans_assign_pre(const float* __restrict__ X, const float* __restrict__ C, int* __restrict__ labels,
-                        const KmProb* __restrict__ probs, int nprob, int K, const float* __restrict__ cmax) {
-    constexpr int DP = (D + 3) / 4 * 4;
-    constexpr int G = DP / 4;
-    __shared__ __align__(16) float sc[kCentTile * DP];
-    __shared__ float shalf[kCentTile];                              // -0.5 * ||c||^2
-    __shared__ float cand_s[kPreCand][P][kAssignThreads];           // [slot][point][thread]: conflict-free
-    __shared__ int cand_i[kPreCand][P][kAssignThreads];
-
-    int lo = 0, hi = nprob - 1;
-    while (lo < hi) {
-        int mid = (lo + hi + 1) >> 1;
-        if (probs[mid].tile0 <= (int)blockIdx.x) lo = mid; else hi = mid - 1;
-    }
-    const KmProb pr = probs[lo];
-    const long long tile = (long long)blockIdx.x - pr.tile0;
-    const float* Cp = C + (size_t)lo * K * D;
-    const int tid = threadIdx.x;
-
-    float x[P][DP];
-    long long row[P];
-    bool live[P];
-    float smax[P], marg[P], xnu[P], delta[P];
-    int ncand[P];
-    bool ovf[P];
-    const float Cm = cmax[lo];
-    constexpr float kU = 5.9604645e-8f;                              // 2^-24
-    constexpr float kGam2D = (2 * D + 2) * kU * 1.02f;               // >= gamma_{2D}
-    constexpr float kGs = 2.f * (D + 3) * kU * 1.02f;                // >= 2 gamma_{D+2} / (1 - gamma_{D+2})
-#pragma unroll
-    for (int p = 0; p < P; ++p) {
-        long long r = tile * (kAssignThreads * P) + p * kAssignThreads + tid;
-        live[p] = r < pr.rows;
-        row[p] = pr.row0 + (live[p] ? r : 0);
-        const float* xr = X + (size_t)row[p] * D;
-        float xn = 0.f;
-#pragma unroll
-        for (int d = 0; d < DP; ++d) {
-            x[p][d] = d < D ? xr[d] : 0.f;
-            xn = __fmaf_rn(x[p][d], x[p][d], xn);
-        }
-        xnu[p] = xn * 1.0001f;                                       // >= ||x||^2
-        const float xnorm = sqrtf(xnu[p]) * 1.0001f;
-        delta[p] = kGam2D * (Cm * Cm + 2.f * xnorm * Cm) * 1.01f + 1e-37f;
-        smax[p] = -3.0e38f;
-        marg[p] = INFINITY;
-        ncand[p] = 0;
-        ovf[p] = false;
-    }
-    auto margin_of = [&](int p) {  // twice the proven bound, in the score domain
-        float e_ub = fmaxf(xnu[p] - 2.f * smax[p] + delta[p], 0.f);
-        return 2.f * delta[p] + kGs * e_ub + 1e-37f;
-    };
-    auto consider = [&](int p, int c, float sv) {
-        if (!(sv >= smax[p] - marg[p])) return;
-        if (sv > smax[p]) {
-            smax[p] = sv;
-            marg[p] = margin_of(p);
-        }
-        int nc = ncand[p];
-        if (nc == kPreCand) {  // drop the entries that fell out of the margin of the current best
-            const float thr = smax[p] - marg[p];
-            int w = 0;
-            for (int r = 0; r < kPreCand; ++r) {
-                float cs = cand_s[r][p][tid];
-                if (cs >= thr) {
-                    cand_s[w][p][tid] = cs;
-                    cand_i[w][p][tid] = cand_i[r][p][tid];
-                    ++w;
-                }
-            }
-            nc = w;
-        }
-        if (nc < kPreCand) {
-            cand_s[nc][p][tid] = sv;
-            cand_i[nc][p][tid] = c;
-            ncand[p] = nc + 1;
-        } else {
-            ncand[p] = nc;
-            ovf[p] = true;
-        }
-    };
-
-    for (int k0 = 0; k0 < K; k0 += kCentTile) {
-        const int kt = K - k0 < kCentTile ? K - k0 : kCentTile;
-        __syncthreads();
-        for (int t = tid; t < kCentTile * DP; t += kAssignThreads) {
-            int c = t / DP, d = t - c * DP;
-            sc[t] = (c < kt && d < D) ? Cp[(size_t)(k0 + c) * D + d] : 0.f;
-        }
-        __syncthreads();
-        if (tid < kCentTile) {
-            float cn = 0.f;
-            for (int d = 0; d < D; ++d) cn = __fmaf_rn(sc[tid * DP + d], sc[tid * DP + d], cn);
-            shalf[tid] = -0.5f * cn;
-        }
-        __syncthreads();
-        for (int c = 0; c < kt; c += 4) {  // kCentTile is a multiple of 4; rows >= kt are zero and ignored
-            float acc[4][P];
-#pragma unroll
-            for (int q = 0; q < 4; ++q)
-#pragma unroll
-                for (int p = 0; p < P; ++p) acc[q][p] = shalf[c + q];
-#pragma unroll
-            for (int g = 0; g < G; ++g) {
-                float4 r4[4];
-#pragma unroll
-                for (int q = 0; q < 4; ++q) r4[q] = reinterpret_cast<const float4*>(sc + (c + q) * DP)[g];
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                    const float cv[4] = {r4[q].x, r4[q].y, r4[q].z, r4[q].w};
-#pragma unroll
-                    for (int e = 0; e < 4; ++e)
-                        if (g * 4 + e < D) {
-#pragma unroll
-                            for (int p = 0; p < P; ++p) acc[q][p] = __fmaf_rn(x[p][g * 4 + e], cv[e], acc[q][p]);
-                        }
-                }
-            }
-#pragma unroll
-            for (int q = 0; q < 4; ++q)
-                if (c + q < kt) {
-#pragma unroll
-                    for (int p = 0; p < P; ++p) consider(p, k0 + c + q, acc[q][p]);
-                }
-        }
-    }
-#pragma unroll
-    for (int p = 0; p < P; ++p) {
-        if (!live[p]) continue;
-        float best = 1e20f;
-        int bk = -1;
-        const bool exact_all = ovf[p] || !(marg[p] < 3.0e38f) || !(smax[p] > -3.0e38f);
-        if (exact_all) {
-            for (int c = 0; c < K; ++c) {
-                float dist = strict_dist<D>(x[p], Cp + (size_t)c * D);
-                if (dist < best) best = dist, bk = c;
-            }
-        } else {
-            const float thr = smax[p] - marg[p];
-            for (int r = 0; r < ncand[p]; ++r) {  // ascending centroid index: strict '<' keeps the lowest on ties
-                if (!(cand_s[r][p][tid] >= thr)) continue;
-                const int c = cand_i[r][p][tid];
-                float dist = strict_dist<D>(x[p], Cp + (size_t)c * D);
-                if (dist < best) best = dist, bk = c;
-            }
-        }
-        labels[row[p]] = bk;
-    }
 }
 
 // any D: one point per thread, x re-read through L1 (slow path for unusual dimensions)
@@ -596,7 +395,6 @@ struct KmWs {
     int* hist;
     int* totals;
     int* offs;
-    float* cmax;
     int* err;
     size_t total;
     bool ok;
@@ -611,7 +409,6 @@ static KmWs km_carve(void* ws, size_t bytes, int64_t n_total, int nprob, int K, 
     w.hist = c.take<int>(sorted ? (size_t)nsub * (K + 1) : 1);
     w.totals = c.take<int>(sorted ? (size_t)nprob * (K + 1) : 1);
     w.offs = c.take<int>(sorted ? (size_t)nprob * (K + 1) : 1);
-    w.cmax = c.take<float>((size_t)nprob + 8);
     w.err = c.take<int>(8);
     w.total = align_up(c.off, 256);
     w.ok = c.ok();
@@ -630,16 +427,8 @@ int64_t kmeans_workspace_bytes(int64_t n_total, int nprob, int K, int D) {
 
 template <int D>
 static void launch_assign(const float* X, const float* C, int* labels, const KmProb* probs, int nprob, int K,
-                          int tiles, const float* cmax, bool prefilter, cudaStream_t st) {
+                          int tiles, cudaStream_t st) {
     constexpr int P = PointsPerThread<D>::value;
-    if constexpr (D >= 9) {
-        if (prefilter && cmax) {
-            k_kmeans_cmax<<<nprob, 256, 0, st>>>(C, K, D, const_cast<float*>(cmax));
-            count_launch();
-            k_kmeans_assign_pre<D, P><<<tiles, kAssignThreads, 0, st>>>(X, C, labels, probs, nprob, K, cmax);
-            return;
-        }
-    }
     k_kmeans_assign<D, P><<<tiles, kAssignThreads, 0, st>>>(X, C, labels, probs, nprob, K);
 }
 
@@ -660,14 +449,14 @@ int kmeans_lloyd(const float* X, const int64_t* row_off, int nprob, int K, int D
                  int* counts, void* ws, int64_t ws_bytes, int assign_mode, unsigned long long* tc_stats,
                  cudaStream_t st) {
     GSX_NVTX("gsx::kmeans_lloyd");
-    GSX_REQUIRE(assign_mode >= 0 && assign_mode <= 4, GSX_ERR_ARG, "kmeans: bad assign_mode %d", assign_mode);
-    if (assign_mode == GSX_KM_ASSIGN_TENSOR || assign_mode == GSX_KM_ASSIGN_TENSOR_BF16)
+    GSX_REQUIRE(assign_mode == GSX_KM_ASSIGN_AUTO || assign_mode == GSX_KM_ASSIGN_STRICT ||
+                    assign_mode == GSX_KM_ASSIGN_TENSOR,
+                GSX_ERR_ARG, "kmeans: bad assign_mode %d", assign_mode);
+    if (assign_mode == GSX_KM_ASSIGN_TENSOR)
         GSX_REQUIRE(kmeans_tc_supported(K, D), GSX_ERR_UNSUPPORTED,
                     "kmeans: tensor-core assign needs D in {9,24,45} and K <= 256 (got K=%d D=%d)", K, D);
-    const bool use_tc = assign_mode == GSX_KM_ASSIGN_TENSOR || assign_mode == GSX_KM_ASSIGN_TENSOR_BF16 ||
+    const bool use_tc = assign_mode == GSX_KM_ASSIGN_TENSOR ||
                         (assign_mode == GSX_KM_ASSIGN_AUTO && kmeans_tc_supported(K, D));
-    const int tc_variant = assign_mode == GSX_KM_ASSIGN_TENSOR_BF16 ? 2 : 0;   // 0: TF32, the only variant built
-    const bool prefilter = assign_mode == GSX_KM_ASSIGN_FMA_PREFILTER;
     GSX_REQUIRE(nprob >= 1 && K >= 1 && D >= 1 && max_iter >= 0, GSX_ERR_ARG, "kmeans: bad shape");
     const int64_t n_total = row_off[nprob] - row_off[0];
     GSX_REQUIRE(row_off[0] == 0, GSX_ERR_ARG, "kmeans: row_off[0] must be 0");
@@ -707,18 +496,18 @@ int kmeans_lloyd(const float* X, const int64_t* row_off, int nprob, int K, int D
     if (use_tc) GSX_CUDA_CHECK(cudaMemsetAsync(w.err, 0, sizeof(int), st));
     for (int it = 0; it < max_iter; ++it) {
         if (use_tc) {
-            int rc = kmeans_assign_tc(X, (long long)n_total * D, C, labels, dp, nprob, K, D, tc_tiles, tc_variant, 0, nullptr,
+            int rc = kmeans_assign_tc(X, (long long)n_total * D, C, labels, dp, nprob, K, D, tc_tiles, 0, nullptr,
                                       tc_stats, w.err, st);
             if (rc) return rc;
         } else
         switch (D) {
-            case 1: launch_assign<1>(X, C, labels, dp, nprob, K, (int)tiles, w.cmax, prefilter, st); break;
-            case 2: launch_assign<2>(X, C, labels, dp, nprob, K, (int)tiles, w.cmax, prefilter, st); break;
-            case 3: launch_assign<3>(X, C, labels, dp, nprob, K, (int)tiles, w.cmax, prefilter, st); break;
-            case 4: launch_assign<4>(X, C, labels, dp, nprob, K, (int)tiles, w.cmax, prefilter, st); break;
-            case 9: launch_assign<9>(X, C, labels, dp, nprob, K, (int)tiles, w.cmax, prefilter, st); break;
-            case 24: launch_assign<24>(X, C, labels, dp, nprob, K, (int)tiles, w.cmax, prefilter, st); break;
-            case 45: launch_assign<45>(X, C, labels, dp, nprob, K, (int)tiles, w.cmax, prefilter, st); break;
+            case 1: launch_assign<1>(X, C, labels, dp, nprob, K, (int)tiles, st); break;
+            case 2: launch_assign<2>(X, C, labels, dp, nprob, K, (int)tiles, st); break;
+            case 3: launch_assign<3>(X, C, labels, dp, nprob, K, (int)tiles, st); break;
+            case 4: launch_assign<4>(X, C, labels, dp, nprob, K, (int)tiles, st); break;
+            case 9: launch_assign<9>(X, C, labels, dp, nprob, K, (int)tiles, st); break;
+            case 24: launch_assign<24>(X, C, labels, dp, nprob, K, (int)tiles, st); break;
+            case 45: launch_assign<45>(X, C, labels, dp, nprob, K, (int)tiles, st); break;
             default:
                 k_kmeans_assign_generic<<<(int)tiles, kAssignThreads, 0, st>>>(X, C, labels, dp, nprob, K, D);
         }
@@ -750,7 +539,7 @@ int kmeans_lloyd(const float* X, const int64_t* row_off, int nprob, int K, int D
 }
 
 // debug / test hook: raw tensor-core scores of the first 128 rows against K centroids (one problem)
-int kmeans_tc_debug_scores(const float* X, int64_t rows, const float* C, int K, int D, int variant, float* scores,
+int kmeans_tc_debug_scores(const float* X, int64_t rows, const float* C, int K, int D, float* scores,
                            void* ws, int64_t ws_bytes, cudaStream_t st) {
     GSX_REQUIRE(kmeans_tc_supported(K, D) && rows >= 1, GSX_ERR_UNSUPPORTED, "kmeans_tc_debug: unsupported shape");
     GSX_REQUIRE(ws_bytes >= 1024, GSX_ERR_WORKSPACE, "kmeans_tc_debug: workspace too small");
@@ -761,7 +550,7 @@ int kmeans_tc_debug_scores(const float* X, int64_t rows, const float* C, int K, 
     GSX_CUDA_CHECK(cudaMemcpyAsync(dp, &hp, sizeof(hp), cudaMemcpyHostToDevice, st));
     GSX_CUDA_CHECK(cudaMemsetAsync(err, 0, sizeof(int), st));
     GSX_CUDA_CHECK(cudaStreamSynchronize(st));
-    int rc = kmeans_assign_tc(X, (long long)rows * D, C, nullptr, dp, 1, K, D, (rows + 127) / 128, variant, 1, scores,
+    int rc = kmeans_assign_tc(X, (long long)rows * D, C, nullptr, dp, 1, K, D, (rows + 127) / 128, 1, scores,
                               nullptr, err, st);
     if (rc) return rc;
     GSX_KERNEL_CHECK();

@@ -1,11 +1,6 @@
 #pragma once
 #include "gsx_common.cuh"
-
-#define GSX_KM_ASSIGN_AUTO 0
-#define GSX_KM_ASSIGN_STRICT 1
-#define GSX_KM_ASSIGN_FMA_PREFILTER 2
-#define GSX_KM_ASSIGN_TENSOR 3
-#define GSX_KM_ASSIGN_TENSOR_BF16 4
+#include "../../include/gsx.h"
 
 namespace gsx {
 
@@ -23,10 +18,9 @@ int kmeans_lloyd(const float* X, const int64_t* row_off, int nprob, int K, int D
                  cudaStream_t st);
 // gsx_kmeans_tc.cu
 bool kmeans_tc_supported(int K, int D);
-bool kmeans_tc16_built();
 int kmeans_assign_tc(const float* X, long long x_floats, const float* C, int* labels, const KmProb* probs_dev, int nprob,
-                     int K, int D, long long tiles, int variant, int mode, float* dump, unsigned long long* stats,
+                     int K, int D, long long tiles, int mode, float* dump, unsigned long long* stats,
                      int* err_flag_dev, cudaStream_t st);
-int kmeans_tc_debug_scores(const float* X, int64_t rows, const float* C, int K, int D, int variant, float* scores,
+int kmeans_tc_debug_scores(const float* X, int64_t rows, const float* C, int K, int D, float* scores,
                            void* ws, int64_t ws_bytes, cudaStream_t st);
 }

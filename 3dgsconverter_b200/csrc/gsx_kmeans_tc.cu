@@ -443,18 +443,11 @@ static int launch_tc_n(const float* X, long long x_floats, const float* C, int* 
     return launch_tc<D, KP, 4>(X, x_floats, C, labels, probs, nprob, K, tiles, mode, dump, stats, err, st);
 }
 
-// The split-bf16 variant (variant 2) is not part of this library.
-bool kmeans_tc16_built() { return false; }
-
 bool kmeans_tc_supported(int K, int D) { return (D == 9 || D == 24 || D == 45) && K >= 1 && K <= kTcMaxN; }
 
 int kmeans_assign_tc(const float* X, long long x_floats, const float* C, int* labels, const KmProb* probs_dev, int nprob,
-                     int K, int D, long long tiles, int variant, int mode, float* dump, unsigned long long* stats,
+                     int K, int D, long long tiles, int mode, float* dump, unsigned long long* stats,
                      int* err_flag_dev, cudaStream_t st) {
-    if (variant != 0) {
-        set_error("kmeans_tc: only the TF32 variant (0) is built, got %d", variant);
-        return GSX_ERR_UNSUPPORTED;
-    }
     switch (D) {
         case 9: return launch_tc_n<9, 16>(X, x_floats, C, labels, probs_dev, nprob, K, tiles, mode, dump, stats, err_flag_dev, st);
         case 24: return launch_tc_n<24, 32>(X, x_floats, C, labels, probs_dev, nprob, K, tiles, mode, dump, stats, err_flag_dev, st);

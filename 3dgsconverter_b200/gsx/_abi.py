@@ -89,7 +89,7 @@ _SIGS = {
     "gsx_kmeans_lloyd_device": (C.c_int, [_vp, C.POINTER(_i64), _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _i64,
                                           _i32, _vp, _vp]),
     "gsx_kmeans_tensor_core_supported": (_i32, [_i32, _i32]),
-    "gsx_kmeans_tc_debug_scores": (C.c_int, [_vp, _i64, _vp, _i32, _i32, _i32, _vp, _vp, _i64, _vp]),
+    "gsx_kmeans_tc_debug_scores": (C.c_int, [_vp, _i64, _vp, _i32, _i32, _vp, _vp, _i64, _vp]),
     "gsx_kmeans_host": (C.c_int, [_vp, _i64, _i32, _i32, _i32, _vp, _vp, _i32]),
     "gsx_kmeans_host_batched": (C.c_int, [_vp, C.POINTER(_i64), _i32, _i32, _i32, _i32, _vp, _vp, _i32]),
     "gsx_records_extract_xyz_opacity": (C.c_int, [_vp, _i64, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _vp]),
@@ -133,7 +133,7 @@ for _name, (_res, _args) in _SIGS.items():
     _fn.argtypes = _args
 
 HASH_MODES = {"i32wrap": 0, "i64": 1}
-KM_ASSIGN = {"auto": 0, "strict": 1, "fma": 2, "tensor": 3, "tensor_bf16": 4}
+KM_ASSIGN = {"auto": 0, "strict": 1, "tensor": 3}
 
 
 def check(rc: int, what: str = ""):

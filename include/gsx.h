@@ -273,32 +273,27 @@ int gsx_sog_centroids(const float* palette_dev, int64_t P, int32_t coeffs, const
  * One call = max_iter x (assign ; update) with the serial index-order float32 sums of SURVEY A.5.
  * labels are those of the last assign (one update behind C, SURVEY F9); counts int32[nprob*K]. */
 int64_t gsx_kmeans_workspace_bytes(int64_t n_total, int32_t nprob, int32_t K, int32_t D);
-/* assign_mode (per call; the labels are bit-identical in every mode):
- *   AUTO           tensor cores when the shape allows it (gsx_kmeans_tensor_core_supported), else STRICT
- *   STRICT         the contract's distance for every (point, centroid) on the FP32 pipes
- *   FMA_PREFILTER  D >= 9: one fma per (point, centroid, dim) scores every centroid, the strict distance is
- *                  evaluated only for the centroids within a proven rounding-error margin of the best score
- *   TENSOR         the same scheme with the score matrix X.C^T - ||c||^2/2 computed by wgmma.mma_async (TF32, float32
- *                  accumulators in registers, two-pass epilogue: row maximum, candidate mask); error if the shape is
- *                  unsupported (D in {9,24,45}, K <= 256)
- *   TENSOR_BF16    a split-bf16 variant of TENSOR that this library does not build: returns GSX_ERR_UNSUPPORTED
- *                  (gsx_kmeans_tensor_core_supported never reports bit 1)
+/* assign_mode (per call; the labels are bit-identical in every mode; any other value is GSX_ERR_ARG):
+ *   AUTO    tensor cores when the shape allows it (gsx_kmeans_tensor_core_supported), else STRICT
+ *   STRICT  the contract's distance for every (point, centroid) on the FP32 pipes
+ *   TENSOR  the score matrix X.C^T - ||c||^2/2 computed by wgmma.mma_async (TF32, float32 accumulators in registers,
+ *           two-pass epilogue: row maximum, candidate mask), then the contract's distance only for the centroids
+ *           within a proven rounding-error margin of the best score; error if the shape is unsupported
+ *           (D in {9,24,45}, K <= 256)
  * tc_stats_dev (may be NULL): 3 uint64 counters accumulated by the TENSOR path {strict distance evaluations,
  * points with more than one candidate, points that needed the full strict scan}. */
 #define GSX_KM_ASSIGN_AUTO 0
 #define GSX_KM_ASSIGN_STRICT 1
-#define GSX_KM_ASSIGN_FMA_PREFILTER 2
 #define GSX_KM_ASSIGN_TENSOR 3
-#define GSX_KM_ASSIGN_TENSOR_BF16 4
 int gsx_kmeans_lloyd_device(const float* X_dev, const int64_t* row_off_host, int32_t nprob, int32_t K, int32_t D,
                             int32_t max_iter, float* C_dev, int32_t* labels_dev, int32_t* counts_dev, void* ws,
                             int64_t ws_bytes, int32_t assign_mode, unsigned long long* tc_stats_dev, void* stream);
-/* 0: shape unsupported; bit 0: the TF32 kernel takes it; bit 1: the split-bf16 variant is compiled in */
+/* 1 if the TENSOR assign takes this shape, else 0 */
 int32_t gsx_kmeans_tensor_core_supported(int32_t K, int32_t D);
 /* Test hook of the tensor-core assign: raw scores s[r][c] = x_r.c - ||c||^2/2 of the first min(rows,128) rows
  * against the K centroids, scores_dev float32[128 * roundup32(K)].  ws >= 1024 bytes. */
 int gsx_kmeans_tc_debug_scores(const float* X_dev, int64_t rows, const float* C_dev, int32_t K, int32_t D,
-                               int32_t variant, float* scores_dev, void* ws, int64_t ws_bytes, void* stream);
+                               float* scores_dev, void* ws, int64_t ws_bytes, void* stream);
 /* Single problem on HOST buffers: binding target for gpu_ops.kmeans on the GPU path (gpu_ops.py:178-191)
  * with the init centroids chosen by the caller (the reference's np.random.choice draw). */
 int gsx_kmeans_host(const float* X_host, int64_t n, int32_t K, int32_t D, int32_t max_iter, float* C_host_inout,

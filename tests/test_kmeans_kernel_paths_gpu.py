@@ -12,12 +12,12 @@ kinds of test:
 
 Constants these cases are built around (csrc/gsx_kmeans.cu, csrc/gsx_kmeans_tc.cu): strict assign 128 threads x P
 points (P = 4 for D <= 4, 2 for D in {9, 24, 45}; any other D runs the generic one-point-per-thread kernel), centroids
-staged 64 at a time and scored in pairs (an odd tail pairs with a zero row); the fma prefilter (D >= 9 only) scores
-four at a time; the tensor-core kernel takes 128-row tiles, D in {9, 24, 45} and K <= 256, in NB = 1, 2 or 4 blocks of
-64 columns whose padding columns get the bias -3e38, and bulk-copies a tile only when X is 16-byte aligned and the
-rounded copy stays inside X; the update partitions 1 024-row sub-tiles by label for K <= 2047 (per-warp counters of
-8 (K+1) ints, opted in above 48 KiB) and scans labels per cluster above that; `k_km_accum` adds 32-row batches, then a
-ragged tail; strict '<', lowest index on ties, 1e20 "no label" sentinel, empty clusters collapse to 0.
+staged 64 at a time and scored in pairs (an odd tail pairs with a zero row); the tensor-core kernel takes 128-row
+tiles, D in {9, 24, 45} and K <= 256, in NB = 1, 2 or 4 blocks of 64 columns whose padding columns get the bias -3e38,
+and bulk-copies a tile only when X is 16-byte aligned and the rounded copy stays inside X; the update partitions
+1 024-row sub-tiles by label for K <= 2047 (per-warp counters of 8 (K+1) ints, opted in above 48 KiB) and scans labels
+per cluster above that; `k_km_accum` adds 32-row batches, then a ragged tail; strict '<', lowest index on ties, 1e20
+"no label" sentinel, empty clusters collapse to 0.
 """
 import functools
 
@@ -45,7 +45,7 @@ def dispatch(mode, K, D):
         nb = 1 if K <= 64 else 2 if K <= 128 else 4
     elif D in FIXED_D:
         P = 4 if D <= 4 else 2
-        kernel, tile, nb = ("pre" if mode == "fma" and D >= 9 else "strict"), THREADS * P, None
+        kernel, tile, nb = "strict", THREADS * P, None
     else:
         kernel, P, tile, nb = "generic", 1, THREADS, None
     sorted_update = K <= MAX_SORT_K
@@ -54,7 +54,7 @@ def dispatch(mode, K, D):
 
 
 def modes_for(K, D):
-    return ("strict", "fma", "auto") + (("tensor",) if tc_supported(K, D) else ())
+    return ("strict", "auto") + (("tensor",) if tc_supported(K, D) else ())
 
 
 def tc_bulk_tiles(n_floats_before, offs, D, x_aligned=True):
@@ -424,7 +424,7 @@ def test_tc_k_sweep(D, geometry, cuda, gsx_lib):
         _check(globals()[geometry], (D, K), 2, cuda)
 
 
-# ================================================================================================ strict / fma sweep
+# ================================================================================================ strict sweep
 SWEEP_D = (1, 2, 3, 4, 9, 24, 45, 5, 7, 46, 64, 65, 100)
 SWEEP_K = (1, 2, 3, 63, 64, 65, 127, 257)
 
@@ -433,20 +433,17 @@ def test_strict_fma_sweep_dispatch():
     kernels = {}
     for D in SWEEP_D:
         for K in SWEEP_K:
-            s, f = dispatch("strict", K, D), dispatch("fma", K, D)
+            s = dispatch("strict", K, D)
             kernels.setdefault(s["kernel"], set()).add(D)
-            kernels.setdefault(f["kernel"], set()).add(D)
             if D <= 4:
-                assert s == f and s["kernel"] == "strict" and s["P"] == 4 and s["tile"] == 512   # fma has no effect
+                assert s["kernel"] == "strict" and s["P"] == 4 and s["tile"] == 512
             elif D in TC_KP:
-                assert s["kernel"] == "strict" and f["kernel"] == "pre" and s["tile"] == 256
+                assert s["kernel"] == "strict" and s["P"] == 2 and s["tile"] == 256
             else:
-                assert s == f and s["kernel"] == "generic" and s["tile"] == 128
-    assert kernels["strict"] == {1, 2, 3, 4, 9, 24, 45} and kernels["pre"] == {9, 24, 45}
-    assert kernels["generic"] == {5, 7, 46, 64, 65, 100}
+                assert s["kernel"] == "generic" and s["P"] == 1 and s["tile"] == 128
+    assert kernels == {"strict": {1, 2, 3, 4, 9, 24, 45}, "generic": {5, 7, 46, 64, 65, 100}}
     assert max(kernels["generic"]) > 64                                  # a second 64-dim strip in the update
     assert {K % CENT_TILE for K in SWEEP_K if K % 2} >= {1, 3, 63}       # odd tails: pair with a zero row
-    assert {K % 4 for K in SWEEP_K} == {0, 1, 2, 3}                      # every prefilter tail of 4
 
 
 @pytest.mark.parametrize("D", SWEEP_D)
@@ -461,9 +458,9 @@ def test_far_geometry_for_odd_k(D):
 @pytest.mark.parametrize("D", SWEEP_D)
 def test_strict_fma_sweep(D, cuda, gsx_lib):
     for K in SWEEP_K:
-        _check(clustered, (3001, D, K, 4000 * D + K), 2, cuda, modes=("strict", "fma", "auto"))
+        _check(clustered, (3001, D, K, 4000 * D + K), 2, cuda, modes=("strict", "auto"))
         if K % 2:
-            _check(far_centroids, (3001, D, K, 3000 * D + K), 1, cuda, modes=("strict", "fma", "auto"))
+            _check(far_centroids, (3001, D, K, 3000 * D + K), 1, cuda, modes=("strict", "auto"))
 
 
 # ================================================================================================ update forms
@@ -743,6 +740,16 @@ def test_subnormal_rows(D, cuda, gsx_lib):
 
 
 # ================================================================================================ API edges
+def test_only_auto_strict_tensor_are_assign_modes(gsx_lib):
+    """AUTO (0), STRICT (1) and TENSOR (3) are the assign modes; any other value is GSX_ERR_ARG (-2), checked before
+    the shape, the workspace or the device."""
+    import ctypes as C
+    off = (C.c_int64 * 2)(0, 1000)
+    for mode in (-1, 2, 4, 5):
+        assert gsx_lib.gsx_kmeans_lloyd_device(None, off, 1, 32, 45, 1, None, None, None, None, 0, mode, None,
+                                               None) == -2, mode
+
+
 @pytest.mark.gpu
 def test_max_iter_zero_returns_init(cuda, gsx_lib):
     import torch
