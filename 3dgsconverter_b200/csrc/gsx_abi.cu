@@ -14,6 +14,7 @@
 #include "gsx_knn_exact.cuh"
 #include "gsx_masks.cuh"
 #include "gsx_morton.cuh"
+#include "gsx_ply.cuh"
 #include "gsx_radix.cuh"
 #include "gsx_readers.cuh"
 #include "gsx_records.cuh"
@@ -670,6 +671,10 @@ int gsx_cply_decode(const uint8_t* chunk_dev, int64_t nchunk, int32_t chunk_row,
                     const float* tables_dev, uint8_t* rows_dev, void* stream) {
     return cply_decode(chunk_dev, nchunk, chunk_row, chunk_offs_host, vertex_dev, n, vertex_row, vertex_offs_host, sh_dev,
                        sh_row, sh_offs_host, nsh, tables_dev, rows_dev, (cudaStream_t)stream);
+}
+int gsx_ply_transcode(const uint8_t* src_dev, int64_t n, int32_t src_row_bytes, uint8_t* dst_dev, int32_t dst_row_bytes,
+                      const int32_t* fields_host, int32_t nfields, void* stream) {
+    return ply_transcode(src_dev, n, src_row_bytes, dst_dev, dst_row_bytes, fields_host, nfields, (cudaStream_t)stream);
 }
 int gsx_sog_decode_palette(const uint8_t* centroids_dev, int64_t palette_size, int32_t coeffs, const float* codebook_dev,
                            int32_t codebook_len, float* palette_dev, int32_t* error_dev, void* stream) {

@@ -118,7 +118,8 @@ _SIGS = {
     "gsx_spz_decode": (C.c_int, [_vp, _i64, _i32, _i32, _i32, _vp, _i32, _vp, _vp]),
     "gsx_cply_decode": (C.c_int, [_vp, _i64, _i32, C.POINTER(_i32), _vp, _i64, _i32, C.POINTER(_i32), _vp, _i32,
                                   C.POINTER(_i32), _i32, _vp, _vp, _vp]),
-    "gsx_sog_decode_palette": (C.c_int, [_vp, _i64, _i32, _vp, _i32, _vp, _vp, _vp]),
+    "gsx_ply_transcode": (C.c_int, [_vp, _i64, _i32, _vp, _i32, C.POINTER(_i32), _i32, _vp]),
+    "gsx_sog_decode_palette":(C.c_int, [_vp, _i64, _i32, _vp, _i32, _vp, _vp, _vp]),
     "gsx_sog_decode": (C.c_int, [C.POINTER(_vp), _i64, _vp, _vp, _i32, _i32, _vp, _i64, _i32, _vp, _vp, _vp]),
     "gsx_copy_h2d": (C.c_int, [_vp, _vp, _i64, _vp]),
     "gsx_copy_d2h": (C.c_int, [_vp, _vp, _i64, _vp]),

@@ -102,29 +102,38 @@ def encode(records, order: torch.Tensor | None = None) -> CompressedPly:
     return CompressedPly(chunk, vertex, sh, names, order)
 
 
-_PLY_TYPES = {("f", 4): ("float", "<f4"), ("u", 4): ("uint", "<u4"), ("u", 1): ("uchar", "u1")}
+PLY_TYPE_NAMES = {("i", 1): "char", ("u", 1): "uchar", ("i", 2): "short", ("u", 2): "ushort", ("i", 4): "int",
+                  ("u", 4): "uint", ("f", 4): "float", ("f", 8): "double"}
+
+
+def ply_header(elements) -> tuple[bytes, list]:
+    """(header, layouts) of a binary little-endian PLY with `elements` = [(name, count, dtype)]: the text plyfile's
+    PlyData(elements, byte_order='<').write emits, restated here because plyfile is not a dependency of gsx
+    (property type names char uchar short ushort int uint float double), and each element's packed little-endian row
+    dtype.  Raises ValueError for a field type plyfile does not write (bool, 8-byte integers, sub-arrays, ...)."""
+    lines = ["ply", "format binary_little_endian 1.0"]
+    layouts = []
+    for name, count, dtype in elements:
+        lines.append(f"element {name} {count}")
+        fields = []
+        for f in dtype.names:
+            dt = dtype.fields[f][0]
+            if dt.shape or (dt.kind, dt.itemsize) not in PLY_TYPE_NAMES:
+                raise ValueError(f"{name}.{f}: unsupported PLY property type {dt}")
+            lines.append(f"property {PLY_TYPE_NAMES[(dt.kind, dt.itemsize)]} {f}")
+            fields.append((f, f"<{dt.kind}{dt.itemsize}"))
+        layouts.append(np.dtype(fields))
+    lines.append("end_header")
+    return ("\n".join(lines) + "\n").encode("ascii"), layouts
 
 
 def write_ply(path, chunk_data: np.ndarray, vertex_data: np.ndarray, sh_data: np.ndarray | None = None) -> None:
     """Binary little-endian PLY with the elements chunk, vertex and (if given) sh -- what _write_ply_file writes through
     plyfile (compressed_ply.py:380-385), for users of gsx without plyfile."""
     elements = [("chunk", chunk_data), ("vertex", vertex_data)] + ([("sh", sh_data)] if sh_data is not None else [])
-    lines = ["ply", "format binary_little_endian 1.0"]
-    layouts = []
-    for name, a in elements:
-        lines.append(f"element {name} {len(a)}")
-        fields = []
-        for f in a.dtype.names:
-            dt = a.dtype.fields[f][0]
-            if (dt.kind, dt.itemsize) not in _PLY_TYPES:
-                raise ValueError(f"{name}.{f}: unsupported PLY property type {dt}")
-            ply_type, np_type = _PLY_TYPES[(dt.kind, dt.itemsize)]
-            lines.append(f"property {ply_type} {f}")
-            fields.append((f, np_type))
-        layouts.append(np.dtype(fields))
-    lines.append("end_header")
+    header, layouts = ply_header([(name, len(a), a.dtype) for name, a in elements])
     with open(path, "wb") as fh:
-        fh.write(("\n".join(lines) + "\n").encode("ascii"))
+        fh.write(header)
         for (_, a), layout in zip(elements, layouts):
             fh.write(np.ascontiguousarray(a.astype(layout)).tobytes())
 

@@ -19,8 +19,10 @@ device, gzip and the file on the host; records gsx refuses go to the original ``
 host, every splat decoded on the device, byte for byte as the reference readers; files gsx refuses go to the original
 ``read``).  With ``patch(sog_reader="device")`` also ``SogFormat.read`` (gsx.sog_reader.decode: ZIP, meta.json and
 WebP on the host, the shN palette and every splat decoded on the device, byte for byte as the reference reader, its
-palette indexing included; bundles gsx refuses go to the original ``read``).  The parquet and plain PLY readers stay
-on the host.
+palette indexing included; bundles gsx refuses go to the original ``read``).  With ``patch(ply="device")`` also the
+``read`` and ``write`` of ``Ply3DGSFormat`` and ``PlyCCFormat`` (gsx.ply: header and field mapping on the host, the rows
+transcoded on the device, byte for byte as the reference; files and records gsx refuses, and writes with
+``extra_elements``, go to the original method).  The parquet reader and writer stay on the host.
 Host-only helpers and everything else of the reference stay as they are.
 """
 from __future__ import annotations
@@ -61,7 +63,7 @@ class _GsxCodebookKMeans:
 
 
 def patch(verbose: bool = False, defer: bool = True, codebook: str = "sklearn", require_cuda: bool = True,
-          sog: str = "host", codecs: str = "host", readers: str = "host", sog_reader: str = "host"):
+          sog: str = "host", codecs: str = "host", readers: str = "host", sog_reader: str = "host", ply: str = "host"):
     """require_cuda: refuse (return False, leave the reference untouched) when no CUDA device is usable, so that a
     CPU-only host keeps the reference's own SciPy / scikit-learn paths (there is no CPU fallback inside gsx).
     sog: "host" keeps the reference's SogFormat.write (with the patched gpu_ops.kmeans and its batch-ahead);
@@ -71,7 +73,9 @@ def patch(verbose: bool = False, defer: bool = True, codebook: str = "sklearn", 
     readers: "host" keeps the reference's .splat / .ksplat / .spz / compressed PLY readers; "device" installs gsx's
     device readers on them (files gsx refuses go to the original read).
     sog_reader: "host" keeps the reference's SogFormat.read; "device" installs gsx.sog_reader's device reader on it
-    (bundles gsx refuses go to the original read)."""
+    (bundles gsx refuses go to the original read).
+    ply: "host" keeps the reference's plain 3DGS and CloudCompare PLY read and write; "device" installs gsx.ply's device
+    reader and writer on Ply3DGSFormat and PlyCCFormat (files and records gsx refuses go to the original method)."""
     if sog not in ("host", "device"):
         raise ValueError(f"sog must be 'host' or 'device', not {sog!r}")
     if codecs not in ("host", "device"):
@@ -80,6 +84,8 @@ def patch(verbose: bool = False, defer: bool = True, codebook: str = "sklearn", 
         raise ValueError(f"readers must be 'host' or 'device', not {readers!r}")
     if sog_reader not in ("host", "device"):
         raise ValueError(f"sog_reader must be 'host' or 'device', not {sog_reader!r}")
+    if ply not in ("host", "device"):
+        raise ValueError(f"ply must be 'host' or 'device', not {ply!r}")
     if require_cuda:
         from . import backend_available
         if not backend_available():
@@ -168,6 +174,18 @@ def patch(verbose: bool = False, defer: bool = True, codebook: str = "sklearn", 
             if hasattr(fmt, clsname):
                 ours.install_reader(getattr(fmt, clsname))   # splat.py:9-80, ksplat.py:29-317, spz.py:18-296,
                 #                                               compressed_ply.py:14-123
+    if ply == "device":
+        from . import ply as gply
+        for modname, clsname, flavor in (("ply_3dgs", "Ply3DGSFormat", "3dgs"), ("ply_cc", "PlyCCFormat", "cc")):
+            fmt = sys.modules.get(f"gsconverter.formats.{modname}")
+            if fmt is None:
+                try:
+                    fmt = importlib.import_module(f"gsconverter.formats.{modname}")
+                except Exception:  # noqa: BLE001  (plyfile missing: nothing to patch there)
+                    continue
+            if hasattr(fmt, clsname):
+                gply.install_reader(getattr(fmt, clsname), flavor)   # ply_3dgs.py:8-60, ply_cc.py:8-62
+                gply.install(getattr(fmt, clsname), flavor)          # ply_3dgs.py:62-121, ply_cc.py:64-132
     if verbose:
         print("[gsx] gsconverter.processing patched: SOR / density / bbox / alpha / K-Means / compressed PLY packing "
               "run on libgsx.so")

@@ -459,6 +459,17 @@ int gsx_cply_decode(const uint8_t* chunk_dev, int64_t nchunk, int32_t chunk_row,
  *   > 3; f_rest = palette_dev[R | G << 8 of the labels].  n < 2^31. */
 int gsx_sog_decode_palette(const uint8_t* centroids_dev, int64_t palette_size, int32_t coeffs, const float* codebook_dev,
                            int32_t codebook_len, float* palette_dev, int32_t* error_dev, void* stream);
+/* gsx_ply_transcode: the field mapping of the plain PLY readers and writers (formats/ply_3dgs.py:44-58 and :103-109,
+ * formats/ply_cc.py:44-60 and :111-116: `converted[t] = vertices[s]`, `output_data[o] = data[f]` into np.zeros rows).
+ * n rows of src_row_bytes bytes at src_dev -> n rows of dst_row_bytes bytes at dst_dev, both contiguous, any alignment,
+ * rows of 1 .. 1024 bytes, n < 2^31.  fields_host int32 [nfields][4] = {src_off, src_type, dst_off, dst_type}, types
+ * numbered 0 char (i1), 1 uchar (u1), 2 short, 3 ushort, 4 int, 5 uint, 6 float (f4), 7 double (f8); destination
+ * bytes no field writes are 0 (the zero fill), fields may not overlap in the destination.  Casts as NumPy's structured
+ * assignment on x86: identity (bytes copied); integer -> float round to nearest; double -> float round to nearest with
+ * x86's NaN rule; integer -> uchar the low byte; float or double -> uchar the low byte of the truncation to int32, 0
+ * for NaN and out-of-range values.  Other pairings are refused (GSX_ERR_ARG). */
+int gsx_ply_transcode(const uint8_t* src_dev, int64_t n, int32_t src_row_bytes, uint8_t* dst_dev, int32_t dst_row_bytes,
+                      const int32_t* fields_host, int32_t nfields, void* stream);
 int gsx_sog_decode(const uint8_t* const* textures_host, int64_t n, const float* position_tables_dev,
                    const float* tables_dev, int32_t scale_codebook_len, int32_t sh0_codebook_len,
                    const float* palette_dev, int64_t palette_size, int32_t coeffs, uint8_t* rows_dev, int32_t* error_dev,
