@@ -6,7 +6,7 @@
 //
 // Design (GPU-first, not a translation of the Taichi kernel):
 //   * grid build entirely on device: min/max reduce -> 64-bit key (bucket hash << 15 |
-//     5+5+5-bit Morton code of the position inside the cell) -> radix sort -> float4
+//     5+5+5-bit Hilbert code of the position inside the cell) -> radix sort -> float4
 //     gather (w carries the original index, so the "unsort" is fused into the query
 //     kernel) -> {start,end} bucket table -> bounding boxes of every aligned run of 32
 //     ("chunk") and 1024 ("super") sorted points.
@@ -40,9 +40,9 @@ namespace gsx {
 #define GSX_D2LIM_BITS 0x60ad78ebu
 #define GSX_FULL 0xffffffffu
 
-constexpr int kMortonBits = 15;       // in-cell Morton code: kMortonBits/3 bits per axis
-constexpr float kMortonScale = (float)(1 << (kMortonBits / 3));
-constexpr float kMortonMax = kMortonScale - 1.f;
+constexpr int kCellCodeBits = 15;     // in-cell Hilbert code: kCellCodeBits/3 bits per axis
+constexpr float kCellCodeScale = (float)(1 << (kCellCodeBits / 3));
+constexpr float kCellCodeMax = kCellCodeScale - 1.f;
 // tuning constants of the query kernel (kSmallBucket also bounds the serial walk of k_sor_bucket_tail)
 constexpr int kSmallBucket = 64;      // buckets up to this size are scanned without box tests
 constexpr int kQueryBatch = 16;       // consecutive queries grabbed per warp
@@ -54,9 +54,10 @@ constexpr int kFlatSupers = 8;
 // names the query kernel's tuning constants in every bench line (gsx_build_info).  epi_smem=1 (batched epilogue),
 // first_sort=1 (first merge as a plain sort), knn16=0 (one query per warp for every K), tma=0 (no TMA staging) and
 // i32=1 (32-bit positions) describe fixed properties of the kernel; they stay so that bench lines remain comparable.
+// cell_order=hilbert15 names the build's in-bucket order (15-bit in-cell Hilbert code), which sets the query's scan count.
 const char* sor_build_info() {
     return "knn=r02c;epi_smem=1;first_sort=1;query_batch=16;minblocks=8;merge_threshold=9;small_bucket=64;"
-           "flat_supers=8;knn16=0;tma=0;i32=1";
+           "flat_supers=8;knn16=0;tma=0;i32=1;cell_order=hilbert15";
 }
 
 // ------------------------------------------------------------------ workspace layout
@@ -211,22 +212,42 @@ __device__ __forceinline__ uint32_t bucket_of(float x, float y, float z, float b
     return bucket_hash(x, y, z, bx, by, bz, cell, n, M64, a, b, c, d, e, f);
 }
 
-// sort key: bucket hash << kMortonBits | Morton code of the position inside the cell (ordering only -- the
+// Hilbert index of (x, y, z) in [0, 32)^3 (Skilling's transpose form, then the bits interleaved x first).  Points
+// consecutive in this order are in face-adjacent sub-cells; the Z curve jumps, so a run of 32 Morton-ordered points
+// of a dense bucket straddles far-apart sub-cells and its chunk box is loose (scripts/sor_layout_model.py counts the
+// chunks a query must scan under both orders).  The top 3k bits are the curve at 2^k sub-cells per axis.
+__device__ __forceinline__ uint32_t hilbert15(uint32_t x, uint32_t y, uint32_t z) {
+#pragma unroll
+    for (uint32_t q = 16; q > 1; q >>= 1) {
+        const uint32_t p = q - 1;
+        if (x & q) x ^= p;
+        if (y & q) x ^= p; else { const uint32_t t = (x ^ y) & p; x ^= t, y ^= t; }
+        if (z & q) x ^= p; else { const uint32_t t = (x ^ z) & p; x ^= t, z ^= t; }
+    }
+    y ^= x, z ^= y;
+    uint32_t t = 0;
+#pragma unroll
+    for (uint32_t q = 16; q > 1; q >>= 1)
+        if (z & q) t ^= q - 1;
+    x ^= t, y ^= t, z ^= t;
+    return (spread6(x) << 2) | (spread6(y) << 1) | spread6(z);
+}
+
+// sort key: bucket hash << kCellCodeBits | Hilbert code of the position inside the cell (ordering only -- the
 // in-bucket order never affects results)
 __device__ __forceinline__ uint64_t bucket_key(float x, float y, float z, float bx, float by, float bz, float cell,
                                                int64_t n, uint64_t M64) {
     float fx, fy, fz, flx, fly, flz;
     const uint32_t h = bucket_hash(x, y, z, bx, by, bz, cell, n, M64, fx, fy, fz, flx, fly, flz);
-    uint32_t sx = (uint32_t)fminf(kMortonMax, fmaxf(0.f, (fx - flx) * kMortonScale));
-    uint32_t sy = (uint32_t)fminf(kMortonMax, fmaxf(0.f, (fy - fly) * kMortonScale));
-    uint32_t sz = (uint32_t)fminf(kMortonMax, fmaxf(0.f, (fz - flz) * kMortonScale));
-    uint32_t mort = (spread6(sx) << 2) | (spread6(sy) << 1) | spread6(sz);
-    return ((uint64_t)h << kMortonBits) | (uint64_t)mort;
+    uint32_t sx = (uint32_t)fminf(kCellCodeMax, fmaxf(0.f, (fx - flx) * kCellCodeScale));
+    uint32_t sy = (uint32_t)fminf(kCellCodeMax, fmaxf(0.f, (fy - fly) * kCellCodeScale));
+    uint32_t sz = (uint32_t)fminf(kCellCodeMax, fmaxf(0.f, (fz - flz) * kCellCodeScale));
+    return ((uint64_t)h << kCellCodeBits) | (uint64_t)hilbert15(sx, sy, sz);
 }
 
-// The sort works on ONE 64-bit word per point: [ bucket | Morton (top mort_bits of the kMortonBits code) | index ].
+// The sort works on ONE 64-bit word per point: [ bucket | cell code (top mort_bits of the kCellCodeBits code) | index ].
 // Only the bits above the index are sorted (stable LSD passes => equal keys stay in index order, as with a separate
-// payload), and a pass moves 8 bytes per point instead of 12.  The Morton field takes what is left of the 64 bits
+// payload), and a pass moves 8 bytes per point instead of 12.  The cell-code field takes what is left of the 64 bits
 // after the bucket and the index (15 bits up to 16.7 M points, 9 at 80 M, 3 at 1 B): it only orders points INSIDE a
 // bucket, which never changes a result.
 struct PackFmt {
@@ -248,15 +269,15 @@ static PackFmt pack_fmt(int64_t n_items, int64_t n_buckets) {
     f.idx_bits = bits_for(n_items);
     f.bucket_bits = bits_for(n_buckets);
     int avail = 64 - f.idx_bits - f.bucket_bits;
-    if (avail > kMortonBits) avail = kMortonBits;
+    if (avail > kCellCodeBits) avail = kCellCodeBits;
     f.mort_bits = avail < 0 ? 0 : avail - avail % 3;
     return f;
 }
 
-__device__ __forceinline__ uint64_t pack_word(uint64_t key /* bucket << kMortonBits | morton */, uint64_t bucket_sub,
+__device__ __forceinline__ uint64_t pack_word(uint64_t key /* bucket << kCellCodeBits | cell code */, uint64_t bucket_sub,
                                               int64_t idx, PackFmt f) {
-    const uint64_t bucket = (key >> kMortonBits) - bucket_sub;
-    const uint64_t mort = (key & ((1ull << kMortonBits) - 1ull)) >> (kMortonBits - f.mort_bits);
+    const uint64_t bucket = (key >> kCellCodeBits) - bucket_sub;
+    const uint64_t mort = (key & ((1ull << kCellCodeBits) - 1ull)) >> (kCellCodeBits - f.mort_bits);
     return (((bucket << f.mort_bits) | mort) << f.idx_bits) | (uint64_t)idx;
 }
 
@@ -736,7 +757,7 @@ __global__ void __launch_bounds__(256) k_sor_owner_keys(const float* __restrict_
                                                         uint64_t M64, int idx_bits, uint64_t* __restrict__ keys) {
     int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    uint64_t h = bucket_key(xyz[3 * i], xyz[3 * i + 1], xyz[3 * i + 2], bx, by, bz, cell, n_global, M64) >> kMortonBits;
+    uint64_t h = bucket_key(xyz[3 * i], xyz[3 * i + 1], xyz[3 * i + 2], bx, by, bz, cell, n_global, M64) >> kCellCodeBits;
     // o = floor(h*G/N) satisfies ceil(o*N/G) <= h; it is the owner unless h < ceil(o*N/G) can happen -- it cannot:
     // o*N/G <= h  =>  ceil(o*N/G) <= h because h is an integer.
     keys[i] = (((h * (uint64_t)world) / (uint64_t)n_global) << idx_bits) | (uint64_t)i;   // owner | slab index

@@ -9,7 +9,7 @@ cells hash to arbitrary buckets, so a halo exchange cannot reproduce it (SURVEY 
      one radix pass; ONE all-gather of the G x G count matrix -> send/recv splits and every owner's segment
      size and base (2 host syncs in total -- they size the buffers);
   3. all-to-all of float4 {x, y, z, global index} (16 B/pt, each point crosses NVLink once);
-  4. B: every owner sorts what it received by (bucket, in-cell Morton code) STRAIGHT INTO its slot of the
+  4. B: every owner sorts what it received by (bucket, in-cell Hilbert code) STRAIGHT INTO its slot of the
      global hash-sorted array; the slots are exchanged with one grouped batch of point-to-point sends
      (an all-gather with ragged segment sizes and no staging copy);
   5. C: bucket table, bucket boxes and chunk/super boxes from the sorted array (two streaming passes, replicated);
@@ -144,7 +144,7 @@ class _GsxSorOps:
         return pos4, cuts
 
     def merge_into(self, pos4_r, n_global, bmin, cell, out, flags_out=None, bucket_range=None):
-        """B: sort the received points of this rank's bucket range by (bucket, in-cell Morton) into `out`; with
+        """B: sort the received points of this rank's bucket range by (bucket, in-cell Hilbert code) into `out`; with
         `flags_out` (uint8 per point) also the bucket-start / cell-change flags stage C consumes."""
         import ctypes as C
         from . import sor

@@ -70,7 +70,7 @@ int gsx_sor_build(const float* xyz_dev, int64_t n, const float* bmin_host, float
  *  A. local_run:  stable partition of the slab by bucket owner (one radix pass); outputs float4
  *     {x,y,z, bits(idx_base + local index)} grouped by owner and cuts_dev[G+1] = first position of every owner
  *     -> the caller exchanges the groups (all-to-all).
- *  B. merge:      sorts the m received points of this rank's bucket range [bucket_lo, bucket_hi) by (bucket, in-cell Morton)
+ *  B. merge:      sorts the m received points of this rank's bucket range [bucket_lo, bucket_hi) by (bucket, in-cell Hilbert code)
  *     -> the caller all-gathers the segments in owner order = the globally hash-sorted array.  With flags_sorted_dev
  *     the owner also emits one byte per sorted point (bit 0: starts a bucket, bit 1: other grid cell than the point
  *     before) -- exchanged along with the segment (1 B/pt next to 16 B/pt), it spares every receiving rank the
@@ -114,7 +114,7 @@ int gsx_sor_mean_dists_strided(int64_t n, int32_t stride, int32_t phase, int32_t
 /* gpu_ops.py:227 (np.argsort of the bucket hashes): stable LSD radix sort, in place, of (uint64 key, int32
  * value) pairs on the key bits [begin_bit, end_bit): 8-bit digits, one "onesweep" kernel per digit (decoupled
  * look-back over per-tile digit counts) after a single histogram pass.  vals_dev == NULL sorts bare 64-bit words
- * (n < 2^30): the form the hash-grid build uses, with word = bucket | in-cell Morton code | original index and only the
+ * (n < 2^30): the form the hash-grid build uses, with word = bucket | in-cell Hilbert code | original index and only the
  * bits above the index sorted -- 8 instead of 12 bytes moved per point and pass. */
 int64_t gsx_sort_pairs_workspace_bytes(int64_t n);
 int gsx_sort_pairs(uint64_t* keys_dev, int32_t* vals_dev, int64_t n, int32_t begin_bit, int32_t end_bit, void* ws,
