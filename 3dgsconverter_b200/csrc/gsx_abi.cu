@@ -235,6 +235,17 @@ int gsx_sor_mean_dists(int64_t n, int32_t k, int32_t hash_mode, const float* bmi
                                     stream);
 }
 
+int gsx_sor_query_counters(int64_t n, void* ws, int64_t ws_bytes, unsigned long long* out8_host, void* stream) {
+    SorWs w;
+    int rc = carve_grid_checked(ws, ws_bytes, n, w);
+    if (rc) return rc;
+    GSX_REQUIRE(out8_host != nullptr, GSX_ERR_ARG, "sor: null counter buffer");
+    GSX_CUDA_CHECK(cudaMemcpyAsync(out8_host, w.stats, 8 * sizeof(unsigned long long), cudaMemcpyDeviceToHost,
+                                   (cudaStream_t)stream));
+    GSX_CUDA_CHECK(cudaStreamSynchronize((cudaStream_t)stream));
+    return GSX_OK;
+}
+
 int64_t gsx_mean_std_workspace_bytes(int64_t n) { return (int64_t)mean_std_ws_bytes(n); }
 
 int gsx_mean_std_f32(const float* a_dev, int64_t n, float* out_dev, void* ws, int64_t ws_bytes, void* stream) {

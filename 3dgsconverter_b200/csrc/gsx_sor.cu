@@ -12,7 +12,7 @@
 //     ("chunk") and 1024 ("super") sorted points.
 //   * query kernel: one warp per query, persistent CTAs with a dynamic batch counter.
 //     Lane p<27 evaluates probe p's hash and loads its bucket entry ({start,end}, and the 32-byte box if non-empty);
-//     the probes are visited nearest box first (redux.min on the lower bound) and dropped once
+//     the probes are visited nearest box first (one redux.min on lower bound | lane, see knn_key) and dropped once
 //     lb >= tau; candidates are streamed 32 at a time with one coalesced float4 load per lane;
 //     the K best d^2 live one per lane in a register (two for K>32) and are maintained with
 //     ballot + shfl insertion or a bitonic merge.
@@ -46,7 +46,10 @@ constexpr float kCellCodeMax = kCellCodeScale - 1.f;
 // tuning constants of the query kernel (kSmallBucket also bounds the serial walk of k_sor_bucket_tail)
 constexpr int kSmallBucket = 64;      // buckets up to this size are scanned without box tests
 constexpr int kQueryBatch = 16;       // consecutive queries grabbed per warp
-constexpr int kMergeThreshold = 9;    // serial insert ~11 instr each vs ~95 for a full merge
+// a scan step with this many improving lanes merges them (17 shfl + 1 vote as a first sort, 23 + 1 as a full merge)
+// instead of inserting them one by one (2 shfl each + 1 per step).  A/B on the 10 M mixed / uniform clouds, k = 16,
+// H100 80GB HBM3 at 700 W, k_sor_knn median ms: 6 -> 6.09 / 4.99, 9 -> 6.08 / 4.97, 12 -> 6.17 / 5.05, 16 -> 6.28 / 5.16.
+constexpr int kMergeThreshold = 9;
 constexpr int kKnnMinBlocks = 8;      // __launch_bounds__ minimum of resident CTAs per SM
 // long buckets that span fewer than this many supers (1024 points each) skip the super-box level.
 // 8 was chosen by A/B timing against 32 on the mixed cloud.
@@ -56,7 +59,7 @@ constexpr int kFlatSupers = 8;
 // i32=1 (32-bit positions) describe fixed properties of the kernel; they stay so that bench lines remain comparable.
 // cell_order=hilbert15 names the build's in-bucket order (15-bit in-cell Hilbert code), which sets the query's scan count.
 const char* sor_build_info() {
-    return "knn=r02c;epi_smem=1;first_sort=1;query_batch=16;minblocks=8;merge_threshold=9;small_bucket=64;"
+    return "knn=r03a;epi_smem=1;first_sort=1;query_batch=16;minblocks=8;merge_threshold=9;small_bucket=64;"
            "flat_supers=8;knn16=0;tma=0;i32=1;cell_order=hilbert15";
 }
 
@@ -934,6 +937,15 @@ __device__ __forceinline__ uint32_t probe_hash(int nx, int ny, int nz, uint32_t 
     }
 }
 
+// Key of a box in a nearest-first group of 32: the lower bound's bit pattern (lb >= +0, so the bits order as the
+// floats do) with the lane number in the low 5 bits -- one redux.min yields the nearest box AND the lane that holds
+// it.  knn_key_lb() (low bits cleared) is <= the true lower bound by < 32 ulp, so `knn_key_lb(key) < tau` may keep
+// a box the exact test would drop and never drops one it would keep; an extra visit cannot change the K smallest.
+// An exhausted lane holds kKeyNone, whose knn_key_lb is a NaN: it fails `< tau` like any box out of reach.
+constexpr unsigned kKeyNone = 0xffffffffu;
+__device__ __forceinline__ unsigned knn_key(float lb, int lane) { return (__float_as_uint(lb) & ~31u) | (unsigned)lane; }
+__device__ __forceinline__ float knn_key_lb(unsigned key) { return __uint_as_float(key & ~31u); }
+
 // Lower bound of the float32 d^2 the scan would compute for any point inside the box: same op
 // sequence (sub, mul, add -- no fma), every op monotone, so lb <= d2(point) exactly.
 __device__ __forceinline__ float box_lb(const float4* __restrict__ aabb, int64_t id, float qx, float qy, float qz) {
@@ -973,7 +985,10 @@ struct TopK {
     __device__ __forceinline__ void refresh_tau() {
         tau = (NREG == 2 && K > 32) ? __shfl_sync(GSX_FULL, v1, K - 33) : __shfl_sync(GSX_FULL, v0, K - 1);
     }
-    // insert warp-uniform x (< tau), gpu_ops.py:154-160 in the d^2 domain
+    // insert warp-uniform x, gpu_ops.py:154-160 in the d^2 domain.  Does NOT refresh tau: the caller does, once per scan
+    // step.  Invariant: the 32 (64) lanes always hold, ascending, the smallest 32 (64) of every value offered so far
+    // (a plain sorted insert that drops the largest), whatever x is.  So an x that passed the tau of the step's start
+    // but is >= the current rank K-1 only moves lanes >= K, which are never read; the K smallest are untouched.
     __device__ __forceinline__ void insert(float x, int lane) {
         float up0 = __shfl_up_sync(GSX_FULL, v0, 1);
         if (NREG == 2) {
@@ -984,20 +999,20 @@ struct TopK {
         }
         if (lane == 0) up0 = 0.f;
         if (v0 > x) v0 = fmaxf(up0, x);
-        refresh_tau();
     }
     // NREG==1 only: merge one candidate per lane (nv; lanes without a candidate pass the sentinel) into
     // the list.  sort(nv) ascending, reverse it, lane-wise min with the ascending list = the 32 smallest
     // of the union as a bitonic sequence, 5 merge stages sort it.  Lanes >= K only ever hold values
     // >= rank K-1, so they never change the K smallest (only the multiset of values matters, A.1-7).
-    __device__ __forceinline__ void merge32(float nv, int lane) {
+    // Returns whether it took the first-sort form (the query counters tell the two forms apart).
+    __device__ __forceinline__ bool merge32(float nv, int lane) {
         nv = warp_sort32(nv, lane);
         // the first merge of a query meets an empty list (32 sentinels): the sorted candidates ARE the merged list --
         // skips the reversal and the 5 merge stages (the sentinel is the largest value either side can hold)
         if (__all_sync(GSX_FULL, v0 == __uint_as_float(GSX_D2LIM_BITS))) {
             v0 = nv;
             refresh_tau();
-            return;
+            return true;
         }
         float r = __shfl_sync(GSX_FULL, nv, 31 - lane);
         float m = fminf(v0, r);
@@ -1005,16 +1020,37 @@ struct TopK {
         for (int j = 16; j > 0; j >>= 1) m = cmpx(m, j, (lane & j) == 0);
         v0 = m;
         refresh_tau();
+        return false;
     }
 };
+
+// The query counters of the STATS instantiation (gsx_sor_query_counters): what a query spends on the warp-collective
+// operations (shfl, vote, redux).  Counter c lives in lane c of one register per thread; every count is warp-uniform.
+enum KnnCounter {
+    kCntInserts,       // serial inserts executed
+    kCntMergesFirst,   // merge32 calls that met an empty list (sort only)
+    kCntMergesFull,    // merge32 calls with the 5 merge stages
+    kCntProbeVisits,   // buckets taken from the probe loop
+    kCntSuperVisits,   // super boxes taken from a super group
+    kCntChunkGroups,   // chunk_group calls (one box test per lane each)
+    kCntChunkVisits,   // chunks taken from a chunk group and scanned
+    kCntScanSteps,     // scan32 calls: chunk visits + small-bucket steps + own-chunk seeds
+    kCntCount
+};
+template <bool STATS>
+__device__ __forceinline__ void knn_count(unsigned long long& cnt, int lane, KnnCounter c) {
+    if (STATS && lane == (int)c) ++cnt;
+}
 
 // positions in the hash-sorted order fit 31 bits (n < 2^31 - 64): 32-bit index arithmetic in the scan loops
 typedef int pos_t;
 
-// distance of the query to candidate j and ballot/shfl insertion of the lanes that beat tau
+// distance of the query to candidate j and ballot/shfl insertion of the lanes that beat the tau of the step's start
+// (tau is refreshed once after the step: see TopK::insert)
 template <int NREG, bool STATS>
 __device__ __forceinline__ void scan32(const float4* __restrict__ spos, pos_t j, bool valid, float qx, float qy,
-                                       float qz, TopK<NREG>& tk, int lane, unsigned long long& n_scanned) {
+                                       float qz, TopK<NREG>& tk, int lane, unsigned long long& n_scanned,
+                                       unsigned long long& cnt) {
     float d2 = INFINITY;
     if (valid) {
         float4 c = __ldg(spos + j);
@@ -1022,18 +1058,22 @@ __device__ __forceinline__ void scan32(const float4* __restrict__ spos, pos_t j,
         d2 = __fadd_rn(__fadd_rn(__fmul_rn(ax, ax), __fmul_rn(ay, ay)), __fmul_rn(az, az));
     }
     if (STATS) n_scanned += __popc(__ballot_sync(GSX_FULL, valid));
+    knn_count<STATS>(cnt, lane, kCntScanSteps);
     bool pass = valid && d2 > 1.0e-12f && d2 < tk.tau;
     unsigned m = __ballot_sync(GSX_FULL, pass);
+    if (m == 0u) return;
     if (NREG == 1 && __popc(m) >= kMergeThreshold) {
-        tk.merge32(pass ? d2 : __uint_as_float(GSX_D2LIM_BITS), lane);
+        const bool first = tk.merge32(pass ? d2 : __uint_as_float(GSX_D2LIM_BITS), lane);
+        knn_count<STATS>(cnt, lane, first ? kCntMergesFirst : kCntMergesFull);
         return;
     }
     while (m) {
         int src = __ffs(m) - 1;
         m &= m - 1;
-        float x = __shfl_sync(GSX_FULL, d2, src);
-        if (x < tk.tau) tk.insert(x, lane);
+        tk.insert(__shfl_sync(GSX_FULL, d2, src), lane);
+        knn_count<STATS>(cnt, lane, kCntInserts);
     }
+    tk.refresh_tau();
 }
 
 // ES > 0: batched epilogue (gpu_ops.py:163-174: serial float32 sum of the valid distances, mean) -- every query of a
@@ -1047,9 +1087,11 @@ __global__ void __launch_bounds__(256, kKnnMinBlocks)
               const float4* __restrict__ saabb, float* __restrict__ final_means, unsigned int* __restrict__ work,
               int64_t q_begin, int64_t q_end, int q_stride, int q_phase, int K, int hash_mode, float bx, float by,
               float bz, float cell,
-              uint32_t n, uint64_t M, unsigned long long* __restrict__ stats) {
+              uint32_t n, uint64_t M, unsigned long long* __restrict__ stats,
+              unsigned long long* __restrict__ query_counters) {
     const int lane = lane_id();
     unsigned long long st_visits = 0, st_scanned = 0, st_boxes = 0, st_queries = 0;
+    unsigned long long st_cnt = 0;   // lane c: query counter c (KnnCounter)
     static_assert(ES >= 0 && ES <= 33, "a row holds at most the 32 ranks of one register + the row number");
     // batched epilogue (ES > 0): [8 warps][kQueryBatch][ES] floats, a row = ES-1 ranks (>= K) + the row number; ES is
     // odd so that the lanes of the final pass (one query each) read distinct banks
@@ -1073,6 +1115,7 @@ __global__ void __launch_bounds__(256, kKnnMinBlocks)
         // consecutive positions inside one 32-bit word (kQueryBatch divides 32, batches are aligned to q_begin).
         const uint32_t cellword = __ldg(cellbits + (qb >> 5));
         int ps = 0, pc = 0;                                  // lane p: bucket range of probe p
+        int s13 = 0, c13 = 0;                                // the centre probe's range, broadcast once per cell
         float blx = 0.f, bly = 0.f, blz = 0.f, bhx = 0.f, bhy = 0.f, bhz = 0.f;  // and its bounding box
         const pos_t qb_p = (pos_t)qb, qe_p = (pos_t)qe;      // positions fit 31 bits (pos_t): 32-bit loop bookkeeping
 #pragma unroll 1
@@ -1094,6 +1137,7 @@ __global__ void __launch_bounds__(256, kKnnMinBlocks)
                         blx = b0.x, bly = b0.y, blz = b0.z, bhx = b1.x, bhy = b1.y, bhz = b1.z;
                     }
                 }
+                s13 = __shfl_sync(GSX_FULL, ps, 13), c13 = __shfl_sync(GSX_FULL, pc, 13);
             }
             if (STATS) {
                 int tot = pc;
@@ -1108,40 +1152,39 @@ __global__ void __launch_bounds__(256, kKnnMinBlocks)
             // lower bound of d^2 to the bucket's box (same monotone op sequence as d^2 itself, see box_lb):
             // probes are visited nearest box first and dropped as soon as lb >= tau.  The query's own bucket
             // has lb == 0 and therefore comes first whenever the centre probe reaches it.
-            unsigned pkey = 0xffffffffu;
+            unsigned pkey = kKeyNone;
             if (pc > 0) {
                 float dx = fmaxf(fmaxf(__fsub_rn(blx, q.x), __fsub_rn(q.x, bhx)), 0.f);
                 float dy = fmaxf(fmaxf(__fsub_rn(bly, q.y), __fsub_rn(q.y, bhy)), 0.f);
                 float dz = fmaxf(fmaxf(__fsub_rn(blz, q.z), __fsub_rn(q.z, bhz)), 0.f);
-                pkey = __float_as_uint(__fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz)));
+                pkey = knn_key(__fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz)), lane);
             }
 
             // seed from the chunk that holds the query itself when its own bucket is big: gives a
             // tight tau before the box walk.  Only legal if the centre probe really reaches the
             // query's bucket range (with the wrapped hash it may not, SURVEY F8).
             int skip_chunk = -1;
-            {
-                int s13 = __shfl_sync(GSX_FULL, ps, 13), c13 = __shfl_sync(GSX_FULL, pc, 13);
-                if (c13 > kSmallBucket && i >= s13 && i < (pos_t)s13 + c13) {
-                    skip_chunk = (int)(i >> 5);
-                    const pos_t j = ((pos_t)skip_chunk << 5) + lane;
-                    scan32<NREG, STATS>(spos, j, j >= s13 && j < (pos_t)s13 + c13, q.x, q.y, q.z, tk, lane,
-                                        st_scanned);
-                }
+            if (c13 > kSmallBucket && i >= s13 && i < (pos_t)s13 + c13) {
+                skip_chunk = (int)(i >> 5);
+                const pos_t j = ((pos_t)skip_chunk << 5) + lane;
+                scan32<NREG, STATS>(spos, j, j >= s13 && j < (pos_t)s13 + c13, q.x, q.y, q.z, tk, lane, st_scanned,
+                                    st_cnt);
             }
 
 #pragma unroll 1
             for (;;) {
                 const unsigned mp = __reduce_min_sync(GSX_FULL, pkey);
-                if (mp == 0xffffffffu || !(__uint_as_float(mp) < tk.tau)) break;
-                const int p = __ffs(__ballot_sync(GSX_FULL, pkey == mp)) - 1;
-                if (lane == p) pkey = 0xffffffffu;
+                if (!(knn_key_lb(mp) < tk.tau)) break;
+                const int p = (int)(mp & 31u);
+                if (lane == p) pkey = kKeyNone;
+                knn_count<STATS>(st_cnt, lane, kCntProbeVisits);
                 const int s = __shfl_sync(GSX_FULL, ps, p), c = __shfl_sync(GSX_FULL, pc, p);
                 const pos_t e = (pos_t)s + c;
                 if (c <= kSmallBucket) {
 #pragma unroll 1
                     for (pos_t base = s; base < e; base += 32)
-                        scan32<NREG, STATS>(spos, base + lane, base + lane < e, q.x, q.y, q.z, tk, lane, st_scanned);
+                        scan32<NREG, STATS>(spos, base + lane, base + lane < e, q.x, q.y, q.z, tk, lane, st_scanned,
+                                            st_cnt);
                     continue;
                 }
                 const int skip = p == 13 ? skip_chunk : -1;
@@ -1151,19 +1194,21 @@ __global__ void __launch_bounds__(256, kKnnMinBlocks)
                 auto chunk_group = [&](const int cbase) {
                     const int cid = cbase + lane;
                     const bool cv = cid >= fc && cid <= lc && cid != skip;
-                    unsigned ckey = 0xffffffffu;
+                    unsigned ckey = kKeyNone;
                     if (cv) {
                         float lb = box_lb(caabb, cid, q.x, q.y, q.z);
-                        if (lb < tk.tau) ckey = __float_as_uint(lb);
+                        if (lb < tk.tau) ckey = knn_key(lb, lane);
                     }
                     if (STATS) st_boxes += __popc(__ballot_sync(GSX_FULL, cv));
+                    knn_count<STATS>(st_cnt, lane, kCntChunkGroups);
                     for (;;) {
-                        unsigned mc = __reduce_min_sync(GSX_FULL, ckey);
-                        if (mc == 0xffffffffu || !(__uint_as_float(mc) < tk.tau)) break;
-                        int srcc = __ffs(__ballot_sync(GSX_FULL, ckey == mc)) - 1;
-                        if (lane == srcc) ckey = 0xffffffffu;
+                        const unsigned mc = __reduce_min_sync(GSX_FULL, ckey);
+                        if (!(knn_key_lb(mc) < tk.tau)) break;
+                        const int srcc = (int)(mc & 31u);
+                        if (lane == srcc) ckey = kKeyNone;
+                        knn_count<STATS>(st_cnt, lane, kCntChunkVisits);
                         const pos_t j = ((pos_t)(cbase + srcc) << 5) + lane;
-                        scan32<NREG, STATS>(spos, j, j >= s && j < e, q.x, q.y, q.z, tk, lane, st_scanned);
+                        scan32<NREG, STATS>(spos, j, j >= s && j < e, q.x, q.y, q.z, tk, lane, st_scanned, st_cnt);
                     }
                 };
                 // a bucket of a few supers: every super box is near the query (it sits in or next to this bucket), so
@@ -1175,17 +1220,18 @@ __global__ void __launch_bounds__(256, kKnnMinBlocks)
                 }
                 for (int sb = fs; sb <= ls; sb += 32) {
                     const int sid = sb + lane;
-                    unsigned skey = 0xffffffffu;
+                    unsigned skey = kKeyNone;
                     if (sid <= ls) {
                         float lb = box_lb(saabb, sid, q.x, q.y, q.z);
-                        if (lb < tk.tau) skey = __float_as_uint(lb);
+                        if (lb < tk.tau) skey = knn_key(lb, lane);
                     }
                     if (STATS) st_boxes += __popc(__ballot_sync(GSX_FULL, sid <= ls));
                     for (;;) {
-                        unsigned ms = __reduce_min_sync(GSX_FULL, skey);
-                        if (ms == 0xffffffffu || !(__uint_as_float(ms) < tk.tau)) break;
-                        int srcs = __ffs(__ballot_sync(GSX_FULL, skey == ms)) - 1;
-                        if (lane == srcs) skey = 0xffffffffu;
+                        const unsigned ms = __reduce_min_sync(GSX_FULL, skey);
+                        if (!(knn_key_lb(ms) < tk.tau)) break;
+                        const int srcs = (int)(ms & 31u);
+                        if (lane == srcs) skey = kKeyNone;
+                        knn_count<STATS>(st_cnt, lane, kCntSuperVisits);
                         chunk_group((sb + srcs) * 32);
                     }
                 }
@@ -1237,6 +1283,7 @@ __global__ void __launch_bounds__(256, kKnnMinBlocks)
         atomicAdd(stats + 2, st_boxes);
         atomicAdd(stats + 3, st_queries);
     }
+    if (STATS && lane < kCntCount) atomicAdd(query_counters + lane, st_cnt);
 }
 
 __global__ void k_fill_f32(float* p, int64_t n, float v) {
@@ -1258,7 +1305,7 @@ static int launch_knn(SorWs& w, int64_t q_begin, int64_t q_end, int q_stride, in
     if (grid < 1) grid = 1;
     kernel<<<(int)grid, 256, smem, st>>>(w.spos, w.tab_se, w.tab_box, w.cellbits, w.caabb, w.saabb, final_means, w.counters,
                                          q_begin, q_end, q_stride, q_phase, K, hash_mode, bmin[0], bmin[1], bmin[2], cell,
-                                         (uint32_t)w.n, M, stats);
+                                         (uint32_t)w.n, M, stats, w.stats);
     return GSX_OK;
 }
 
@@ -1272,6 +1319,7 @@ int sor_mean_dists(SorWs& w, int64_t q_begin, int64_t q_end, int q_stride, int q
     GSX_REQUIRE(q_begin >= 0 && q_end <= n && q_begin <= q_end, GSX_ERR_ARG, "sor: bad query range");
     GSX_REQUIRE(q_stride >= 1 && q_phase >= 0 && q_phase < q_stride, GSX_ERR_ARG, "sor: bad query stride/phase");
     int K = k < 50 ? k : 50;  // gpu_ops.py:244
+    if (stats) GSX_CUDA_CHECK(cudaMemsetAsync(w.stats, 0, kCntCount * sizeof(unsigned long long), st));
     if (q_end == q_begin) return GSX_OK;
     if (!(cell > 1e-8f)) {  // gpu_ops.py:175-176 (unreachable through the driver: cell >= 1e-4)
         GSX_REQUIRE(q_begin == 0 && q_end == n, GSX_ERR_UNSUPPORTED, "sor: degenerate cell with a query range");

@@ -47,6 +47,7 @@ _SIGS = {
     "gsx_sor_mean_dists": (C.c_int, [_i64, _i32, _i32, _f32p, C.c_float, _vp, _i64, _vp, _vp, _vp]),
     "gsx_sor_mean_dists_range": (C.c_int, [_i64, _i64, _i64, _i32, _i32, _f32p, C.c_float, _vp, _i64, _vp, _vp, _vp]),
     "gsx_sor_mean_dists_strided": (C.c_int, [_i64, _i32, _i32, _i32, _i32, _f32p, C.c_float, _vp, _i64, _vp, _vp, _vp]),
+    "gsx_sor_query_counters": (C.c_int, [_i64, _vp, _i64, _vp, _vp]),
     "gsx_sort_pairs_workspace_bytes": (_i64, [_i64]),
     "gsx_sort_pairs": (C.c_int, [_vp, _vp, _i64, _i32, _i32, _vp, _i64, _vp]),
     "gsx_mean_std_workspace_bytes": (_i64, [_i64]),

@@ -72,9 +72,23 @@ def build_grid(xyz: torch.Tensor, ws: torch.Tensor | None = None, cell_scale: fl
     return SorGrid(n, ws, bmin, cell)
 
 
+QUERY_COUNTERS = ("inserts", "merges_first", "merges_full", "probe_visits", "super_visits", "chunk_groups",
+                  "chunk_visits", "scan_steps")
+
+
+def _stats_dict(grid: SorGrid, stats: torch.Tensor) -> dict:
+    """The 4 counters of the caller's buffer and the kernel's 8 query counters (gsx_sor_query_counters)."""
+    v = stats.cpu().numpy()
+    c = (C.c_ulonglong * 8)()
+    check(lib.gsx_sor_query_counters(grid.n, _ptr(grid.ws), grid.ws.numel(), C.cast(c, C.c_void_p), _stream()),
+          "gsx_sor_query_counters")
+    return dict(visits=int(v[0]), scanned=int(v[1]), box_tests=int(v[2]), queries=int(v[3]),
+                **{name: int(c[i]) for i, name in enumerate(QUERY_COUNTERS)})
+
+
 def mean_dists(grid: SorGrid, k: int, hash_mode: str | None = None, out: torch.Tensor | None = None,
                want_stats: bool = False, q_range: tuple[int, int] | None = None):
-    """gpu_ops.py:98-176 + unsort (:255-256).  Returns final_means (and the 4 counters if asked)."""
+    """gpu_ops.py:98-176 + unsort (:255-256).  Returns final_means (and the counters if asked)."""
     mode = HASH_MODES[hash_mode or default_hash_mode()]
     dev = grid.ws.device
     if out is None:
@@ -85,8 +99,7 @@ def mean_dists(grid: SorGrid, k: int, hash_mode: str | None = None, out: torch.T
                                        grid.cell, _ptr(grid.ws), grid.ws.numel(), _ptr(out), _ptr(stats), _stream()),
           "gsx_sor_mean_dists")
     if want_stats:
-        v = stats.cpu().numpy()
-        return out, dict(visits=int(v[0]), scanned=int(v[1]), box_tests=int(v[2]), queries=int(v[3]))
+        return out, _stats_dict(grid, stats)
     return out
 
 
@@ -99,8 +112,7 @@ def mean_dists_strided(grid: SorGrid, k: int, hash_mode: str | None, out: torch.
                                          grid.bmin.ctypes.data_as(C.POINTER(C.c_float)), grid.cell, _ptr(grid.ws),
                                          grid.ws.numel(), _ptr(out), _ptr(stats), _stream()), "gsx_sor_mean_dists_strided")
     if want_stats:
-        v = stats.cpu().numpy()
-        return out, dict(visits=int(v[0]), scanned=int(v[1]), box_tests=int(v[2]), queries=int(v[3]))
+        return out, _stats_dict(grid, stats)
     return out
 
 

@@ -111,6 +111,13 @@ int gsx_sor_mean_dists_strided(int64_t n, int32_t stride, int32_t phase, int32_t
                                const float* bmin_host, float cell, void* ws, int64_t ws_bytes, float* final_means_dev,
                                unsigned long long* stats_dev, void* stream);
 
+/* The query kernel's own counters of the last gsx_sor_mean_dists* call on this workspace that passed a non-NULL
+ * stats_dev (that call zeroes them, also for an empty query range), copied to the HOST array out8_host after a
+ * synchronise of `stream`: {serial inserts, first merges (sort only), full merges, probe-loop bucket visits, super-box
+ * visits, chunk-group box-test rounds, chunk visits, scan steps of 32 candidates (chunk visits + small-bucket steps +
+ * own-chunk seeds)}.  They count what a query spends on warp shuffles, votes and reductions (DESIGN 4.2). */
+int gsx_sor_query_counters(int64_t n, void* ws, int64_t ws_bytes, unsigned long long* out8_host, void* stream);
+
 /* gpu_ops.py:227 (np.argsort of the bucket hashes): stable LSD radix sort, in place, of (uint64 key, int32
  * value) pairs on the key bits [begin_bit, end_bit): 8-bit digits, one "onesweep" kernel per digit (decoupled
  * look-back over per-tile digit counts) after a single histogram pass.  vals_dev == NULL sorts bare 64-bit words
