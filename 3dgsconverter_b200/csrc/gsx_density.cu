@@ -16,13 +16,15 @@
 
 #include <limits.h>
 #include <math.h>
-#include <stdlib.h>
 #include <vector>
 
 namespace gsx {
 
 constexpr int kAxisBits = 21;
 constexpr long long kAxisLim = 1ll << kAxisBits;
+
+// Slots of the counter array of the dense-voxel extraction.
+enum : int { kDense = 0, kDistinct = 1, kOutside = 2 };
 
 // A NaN quotient, or one outside the int64 range, gives INT64_MIN on host and device alike: what the reference's
 // np.floor(...).astype(np.int64) gives on x86.  (The device conversion alone saturates +inf to INT64_MAX, and the
@@ -36,15 +38,8 @@ __host__ __device__ __forceinline__ long long voxel_of(float v, float voxel) {
     return fabsf(f) < 9.2233720368547758e18f ? (long long)f : LLONG_MIN;   // -2^63 itself maps to INT64_MIN too
 }
 
-__device__ __forceinline__ uint64_t mix64(uint64_t x) {
-    x ^= x >> 33;
-    x *= 0xff51afd7ed558ccdull;
-    x ^= x >> 33;
-    x *= 0xc4ceb9fe1a85ec53ull;
-    x ^= x >> 33;
-    return x;
-}
-static inline uint64_t mix64_host(uint64_t x) {
+// Hash of the device tables and of the keep sets the host builds.
+__host__ __device__ __forceinline__ uint64_t mix64(uint64_t x) {
     x ^= x >> 33;
     x *= 0xff51afd7ed558ccdull;
     x ^= x >> 33;
@@ -53,9 +48,40 @@ static inline uint64_t mix64_host(uint64_t x) {
     return x;
 }
 
+// Key of a voxel relative to the box origin when every extent is < 2^21: three 21-bit fields, + 1 (0 = empty slot).
+__host__ __device__ __forceinline__ uint64_t pack_rel(long long rx, long long ry, long long rz) {
+    return (((uint64_t)rx << (2 * kAxisBits)) | ((uint64_t)ry << kAxisBits) | (uint64_t)rz) + 1ull;
+}
+
+// Two-word key for boxes that span 2^21 or more voxels on some axis (one far-away flyer with a small voxel):
+// a = (rx << 32 | ry) + 1, b = rz + 1, exact for any extent < 2^31.
+__host__ __device__ __forceinline__ void wide_key(long long rx, long long ry, long long rz, unsigned long long& a,
+                                                  unsigned long long& b) {
+    a = (((unsigned long long)rx << 32) | (unsigned long long)ry) + 1ull;
+    b = (unsigned long long)rz + 1ull;
+}
+
+__host__ __device__ __forceinline__ uint64_t wide_slot(unsigned long long a, unsigned long long b) {
+    return mix64(a ^ mix64(b));
+}
+
+struct Vox {
+    long long x, y, z;
+};
+
 struct VoxGrid {
     long long q0[3];   // voxel-space origin
     long long dim[3];  // extent in voxels
+
+    // Row-major cell index (z fastest) of a voxel in the box.
+    __device__ __forceinline__ size_t cell(long long qx, long long qy, long long qz) const {
+        return ((size_t)(qx - q0[0]) * dim[1] + (size_t)(qy - q0[1])) * dim[2] + (size_t)(qz - q0[2]);
+    }
+    __device__ __forceinline__ Vox voxel(size_t c) const {
+        const size_t z = c % (size_t)dim[2], y = (c / (size_t)dim[2]) % (size_t)dim[1],
+                     x = c / ((size_t)dim[2] * (size_t)dim[1]);
+        return {(long long)x + q0[0], (long long)y + q0[1], (long long)z + q0[2]};
+    }
 };
 
 // Whether voxel q lies in the box.  Compares before subtracting, so INT64_MIN - q0 is never formed.  Only rows with a
@@ -63,6 +89,31 @@ struct VoxGrid {
 __device__ __forceinline__ bool in_box(long long qx, long long qy, long long qz, const VoxGrid& g) {
     return qx >= g.q0[0] && qx <= g.q0[0] + (g.dim[0] - 1) && qy >= g.q0[1] && qy <= g.q0[1] + (g.dim[1] - 1) &&
            qz >= g.q0[2] && qz <= g.q0[2] + (g.dim[2] - 1);
+}
+
+// Appends a voxel to the dense list: every append takes a slot of counters[kDense], the first `cap` are stored.
+// `voxel()` is called only for a stored slot.  Returns the slot.
+template <class VoxelOf>
+__device__ __forceinline__ unsigned long long dense_append(unsigned long long* counters, long long* dense_vox,
+                                                           int64_t cap, VoxelOf voxel) {
+    const unsigned long long slot = atomicAdd(counters + kDense, 1ull);
+    if ((int64_t)slot < cap) {
+        const Vox q = voxel();
+        dense_vox[3 * slot] = q.x;
+        dense_vox[3 * slot + 1] = q.y;
+        dense_vox[3 * slot + 2] = q.z;
+    }
+    return slot;
+}
+
+// The dense-voxel rule of one counting add of c rows to a voxel whose counter held `old`: the first add counts a
+// distinct voxel, and the add that carries the count across thr (old < thr <= old + c: exactly one add does) appends
+// the voxel to the dense list.
+template <class VoxelOf>
+__device__ __forceinline__ void dense_rule(int old, int c, int thr, unsigned long long* counters,
+                                           long long* dense_vox, int64_t cap, VoxelOf voxel) {
+    if (old == 0) atomicAdd(counters + kDistinct, 1ull);
+    if (old < thr && old + c >= thr) dense_append(counters, dense_vox, cap, voxel);
 }
 
 int64_t density_workspace_bytes(int64_t n, int64_t cap) {
@@ -74,33 +125,110 @@ int64_t density_workspace_bytes(int64_t n, int64_t cap) {
     return (int64_t)(slots * 12 + 6 * 1024 * 4 + (size_t)cap * 28 + 8192);
 }
 
-// ---------------------------------------------------------------- dense-grid path
-__global__ void __launch_bounds__(256) k_vox_count_grid(const float* __restrict__ xyz, int64_t n, float voxel,
-                                                        VoxGrid g, int thr, int* __restrict__ grid,
-                                                        unsigned long long* __restrict__ counters,
-                                                        long long* __restrict__ dense_vox, int64_t cap) {
-    int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    long long qx = voxel_of(xyz[3 * i], voxel), qy = voxel_of(xyz[3 * i + 1], voxel),
-              qz = voxel_of(xyz[3 * i + 2], voxel);
-    if (!in_box(qx, qy, qz, g)) {
-        atomicAdd(counters + 2, 1ull);  // points dropped (non-finite coordinates)
-        return;
+// ---------------------------------------------------------------- counter tables
+// at() returns the counter of an in-box voxel, claiming its slot on first sight; find() returns the count of a voxel.
+
+struct GridTable {   // dense int32 grid over the voxel box
+    int* cnt;
+    __device__ __forceinline__ int* at(const VoxGrid& g, long long qx, long long qy, long long qz) const {
+        return cnt + g.cell(qx, qy, qz);
     }
-    size_t idx = ((size_t)(qx - g.q0[0]) * g.dim[1] + (size_t)(qy - g.q0[1])) * g.dim[2] + (size_t)(qz - g.q0[2]);
-    int old = atomicAdd(grid + idx, 1);
-    if (old == 0) atomicAdd(counters + 1, 1ull);  // number of distinct voxels
-    if (old + 1 == thr) {
-        unsigned long long slot = atomicAdd(counters, 1ull);
-        if ((int64_t)slot < cap) {
-            dense_vox[3 * slot] = qx;
-            dense_vox[3 * slot + 1] = qy;
-            dense_vox[3 * slot + 2] = qz;
+    __device__ __forceinline__ int find(const VoxGrid& g, long long qx, long long qy, long long qz) const {
+        return cnt[g.cell(qx, qy, qz)];
+    }
+};
+
+struct HashTable {   // 3 x 21-bit keys: key at keys[s], count at cnt[s]
+    unsigned long long* keys;
+    int* cnt;
+    uint64_t slot_mask;
+    __device__ __forceinline__ int* at(const VoxGrid& g, long long qx, long long qy, long long qz) const {
+        const uint64_t key = pack_rel(qx - g.q0[0], qy - g.q0[1], qz - g.q0[2]);
+        uint64_t s = mix64(key) & slot_mask;
+        for (;;) {
+            unsigned long long cur = keys[s];
+            if (cur == 0ull) {
+                unsigned long long prev = atomicCAS(keys + s, 0ull, (unsigned long long)key);
+                cur = prev == 0ull ? (unsigned long long)key : prev;
+            }
+            if (cur == key) break;
+            s = (s + 1) & slot_mask;
+        }
+        return cnt + s;
+    }
+    __device__ __forceinline__ int find(const VoxGrid& g, long long qx, long long qy, long long qz) const {
+        const uint64_t key = pack_rel(qx - g.q0[0], qy - g.q0[1], qz - g.q0[2]);
+        uint64_t s = mix64(key) & slot_mask;
+        while (keys[s] != key) s = (s + 1) & slot_mask;
+        return cnt[s];
+    }
+};
+
+// Two-word keys {a, b} at ha[s], hb[s].  A slot is claimed by a CAS on `a`; the owner then publishes `b`; a thread
+// that finds its own `a` waits for `b` (independent thread scheduling makes the intra-warp wait safe) and moves on if
+// it differs (same x,y column, other z).
+struct WideHashTable {
+    unsigned long long* ha;
+    unsigned long long* hb;
+    int* cnt;
+    uint64_t slot_mask;
+    __device__ __forceinline__ uint64_t slot(const VoxGrid& g, long long qx, long long qy, long long qz,
+                                             bool insert) const {
+        unsigned long long a, b;
+        wide_key(qx - g.q0[0], qy - g.q0[1], qz - g.q0[2], a, b);
+        uint64_t s = wide_slot(a, b) & slot_mask;
+        for (;;) {
+            unsigned long long cur = *((volatile unsigned long long*)(ha + s));
+            if (cur == 0ull) {
+                if (!insert) return ~0ull;
+                unsigned long long prev = atomicCAS(ha + s, 0ull, a);
+                if (prev == 0ull) {
+                    atomicExch(hb + s, b);
+                    return s;
+                }
+                cur = prev;
+            }
+            if (cur == a) {
+                unsigned long long bv;
+                do {
+                    bv = *((volatile unsigned long long*)(hb + s));
+                } while (bv == 0ull);
+                if (bv == b) return s;
+            }
+            s = (s + 1) & slot_mask;
         }
     }
+    __device__ __forceinline__ int* at(const VoxGrid& g, long long qx, long long qy, long long qz) const {
+        return cnt + slot(g, qx, qy, qz, true);
+    }
+    __device__ __forceinline__ int find(const VoxGrid& g, long long qx, long long qy, long long qz) const {
+        const uint64_t s = slot(g, qx, qy, qz, false);
+        return s == ~0ull ? 0 : cnt[s];
+    }
+};
+
+// ---------------------------------------------------------------- histogram kernels
+// One row per thread into any table.  DENSE: with the dense-voxel rule of the one-shot path.  Without it (the staged
+// grid) the add's old value is unused and the add compiles to a reduction, which does not wait for a reply; a run-time
+// switch would not do, as the compiler merges the two adds into one that returns the old value.
+template <bool DENSE, class Table>
+__global__ void __launch_bounds__(256) k_vox_count(const float* __restrict__ xyz, int64_t n, float voxel, VoxGrid g,
+                                                   Table tab, int thr, unsigned long long* __restrict__ counters,
+                                                   long long* __restrict__ dense_vox, int64_t cap,
+                                                   unsigned long long* __restrict__ oob) {
+    int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const long long qx = voxel_of(xyz[3 * i], voxel), qy = voxel_of(xyz[3 * i + 1], voxel),
+                    qz = voxel_of(xyz[3 * i + 2], voxel);
+    if (!in_box(qx, qy, qz, g)) {
+        atomicAdd(oob, 1ull);  // rows dropped (non-finite coordinates)
+        return;
+    }
+    const int old = atomicAdd(tab.at(g, qx, qy, qz), 1);
+    if (DENSE) dense_rule(old, 1, thr, counters, dense_vox, cap, [&] { return Vox{qx, qy, qz}; });
 }
 
-// Same histogram with per-block aggregation: clustered clouds put 10^5..10^6 points into a handful of voxels and
+// Dense-grid histogram with per-block aggregation: clustered clouds put 10^5..10^6 points into a handful of voxels and
 // same-address global atomics serialise in L2.  Each block first counts its 2048 points in a 1024-slot shared-memory
 // hash (cell index -> count) and then issues ONE global atomicAdd per distinct cell; the increment may be > 1, so the
 // threshold crossing is detected as old < thr <= old + c (still exactly one block sees it).
@@ -119,18 +247,7 @@ __global__ void __launch_bounds__(256) k_vox_count_grid_agg(const float* __restr
     const int64_t base = (int64_t)blockIdx.x * (256 * kAggItems);
     unsigned long long bad = 0;   // rows dropped (non-finite coordinates)
     auto commit = [&](unsigned int idx, int c) {
-        int old = atomicAdd(grid + idx, c);
-        if (old == 0) atomicAdd(counters + 1, 1ull);
-        if (old < thr && old + c >= thr) {
-            unsigned long long slot = atomicAdd(counters, 1ull);
-            if ((int64_t)slot < cap) {
-                size_t cz = idx % (size_t)g.dim[2], cy = (idx / (size_t)g.dim[2]) % (size_t)g.dim[1],
-                       cx = idx / ((size_t)g.dim[2] * (size_t)g.dim[1]);
-                dense_vox[3 * slot] = (long long)cx + g.q0[0];
-                dense_vox[3 * slot + 1] = (long long)cy + g.q0[1];
-                dense_vox[3 * slot + 2] = (long long)cz + g.q0[2];
-            }
-        }
+        dense_rule(atomicAdd(grid + idx, c), c, thr, counters, dense_vox, cap, [&] { return g.voxel(idx); });
     };
 #pragma unroll 2
     for (int e = 0; e < kAggItems; ++e) {
@@ -142,8 +259,7 @@ __global__ void __launch_bounds__(256) k_vox_count_grid_agg(const float* __restr
             ++bad;
             continue;
         }
-        const unsigned int idx =
-            (unsigned int)(((size_t)(qx - g.q0[0]) * g.dim[1] + (size_t)(qy - g.q0[1])) * g.dim[2] + (size_t)(qz - g.q0[2]));
+        const unsigned int idx = (unsigned int)g.cell(qx, qy, qz);
         unsigned int slot = (idx * 2654435761u) >> 22;  // 10 bits
         bool placed = false;
 #pragma unroll 1
@@ -157,7 +273,7 @@ __global__ void __launch_bounds__(256) k_vox_count_grid_agg(const float* __restr
         }
         if (!placed) commit(idx, 1);
     }
-    if (bad) atomicAdd(counters + 2, bad);
+    if (bad) atomicAdd(counters + kOutside, bad);
     __syncthreads();
     for (int t = threadIdx.x; t < kAggSlots; t += 256)
         if (sval[t] > 0) commit(skey[t], sval[t]);
@@ -187,7 +303,7 @@ __global__ void __launch_bounds__(512)
             ++bad;
             return;
         }
-        atomicAdd(&sh_hist[(int)(((qx - g.q0[0]) * g.dim[1] + (qy - g.q0[1])) * g.dim[2] + (qz - g.q0[2]))], 1);
+        atomicAdd(&sh_hist[(int)g.cell(qx, qy, qz)], 1);
     };
     for (int64_t t = g0 + threadIdx.x; t < g1; t += blockDim.x) {
         if (vec) {
@@ -209,18 +325,7 @@ __global__ void __launch_bounds__(512)
         const int c = sh_hist[t];
         if (c == 0) continue;
         const int old = atomicAdd(grid + t, c);
-        if (thr > 0) {
-            if (old == 0) atomicAdd(counters + 1, 1ull);
-            if (old < thr && old + c >= thr) {
-                const unsigned long long slot = atomicAdd(counters, 1ull);
-                if ((int64_t)slot < cap) {
-                    const long long cz = t % g.dim[2], cy = (t / g.dim[2]) % g.dim[1], cx = t / (g.dim[2] * g.dim[1]);
-                    dense_vox[3 * slot] = cx + g.q0[0];
-                    dense_vox[3 * slot + 1] = cy + g.q0[1];
-                    dense_vox[3 * slot + 2] = cz + g.q0[2];
-                }
-            }
-        }
+        if (thr > 0) dense_rule(old, c, thr, counters, dense_vox, cap, [&] { return g.voxel(t); });
     }
 }
 
@@ -242,141 +347,12 @@ static int launch_vox_count_smem(const float* xyz, int64_t n, float voxel, const
     return GSX_OK;
 }
 
-__global__ void k_vox_dense_counts_grid(const long long* __restrict__ dense_vox, int64_t nd, VoxGrid g,
-                                        const int* __restrict__ grid, int* __restrict__ dense_cnt) {
-    int64_t s = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (s >= nd) return;
-    size_t idx = ((size_t)(dense_vox[3 * s] - g.q0[0]) * g.dim[1] + (size_t)(dense_vox[3 * s + 1] - g.q0[1])) * g.dim[2] +
-                 (size_t)(dense_vox[3 * s + 2] - g.q0[2]);
-    dense_cnt[s] = grid[idx];
-}
-
-// ---------------------------------------------------------------- hash path
-__device__ __forceinline__ uint64_t pack_rel(long long rx, long long ry, long long rz) {
-    return (((uint64_t)rx << (2 * kAxisBits)) | ((uint64_t)ry << kAxisBits) | (uint64_t)rz) + 1ull;  // 0 = empty
-}
-
-__global__ void __launch_bounds__(256) k_vox_count_hash(const float* __restrict__ xyz, int64_t n, float voxel,
-                                                        VoxGrid g, int thr, unsigned long long* hkeys,
-                                                        int* hcnt, uint64_t slot_mask,
-                                                        unsigned long long* __restrict__ counters,
-                                                        long long* __restrict__ dense_vox, int64_t cap) {
-    int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    long long qx = voxel_of(xyz[3 * i], voxel), qy = voxel_of(xyz[3 * i + 1], voxel),
-              qz = voxel_of(xyz[3 * i + 2], voxel);
-    if (!in_box(qx, qy, qz, g)) {
-        atomicAdd(counters + 2, 1ull);
-        return;
-    }
-    uint64_t key = pack_rel(qx - g.q0[0], qy - g.q0[1], qz - g.q0[2]);
-    uint64_t s = mix64(key) & slot_mask;
-    for (;;) {
-        unsigned long long cur = hkeys[s];
-        if (cur == 0ull) {
-            unsigned long long prev = atomicCAS(hkeys + s, 0ull, (unsigned long long)key);
-            cur = prev == 0ull ? (unsigned long long)key : prev;
-        }
-        if (cur == key) break;
-        s = (s + 1) & slot_mask;
-    }
-    int old = atomicAdd(hcnt + s, 1);
-    if (old == 0) atomicAdd(counters + 1, 1ull);
-    if (old + 1 == thr) {
-        unsigned long long slot = atomicAdd(counters, 1ull);
-        if ((int64_t)slot < cap) {
-            dense_vox[3 * slot] = qx;
-            dense_vox[3 * slot + 1] = qy;
-            dense_vox[3 * slot + 2] = qz;
-        }
-    }
-}
-
-__global__ void k_vox_dense_counts_hash(const long long* __restrict__ dense_vox, int64_t nd, VoxGrid g,
-                                        const unsigned long long* __restrict__ hkeys, const int* __restrict__ hcnt,
-                                        uint64_t slot_mask, int* __restrict__ dense_cnt) {
+template <class Table>
+__global__ void k_vox_dense_counts(const long long* __restrict__ dense_vox, int64_t nd, VoxGrid g, Table tab,
+                                   int* __restrict__ dense_cnt) {
     int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= nd) return;
-    uint64_t key = pack_rel(dense_vox[3 * t] - g.q0[0], dense_vox[3 * t + 1] - g.q0[1], dense_vox[3 * t + 2] - g.q0[2]);
-    uint64_t s = mix64(key) & slot_mask;
-    while (hkeys[s] != key) s = (s + 1) & slot_mask;
-    dense_cnt[t] = hcnt[s];
-}
-
-// Wide-key variant for voxel boxes that span 2^21 or more voxels on some axis (one far-away flyer with a small voxel):
-// the slot key is the pair a = (rx << 32 | ry) + 1, b = rz + 1 (extents < 2^31).  A slot is claimed by a CAS on `a`;
-// the owner then publishes `b`; a thread that finds its own `a` waits for `b` (independent thread scheduling makes
-// the intra-warp wait safe) and moves on if it differs (same x,y column, other z).  Exact for any extent < 2^31.
-__device__ __forceinline__ void wide_key(long long rx, long long ry, long long rz, unsigned long long& a,
-                                         unsigned long long& b) {
-    a = (((unsigned long long)rx << 32) | (unsigned long long)ry) + 1ull;
-    b = (unsigned long long)rz + 1ull;
-}
-
-__device__ __forceinline__ uint64_t wide_find_or_insert(unsigned long long a, unsigned long long b,
-                                                        unsigned long long* ha, unsigned long long* hb,
-                                                        uint64_t slot_mask, bool insert) {
-    uint64_t s = mix64(a ^ mix64(b)) & slot_mask;
-    for (;;) {
-        unsigned long long cur = *((volatile unsigned long long*)(ha + s));
-        if (cur == 0ull) {
-            if (!insert) return ~0ull;
-            unsigned long long prev = atomicCAS(ha + s, 0ull, a);
-            if (prev == 0ull) {
-                atomicExch(hb + s, b);
-                return s;
-            }
-            cur = prev;
-        }
-        if (cur == a) {
-            unsigned long long bv;
-            do {
-                bv = *((volatile unsigned long long*)(hb + s));
-            } while (bv == 0ull);
-            if (bv == b) return s;
-        }
-        s = (s + 1) & slot_mask;
-    }
-}
-
-__global__ void __launch_bounds__(256) k_vox_count_hash_wide(const float* __restrict__ xyz, int64_t n, float voxel,
-                                                             VoxGrid g, int thr, unsigned long long* ha,
-                                                             unsigned long long* hb, int* hcnt, uint64_t slot_mask,
-                                                             unsigned long long* __restrict__ counters,
-                                                             long long* __restrict__ dense_vox, int64_t cap) {
-    int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    long long qx = voxel_of(xyz[3 * i], voxel), qy = voxel_of(xyz[3 * i + 1], voxel),
-              qz = voxel_of(xyz[3 * i + 2], voxel);
-    if (!in_box(qx, qy, qz, g)) {
-        atomicAdd(counters + 2, 1ull);
-        return;
-    }
-    unsigned long long a, b;
-    wide_key(qx - g.q0[0], qy - g.q0[1], qz - g.q0[2], a, b);
-    uint64_t s = wide_find_or_insert(a, b, ha, hb, slot_mask, true);
-    int old = atomicAdd(hcnt + s, 1);
-    if (old == 0) atomicAdd(counters + 1, 1ull);
-    if (old + 1 == thr) {
-        unsigned long long slot = atomicAdd(counters, 1ull);
-        if ((int64_t)slot < cap) {
-            dense_vox[3 * slot] = qx;
-            dense_vox[3 * slot + 1] = qy;
-            dense_vox[3 * slot + 2] = qz;
-        }
-    }
-}
-
-__global__ void k_vox_dense_counts_hash_wide(const long long* __restrict__ dense_vox, int64_t nd, VoxGrid g,
-                                             unsigned long long* ha, unsigned long long* hb,
-                                             const int* __restrict__ hcnt, uint64_t slot_mask,
-                                             int* __restrict__ dense_cnt) {
-    int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (t >= nd) return;
-    unsigned long long a, b;
-    wide_key(dense_vox[3 * t] - g.q0[0], dense_vox[3 * t + 1] - g.q0[1], dense_vox[3 * t + 2] - g.q0[2], a, b);
-    uint64_t s = wide_find_or_insert(a, b, ha, hb, slot_mask, false);
-    dense_cnt[t] = s == ~0ull ? 0 : hcnt[s];
+    dense_cnt[t] = tab.find(g, dense_vox[3 * t], dense_vox[3 * t + 1], dense_vox[3 * t + 2]);
 }
 
 int density_voxel_count(const float* xyz, int64_t n, float voxel, int64_t min_points, int64_t* dense_vox_host,
@@ -423,88 +399,72 @@ int density_voxel_count(const float* xyz, int64_t n, float voxel, int64_t min_po
     GSX_REQUIRE(thr_ll < 2147483647ll, GSX_ERR_ARG, "density: min_points too large");
     int thr = (int)thr_ll;
     GSX_CUDA_CHECK(cudaMemsetAsync(counters, 0, 4 * sizeof(unsigned long long), st));
-    int blocks = (int)((n + 255) / 256);
-    bool use_grid = cells * 4.0 <= (double)blob_bytes;
-    uint64_t slot_mask = 0;
-    unsigned long long* hkeys = nullptr;
-    unsigned long long* hkeys_b = nullptr;
-    int* hcnt = nullptr;
-    if (use_grid) {
-        size_t ncell = (size_t)g.dim[0] * g.dim[1] * g.dim[2];
+    auto count_rows = [&](const auto& tab) {
+        k_vox_count<true><<<(int)((n + 255) / 256), 256, 0, st>>>(xyz, n, voxel, g, tab, thr, counters, dvox, cap,
+                                                                  counters + kOutside);
+    };
+    // After the histogram: the refusals, then the counts of the dense voxels looked up in `tab`.
+    auto read_dense = [&](const auto& tab) -> int {
+        GSX_KERNEL_CHECK();
+        unsigned long long hc[3];   // counters[kDense], [kDistinct], [kOutside]
+        GSX_CUDA_CHECK(cudaMemcpyAsync(hc, counters, sizeof(hc), cudaMemcpyDeviceToHost, st));
+        GSX_CUDA_CHECK(cudaStreamSynchronize(st));
+        *n_dense_host = (int64_t)hc[kDense];
+        if (n_voxels_host) *n_voxels_host = (int64_t)hc[kDistinct];
+        // The reference puts a NaN row in a voxel outside the finite box.  Fewer than thr such rows make no dense
+        // voxel, so dropping them is exact; with thr or more, one of those voxels may be dense, and that is refused.
+        GSX_REQUIRE(hc[kOutside] < (unsigned long long)thr, GSX_ERR_UNSUPPORTED,
+                    "density: %llu points have non-finite (NaN) coordinates, at least min_points = %d", hc[kOutside],
+                    thr);
+        GSX_REQUIRE((int64_t)hc[kDense] <= cap, GSX_ERR_WORKSPACE, "density: %llu dense voxels exceed cap %lld",
+                    hc[kDense], (long long)cap);
+        const int64_t nd = (int64_t)hc[kDense];
+        if (nd > 0) {
+            k_vox_dense_counts<<<(int)((nd + 127) / 128), 128, 0, st>>>(dvox, nd, g, tab, dcnt);
+            GSX_KERNEL_CHECK();
+            GSX_CUDA_CHECK(cudaMemcpyAsync(dense_vox_host, dvox, (size_t)nd * 24, cudaMemcpyDeviceToHost, st));
+            GSX_CUDA_CHECK(cudaMemcpyAsync(dense_cnt_host, dcnt, (size_t)nd * 4, cudaMemcpyDeviceToHost, st));
+            GSX_CUDA_CHECK(cudaStreamSynchronize(st));
+        }
+        return GSX_OK;
+    };
+
+    if (cells * 4.0 <= (double)blob_bytes) {
+        const GridTable tab{(int*)blob};
+        const size_t ncell = (size_t)g.dim[0] * g.dim[1] * g.dim[2];
         GSX_CUDA_CHECK(cudaMemsetAsync(blob, 0, ncell * 4, st));
         if (ncell <= (size_t)kSmemCells) {
-            int rc2 = launch_vox_count_smem(xyz, n, voxel, g, ncell, thr, (int*)blob, counters, dvox, cap, counters + 2,
-                                            st);
-            if (rc2) return rc2;
+            rc = launch_vox_count_smem(xyz, n, voxel, g, ncell, thr, tab.cnt, counters, dvox, cap, counters + kOutside,
+                                       st);
+            if (rc) return rc;
         } else if (ncell < 0xfffffff0ull) {
-            int ablocks = (int)((n + 256 * kAggItems - 1) / (256 * kAggItems));
-            k_vox_count_grid_agg<<<ablocks, 256, 0, st>>>(xyz, n, voxel, g, thr, (int*)blob, counters, dvox, cap);
+            const int ablocks = (int)((n + 256 * kAggItems - 1) / (256 * kAggItems));
+            k_vox_count_grid_agg<<<ablocks, 256, 0, st>>>(xyz, n, voxel, g, thr, tab.cnt, counters, dvox, cap);
         } else {
-            k_vox_count_grid<<<blocks, 256, 0, st>>>(xyz, n, voxel, g, thr, (int*)blob, counters, dvox, cap);
+            count_rows(tab);
         }
-    } else {
-        size_t slots = 64;
-        while (slots < (size_t)2 * n) slots <<= 1;
-        GSX_REQUIRE(slots * 12 <= blob_bytes, GSX_ERR_WORKSPACE, "density: workspace too small for the hash table");
-        hkeys = (unsigned long long*)blob;
-        hcnt = (int*)(blob + slots * 8);
-        slot_mask = slots - 1;
-        if (!wide) {
-            GSX_CUDA_CHECK(cudaMemsetAsync(blob, 0, slots * 12, st));
-            k_vox_count_hash<<<blocks, 256, 0, st>>>(xyz, n, voxel, g, thr, hkeys, hcnt, slot_mask, counters, dvox, cap);
-        } else {  // two-word keys in the same budget: half the slots (still >= n), 20 bytes each
-            slots >>= 1;
-            hkeys_b = hkeys + slots;
-            hcnt = (int*)(blob + slots * 16);
-            slot_mask = slots - 1;
-            GSX_CUDA_CHECK(cudaMemsetAsync(blob, 0, slots * 20, st));
-            k_vox_count_hash_wide<<<blocks, 256, 0, st>>>(xyz, n, voxel, g, thr, hkeys, hkeys_b, hcnt, slot_mask,
-                                                          counters, dvox, cap);
-        }
+        return read_dense(tab);
     }
-    GSX_KERNEL_CHECK();
-    unsigned long long hc[3];   // dense voxels, distinct voxels, points outside the box
-    GSX_CUDA_CHECK(cudaMemcpyAsync(hc, counters, sizeof(hc), cudaMemcpyDeviceToHost, st));
-    GSX_CUDA_CHECK(cudaStreamSynchronize(st));
-    *n_dense_host = (int64_t)hc[0];
-    if (n_voxels_host) *n_voxels_host = (int64_t)hc[1];
-    // The reference puts a NaN row in a voxel outside the finite box.  Fewer than thr such rows make no dense voxel,
-    // so dropping them is exact; with thr or more, one of those voxels may be dense, and that is refused.
-    GSX_REQUIRE(hc[2] < (unsigned long long)thr, GSX_ERR_UNSUPPORTED,
-                "density: %llu points have non-finite (NaN) coordinates, at least min_points = %d", hc[2], thr);
-    GSX_REQUIRE((int64_t)hc[0] <= cap, GSX_ERR_WORKSPACE, "density: %llu dense voxels exceed cap %lld", hc[0],
-                (long long)cap);
-    int64_t nd = (int64_t)hc[0];
-    if (nd > 0) {
-        int b2 = (int)((nd + 127) / 128);
-        if (use_grid) k_vox_dense_counts_grid<<<b2, 128, 0, st>>>(dvox, nd, g, (const int*)blob, dcnt);
-        else if (!wide) k_vox_dense_counts_hash<<<b2, 128, 0, st>>>(dvox, nd, g, hkeys, hcnt, slot_mask, dcnt);
-        else k_vox_dense_counts_hash_wide<<<b2, 128, 0, st>>>(dvox, nd, g, hkeys, hkeys_b, hcnt, slot_mask, dcnt);
-        GSX_KERNEL_CHECK();
-        GSX_CUDA_CHECK(cudaMemcpyAsync(dense_vox_host, dvox, (size_t)nd * 24, cudaMemcpyDeviceToHost, st));
-        GSX_CUDA_CHECK(cudaMemcpyAsync(dense_cnt_host, dcnt, (size_t)nd * 4, cudaMemcpyDeviceToHost, st));
-        GSX_CUDA_CHECK(cudaStreamSynchronize(st));
+    size_t slots = 64;
+    while (slots < (size_t)2 * n) slots <<= 1;
+    GSX_REQUIRE(slots * 12 <= blob_bytes, GSX_ERR_WORKSPACE, "density: workspace too small for the hash table");
+    if (!wide) {
+        const HashTable tab{(unsigned long long*)blob, (int*)(blob + slots * 8), slots - 1};
+        GSX_CUDA_CHECK(cudaMemsetAsync(blob, 0, slots * 12, st));
+        count_rows(tab);
+        return read_dense(tab);
     }
-    return GSX_OK;
+    slots >>= 1;   // two-word keys in the same budget: half the slots (still >= n), 20 bytes each
+    const WideHashTable tab{(unsigned long long*)blob, (unsigned long long*)blob + slots, (int*)(blob + slots * 16),
+                            slots - 1};
+    GSX_CUDA_CHECK(cudaMemsetAsync(blob, 0, slots * 20, st));
+    count_rows(tab);
+    return read_dense(tab);
 }
 
 // ---------------------------------------------------------------- staged dense-grid API (multi-GPU)
 // Rank-local histogram into a caller-owned int32 grid over a caller-chosen voxel box (the global one);
 // the caller all-reduces the grid and then extracts the dense voxels.
-__global__ void __launch_bounds__(256) k_vox_count_grid_only(const float* __restrict__ xyz, int64_t n, float voxel,
-                                                             VoxGrid g, int* __restrict__ grid,
-                                                             unsigned long long* __restrict__ oob) {
-    int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const long long qx = voxel_of(xyz[3 * i], voxel), qy = voxel_of(xyz[3 * i + 1], voxel),
-                    qz = voxel_of(xyz[3 * i + 2], voxel);
-    if (!in_box(qx, qy, qz, g)) {
-        atomicAdd(oob, 1ull);
-        return;
-    }
-    atomicAdd(grid + ((size_t)(qx - g.q0[0]) * g.dim[1] + (size_t)(qy - g.q0[1])) * g.dim[2] + (size_t)(qz - g.q0[2]), 1);
-}
-
 __global__ void __launch_bounds__(256) k_vox_grid_dense(const int* __restrict__ grid, size_t ncell, VoxGrid g, int thr,
                                                         unsigned long long* __restrict__ counters,
                                                         long long* __restrict__ dense_vox,
@@ -512,18 +472,10 @@ __global__ void __launch_bounds__(256) k_vox_grid_dense(const int* __restrict__ 
     size_t c = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (c >= ncell) return;
     int v = grid[c];
-    if (v > 0) atomicAdd(counters + 1, 1ull);
+    if (v > 0) atomicAdd(counters + kDistinct, 1ull);
     if (v >= thr) {
-        unsigned long long slot = atomicAdd(counters, 1ull);
-        if ((int64_t)slot < cap) {
-            long long z = (long long)(c % (size_t)g.dim[2]);
-            long long y = (long long)((c / (size_t)g.dim[2]) % (size_t)g.dim[1]);
-            long long x = (long long)(c / ((size_t)g.dim[2] * (size_t)g.dim[1]));
-            dense_vox[3 * slot] = x + g.q0[0];
-            dense_vox[3 * slot + 1] = y + g.q0[1];
-            dense_vox[3 * slot + 2] = z + g.q0[2];
-            dense_cnt[slot] = v;
-        }
+        const unsigned long long slot = dense_append(counters, dense_vox, cap, [&] { return g.voxel(c); });
+        if ((int64_t)slot < cap) dense_cnt[slot] = v;
     }
 }
 
@@ -559,7 +511,8 @@ int density_grid_count(const float* xyz, int64_t n, float voxel, const int64_t* 
         rc = launch_vox_count_smem(xyz, n, voxel, g, ncell, 0, grid_dev, nullptr, nullptr, 0, oob_dev, st);
         if (rc) return rc;
     } else {
-        k_vox_count_grid_only<<<(int)((n + 255) / 256), 256, 0, st>>>(xyz, n, voxel, g, grid_dev, oob_dev);
+        k_vox_count<false><<<(int)((n + 255) / 256), 256, 0, st>>>(xyz, n, voxel, g, GridTable{grid_dev}, 0, nullptr,
+                                                                   nullptr, 0, oob_dev);
     }
     GSX_KERNEL_CHECK();
     return GSX_OK;
@@ -584,127 +537,121 @@ int density_grid_dense(const int* grid_dev, const int64_t* q0, const int64_t* di
     k_vox_grid_dense<<<(unsigned)((ncell + 255) / 256), 256, 0, st>>>(grid_dev, ncell, g, (int)thr_ll, counters, dvox,
                                                                       dcnt, cap);
     GSX_KERNEL_CHECK();
-    unsigned long long hc[2];
+    unsigned long long hc[2];   // counters[kDense], [kDistinct]
     GSX_CUDA_CHECK(cudaMemcpyAsync(hc, counters, sizeof(hc), cudaMemcpyDeviceToHost, st));
     GSX_CUDA_CHECK(cudaStreamSynchronize(st));
-    *n_dense_host = (int64_t)hc[0];
-    if (n_voxels_host) *n_voxels_host = (int64_t)hc[1];
-    GSX_REQUIRE((int64_t)hc[0] <= cap, GSX_ERR_WORKSPACE, "density: %llu dense voxels exceed cap %lld", hc[0],
-                (long long)cap);
-    if (hc[0] > 0) {
-        GSX_CUDA_CHECK(cudaMemcpyAsync(dense_vox_host, dvox, (size_t)hc[0] * 24, cudaMemcpyDeviceToHost, st));
-        GSX_CUDA_CHECK(cudaMemcpyAsync(dense_cnt_host, dcnt, (size_t)hc[0] * 4, cudaMemcpyDeviceToHost, st));
+    *n_dense_host = (int64_t)hc[kDense];
+    if (n_voxels_host) *n_voxels_host = (int64_t)hc[kDistinct];
+    GSX_REQUIRE((int64_t)hc[kDense] <= cap, GSX_ERR_WORKSPACE, "density: %llu dense voxels exceed cap %lld",
+                hc[kDense], (long long)cap);
+    if (hc[kDense] > 0) {
+        GSX_CUDA_CHECK(cudaMemcpyAsync(dense_vox_host, dvox, (size_t)hc[kDense] * 24, cudaMemcpyDeviceToHost, st));
+        GSX_CUDA_CHECK(cudaMemcpyAsync(dense_cnt_host, dcnt, (size_t)hc[kDense] * 4, cudaMemcpyDeviceToHost, st));
         GSX_CUDA_CHECK(cudaStreamSynchronize(st));
     }
     return GSX_OK;
 }
 
 // ---------------------------------------------------------------- membership mask
+// Keep sets: contains() tells whether a voxel is one of the kept voxels.  The host builds the set in the workspace.
+
+// Bitmap form: when the bounding box of the kept voxels is small (the usual case -- a few clusters of voxels of one
+// scene unit) one bit per voxel of that box replaces the hash probe: the whole set is a few KiB that stay in L1, and
+// the kernel streams at the speed of the bbox mask instead of waiting on dependent table reads.
+struct VoxBits {
+    long long ox, oy, oz;
+    unsigned long long dx, dy, dz;
+    const uint32_t* bits;
+    __device__ __forceinline__ uint8_t contains(long long qx, long long qy, long long qz) const {
+        const unsigned long long rx = (unsigned long long)(qx - ox), ry = (unsigned long long)(qy - oy),
+                                 rz = (unsigned long long)(qz - oz);
+        if (rx >= dx || ry >= dy || rz >= dz) return 0;    // (negative differences wrap to huge values)
+        const uint32_t idx = (uint32_t)((rx * dy + ry) * dz + rz);
+        return (uint8_t)((__ldg(bits + (idx >> 5)) >> (idx & 31u)) & 1u);
+    }
+};
+
+// Hash form: the keys of HashTable (one word per slot), or for kept voxels that span >= 2^21 on some axis the
+// two-word keys of WideHashTable with {a, b} at set[2s], set[2s+1].
 template <bool WIDE>
-__device__ __forceinline__ uint8_t vox_member_one(float x, float y, float z, float voxel, long long ox,
-                                                  long long oy, long long oz,
-                                                  const unsigned long long* __restrict__ set, uint64_t slot_mask) {
-    long long rx = voxel_of(x, voxel) - ox, ry = voxel_of(y, voxel) - oy, rz = voxel_of(z, voxel) - oz;
-    if (WIDE) {  // two-word keys {a, b} at set[2s], set[2s+1]: kept voxels that span >= 2^21 on some axis
-        if (rx < 0 || ry < 0 || rz < 0 || rx >= (1ll << 31) || ry >= (1ll << 31) || rz >= (1ll << 31)) return 0;
-        unsigned long long a, b;
-        wide_key(rx, ry, rz, a, b);
-        uint64_t s = mix64(a ^ mix64(b)) & slot_mask;
+struct KeepHash {
+    long long ox, oy, oz;
+    const unsigned long long* set;
+    uint64_t slot_mask;
+    __device__ __forceinline__ uint8_t contains(long long qx, long long qy, long long qz) const {
+        const long long rx = qx - ox, ry = qy - oy, rz = qz - oz;
+        if (WIDE) {
+            if (rx < 0 || ry < 0 || rz < 0 || rx >= (1ll << 31) || ry >= (1ll << 31) || rz >= (1ll << 31)) return 0;
+            unsigned long long a, b;
+            wide_key(rx, ry, rz, a, b);
+            uint64_t s = wide_slot(a, b) & slot_mask;
+            for (;;) {
+                unsigned long long ca = __ldg(set + 2 * s);
+                if (ca == 0ull) return 0;
+                if (ca == a && __ldg(set + 2 * s + 1) == b) return 1;
+                s = (s + 1) & slot_mask;
+            }
+        }
+        if (rx < 0 || ry < 0 || rz < 0 || rx >= kAxisLim || ry >= kAxisLim || rz >= kAxisLim) return 0;
+        uint64_t key = pack_rel(rx, ry, rz);
+        uint64_t s = mix64(key) & slot_mask;
         for (;;) {
-            unsigned long long ca = __ldg(set + 2 * s);
-            if (ca == 0ull) return 0;
-            if (ca == a && __ldg(set + 2 * s + 1) == b) return 1;
+            unsigned long long cur = __ldg(set + s);
+            if (cur == key) return 1;
+            if (cur == 0ull) return 0;
             s = (s + 1) & slot_mask;
         }
     }
-    if (rx < 0 || ry < 0 || rz < 0 || rx >= kAxisLim || ry >= kAxisLim || rz >= kAxisLim) return 0;
-    uint64_t key = pack_rel(rx, ry, rz);
-    uint64_t s = mix64(key) & slot_mask;
-    for (;;) {
-        unsigned long long cur = __ldg(set + s);
-        if (cur == key) return 1;
-        if (cur == 0ull) return 0;
-        s = (s + 1) & slot_mask;
-    }
+};
+
+template <class Set>
+__device__ __forceinline__ uint8_t vox_member(const Set& set, float x, float y, float z, float voxel) {
+    return set.contains(voxel_of(x, voxel), voxel_of(y, voxel), voxel_of(z, voxel));
 }
 
-template <bool WIDE>
+template <class Set>
 __global__ void __launch_bounds__(256) k_vox_member(const float* __restrict__ xyz, int64_t begin, int64_t n,
-                                                    float voxel, long long ox, long long oy, long long oz,
-                                                    const unsigned long long* __restrict__ set, uint64_t slot_mask,
-                                                    uint8_t* __restrict__ mask) {
+                                                    float voxel, Set set, uint8_t* __restrict__ mask) {
     int64_t i = begin + (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    mask[i] = vox_member_one<WIDE>(xyz[3 * i], xyz[3 * i + 1], xyz[3 * i + 2], voxel, ox, oy, oz, set, slot_mask);
+    mask[i] = vox_member(set, xyz[3 * i], xyz[3 * i + 1], xyz[3 * i + 2], voxel);
 }
 
 // 4 points (3 x 128-bit loads) per thread, uchar4 store
-template <bool WIDE>
-__global__ void __launch_bounds__(256) k_vox_member4(const float4* __restrict__ xyz4, int64_t n4, float voxel,
-                                                     long long ox, long long oy, long long oz,
-                                                     const unsigned long long* __restrict__ set, uint64_t slot_mask,
+template <class Set>
+__global__ void __launch_bounds__(256) k_vox_member4(const float4* __restrict__ xyz4, int64_t n4, float voxel, Set set,
                                                      uchar4* __restrict__ mask4) {
     int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= n4) return;
     float4 a = ld_stream_f4(xyz4 + 3 * t), b = ld_stream_f4(xyz4 + 3 * t + 1), c = ld_stream_f4(xyz4 + 3 * t + 2);
     uchar4 o;
-    o.x = vox_member_one<WIDE>(a.x, a.y, a.z, voxel, ox, oy, oz, set, slot_mask);
-    o.y = vox_member_one<WIDE>(a.w, b.x, b.y, voxel, ox, oy, oz, set, slot_mask);
-    o.z = vox_member_one<WIDE>(b.z, b.w, c.x, voxel, ox, oy, oz, set, slot_mask);
-    o.w = vox_member_one<WIDE>(c.y, c.z, c.w, voxel, ox, oy, oz, set, slot_mask);
+    o.x = vox_member(set, a.x, a.y, a.z, voxel);
+    o.y = vox_member(set, a.w, b.x, b.y, voxel);
+    o.z = vox_member(set, b.z, b.w, c.x, voxel);
+    o.w = vox_member(set, c.y, c.z, c.w, voxel);
     mask4[t] = o;
 }
 
-// Bitmap form of the keep set: when the bounding box of the kept voxels is small (the usual case -- a few clusters of
-// voxels of one scene unit) one bit per voxel of that box replaces the hash probe: the whole set is a few KiB that stay
-// in L1, and the kernel streams at the speed of the bbox mask instead of waiting on dependent table reads.
-struct VoxBits {
-    long long ox, oy, oz;
-    unsigned long long dx, dy, dz;
-};
-
-__device__ __forceinline__ uint8_t vox_member_bit(float x, float y, float z, float voxel, const VoxBits& g,
-                                                  const uint32_t* __restrict__ bits) {
-    const unsigned long long rx = (unsigned long long)(voxel_of(x, voxel) - g.ox),
-                             ry = (unsigned long long)(voxel_of(y, voxel) - g.oy),
-                             rz = (unsigned long long)(voxel_of(z, voxel) - g.oz);
-    if (rx >= g.dx || ry >= g.dy || rz >= g.dz) return 0;    // (negative differences wrap to huge values)
-    const uint32_t idx = (uint32_t)((rx * g.dy + ry) * g.dz + rz);
-    return (uint8_t)((__ldg(bits + (idx >> 5)) >> (idx & 31u)) & 1u);
-}
-
-__global__ void __launch_bounds__(256) k_vox_member_bits(const float* __restrict__ xyz, int64_t begin, int64_t n,
-                                                         float voxel, VoxBits g, const uint32_t* __restrict__ bits,
-                                                         uint8_t* __restrict__ mask) {
-    int64_t i = begin + (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    mask[i] = vox_member_bit(xyz[3 * i], xyz[3 * i + 1], xyz[3 * i + 2], voxel, g, bits);
-}
-
-__global__ void __launch_bounds__(256) k_vox_member_bits4(const float4* __restrict__ xyz4, int64_t n4, float voxel,
-                                                          VoxBits g, const uint32_t* __restrict__ bits,
-                                                          uchar4* __restrict__ mask4) {
-    int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (t >= n4) return;
-    float4 a = ld_stream_f4(xyz4 + 3 * t), b = ld_stream_f4(xyz4 + 3 * t + 1), c = ld_stream_f4(xyz4 + 3 * t + 2);
-    uchar4 o;
-    o.x = vox_member_bit(a.x, a.y, a.z, voxel, g, bits);
-    o.y = vox_member_bit(a.w, b.x, b.y, voxel, g, bits);
-    o.z = vox_member_bit(b.z, b.w, c.x, voxel, g, bits);
-    o.w = vox_member_bit(c.y, c.z, c.w, voxel, g, bits);
-    mask4[t] = o;
+// The 4-wide kernel over whole groups of 4 rows when xyz is 16-byte and the mask 4-byte aligned, the scalar one over
+// the rest.
+template <class Set>
+static int launch_member(const float* xyz, int64_t n, float voxel, const Set& set, uint8_t* mask, cudaStream_t st) {
+    int64_t n4 = 0;
+    if (((uintptr_t)xyz % 16 == 0) && ((uintptr_t)mask % 4 == 0)) {
+        n4 = n / 4;
+        if (n4 > 0) {
+            k_vox_member4<<<(int)((n4 + 255) / 256), 256, 0, st>>>((const float4*)xyz, n4, voxel, set, (uchar4*)mask);
+            GSX_KERNEL_CHECK();
+        }
+    }
+    if (n - 4 * n4 > 0) {
+        k_vox_member<<<(int)((n - 4 * n4 + 255) / 256), 256, 0, st>>>(xyz, 4 * n4, n, voxel, set, mask);
+        GSX_KERNEL_CHECK();
+    }
+    return GSX_OK;
 }
 
 constexpr unsigned long long kMaxKeepBits = 1ull << 27;   // 16 MiB of bitmap at most; larger boxes use the hash set
-
-static bool keep_bitmap_enabled() {
-    static int v = -1;
-    if (v < 0) {
-        const char* e = getenv("GSX_DENSITY_BITMAP");
-        v = !(e && e[0] == '0');
-    }
-    return v != 0;
-}
 
 int density_member_mask(const float* xyz, int64_t n, float voxel, const int64_t* keep, int64_t n_keep, uint8_t* mask,
                         void* ws, int64_t ws_bytes, cudaStream_t st) {
@@ -733,7 +680,7 @@ int density_member_mask(const float* xyz, int64_t n, float voxel, const int64_t*
         const bool small = dx <= kMaxKeepBits && dy <= kMaxKeepBits && dx * dy <= kMaxKeepBits &&
                            dx * dy * dz <= kMaxKeepBits;
         const size_t nwords = small ? (size_t)((dx * dy * dz + 31) / 32) : 0;
-        if (small && keep_bitmap_enabled() && nwords * 4 <= (size_t)ws_bytes) {
+        if (small && nwords * 4 <= (size_t)ws_bytes) {
             std::vector<uint32_t> bm(nwords, 0u);
             for (int64_t t = 0; t < n_keep; ++t) {
                 const unsigned long long idx = ((unsigned long long)(keep[3 * t] - o[0]) * dy +
@@ -743,22 +690,7 @@ int density_member_mask(const float* xyz, int64_t n, float voxel, const int64_t*
             }
             GSX_CUDA_CHECK(cudaMemcpyAsync(ws, bm.data(), nwords * 4, cudaMemcpyHostToDevice, st));
             GSX_CUDA_CHECK(cudaStreamSynchronize(st));  // bm is a stack-owned pageable buffer
-            const VoxBits g{o[0], o[1], o[2], dx, dy, dz};
-            const uint32_t* bits = (const uint32_t*)ws;
-            int64_t n4 = 0;
-            if (((uintptr_t)xyz % 16 == 0) && ((uintptr_t)mask % 4 == 0)) {
-                n4 = n / 4;
-                if (n4 > 0) {
-                    k_vox_member_bits4<<<(int)((n4 + 255) / 256), 256, 0, st>>>((const float4*)xyz, n4, voxel, g, bits,
-                                                                               (uchar4*)mask);
-                    GSX_KERNEL_CHECK();
-                }
-            }
-            if (n - 4 * n4 > 0) {
-                k_vox_member_bits<<<(int)((n - 4 * n4 + 255) / 256), 256, 0, st>>>(xyz, 4 * n4, n, voxel, g, bits, mask);
-                GSX_KERNEL_CHECK();
-            }
-            return GSX_OK;
+            return launch_member(xyz, n, voxel, VoxBits{o[0], o[1], o[2], dx, dy, dz, (const uint32_t*)ws}, mask, st);
         }
     }
     size_t slots = 64;
@@ -767,16 +699,16 @@ int density_member_mask(const float* xyz, int64_t n, float voxel, const int64_t*
     GSX_REQUIRE(slots * 8 * words <= (size_t)ws_bytes, GSX_ERR_WORKSPACE, "density: workspace too small for the keep set");
     std::vector<unsigned long long> tab(slots * words, 0ull);
     for (int64_t t = 0; t < n_keep; ++t) {
-        const uint64_t rx = (uint64_t)(keep[3 * t] - o[0]), ry = (uint64_t)(keep[3 * t + 1] - o[1]),
-                       rz = (uint64_t)(keep[3 * t + 2] - o[2]);
+        const long long rx = keep[3 * t] - o[0], ry = keep[3 * t + 1] - o[1], rz = keep[3 * t + 2] - o[2];
         if (!wide) {
-            uint64_t key = ((rx << (2 * kAxisBits)) | (ry << kAxisBits) | rz) + 1ull;
-            uint64_t s = mix64_host(key) & (slots - 1);
+            const uint64_t key = pack_rel(rx, ry, rz);
+            uint64_t s = mix64(key) & (slots - 1);
             while (tab[s] != 0ull && tab[s] != key) s = (s + 1) & (slots - 1);
             tab[s] = key;
         } else {
-            uint64_t a = ((rx << 32) | ry) + 1ull, b = rz + 1ull;
-            uint64_t s = mix64_host(a ^ mix64_host(b)) & (slots - 1);
+            unsigned long long a, b;
+            wide_key(rx, ry, rz, a, b);
+            uint64_t s = wide_slot(a, b) & (slots - 1);
             while (tab[2 * s] != 0ull && !(tab[2 * s] == a && tab[2 * s + 1] == b)) s = (s + 1) & (slots - 1);
             tab[2 * s] = a;
             tab[2 * s + 1] = b;
@@ -785,23 +717,8 @@ int density_member_mask(const float* xyz, int64_t n, float voxel, const int64_t*
     GSX_CUDA_CHECK(cudaMemcpyAsync(ws, tab.data(), slots * 8 * words, cudaMemcpyHostToDevice, st));
     GSX_CUDA_CHECK(cudaStreamSynchronize(st));  // tab is a stack-owned pageable buffer
     const unsigned long long* set = (const unsigned long long*)ws;
-    int64_t n4 = 0;
-    if (((uintptr_t)xyz % 16 == 0) && ((uintptr_t)mask % 4 == 0)) {
-        n4 = n / 4;
-        if (n4 > 0) {
-            const int b4 = (int)((n4 + 255) / 256);
-            if (wide) k_vox_member4<true><<<b4, 256, 0, st>>>((const float4*)xyz, n4, voxel, o[0], o[1], o[2], set, slots - 1, (uchar4*)mask);
-            else k_vox_member4<false><<<b4, 256, 0, st>>>((const float4*)xyz, n4, voxel, o[0], o[1], o[2], set, slots - 1, (uchar4*)mask);
-            GSX_KERNEL_CHECK();
-        }
-    }
-    if (n - 4 * n4 > 0) {
-        const int b1 = (int)((n - 4 * n4 + 255) / 256);
-        if (wide) k_vox_member<true><<<b1, 256, 0, st>>>(xyz, 4 * n4, n, voxel, o[0], o[1], o[2], set, slots - 1, mask);
-        else k_vox_member<false><<<b1, 256, 0, st>>>(xyz, 4 * n4, n, voxel, o[0], o[1], o[2], set, slots - 1, mask);
-        GSX_KERNEL_CHECK();
-    }
-    return GSX_OK;
+    if (wide) return launch_member(xyz, n, voxel, KeepHash<true>{o[0], o[1], o[2], set, slots - 1}, mask, st);
+    return launch_member(xyz, n, voxel, KeepHash<false>{o[0], o[1], o[2], set, slots - 1}, mask, st);
 }
 
 }  // namespace gsx

@@ -15,7 +15,7 @@ Constants these cases are built around (csrc/gsx_density.cu): a voxel box of <= 
 memory by persistent 512-thread CTAs (`k_vox_count_smem`, 4 rows per float4 group, ragged tail of < 4 rows read by
 block 0, scalar loads when xyz is not 16-byte aligned), a larger box that fits the workspace by `k_vox_count_grid_agg`
 (2 048 rows per CTA into a 1 024-slot shared table, eight probes, then one global add per row), a box of 2^32 - 16
-cells or more by `k_vox_count_grid`; a box that does not fit the workspace goes to the hash table, with 3 x 21-bit
+cells or more by `k_vox_count<GridTable>`; a box that does not fit the workspace goes to the hash table, with 3 x 21-bit
 keys, or two-word keys when an extent reaches 2^21.  The kept voxels are a bitmap when their box has <= 2^27 voxels
 and the bitmap fits the workspace, a hash set otherwise.
 
@@ -526,7 +526,7 @@ def test_count_form_reaches_branch(form, n):
 
 
 def test_plain_grid_kernel_threshold():
-    """k_vox_count_grid runs for a box of >= 2^32 - 16 cells held as a grid, i.e. blob >= 4 (2^32 - 16) bytes.  The
+    """k_vox_count<GridTable> runs for a box of >= 2^32 - 16 cells held as a grid, i.e. blob >= 4 (2^32 - 16) bytes.  The
     blob grows with the hash table of >= 2n slots (12 bytes each), so the smallest n that reaches it is stated here;
     the kernel is not run at that size."""
     n = 1
