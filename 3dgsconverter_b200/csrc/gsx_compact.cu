@@ -175,6 +175,9 @@ int compact_points(const uint8_t* mask, int64_t n, const float* xyz, const float
         *count_host = 0;
         return GSX_OK;
     }
+    // the surviving row indices are int32 (a row >= 2^31 would wrap) and the two-pass positions uint32
+    GSX_REQUIRE(n < (1ll << 31), GSX_ERR_UNSUPPORTED, "compact: n = %lld rows, int32 row indices need n < 2^31",
+                (long long)n);
     GSX_REQUIRE(ws_bytes >= compact_workspace_bytes(n), GSX_ERR_WORKSPACE, "compact: workspace too small");
     GSX_REQUIRE((opacity == nullptr) == (opacity_out == nullptr), GSX_ERR_ARG, "compact: opacity in/out mismatch");
     if (n < (1ll << 30)) {   // the look-back words carry 30-bit survivor counts (kLbVal)

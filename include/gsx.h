@@ -183,7 +183,8 @@ double gsx_alpha_logit_threshold(double min_opacity_u8);
 /* ---- compaction of the filters' working set: the `vertices[mask]` steps of data_processor.py:114,149,209,
  * 217-224 for the columns the filters read (xyz, opacity) plus the surviving ORIGINAL row indices; stable like
  * NumPy boolean indexing.  opacity_dev/opacity_out_dev may both be NULL; idx_dev NULL = identity.
- * *count_host = number of survivors (one 4-byte D2H sync). */
+ * *count_host = number of survivors (one 4-byte D2H sync).  Any non-zero mask byte keeps its row.
+ * n >= 2^31 is refused with GSX_ERR_UNSUPPORTED (the surviving row indices are int32). */
 int64_t gsx_compact_workspace_bytes(int64_t n);
 int gsx_compact_points(const uint8_t* mask_dev, int64_t n, const float* xyz_dev, const float* opacity_dev,
                        const int32_t* idx_dev, float* xyz_out_dev, float* opacity_out_dev, int32_t* idx_out_dev,

@@ -86,7 +86,7 @@ def test_mean_std_matches_numpy(cuda, gsx_lib):
     import torch
     from gsx import sor
     rng = np.random.default_rng(11)
-    for n in (1, 5, 8, 9, 27, 100, 128, 129, 1000, 4097, 100_003, 3_000_001, 16_777_216 + 5):
+    for n in (1, 5, 8, 9, 27, 100, 128, 129, 264, 1000, 4097, 100_003, 131_073, 3_000_001, 16_777_216 + 5):
         a = rng.gamma(2.0, 0.3, n).astype(np.float32)
         want = np.array([np.mean(a), np.std(a)], dtype=np.float32)
         # 16-byte aligned vector: two lanes per leaf with float4 loads; offset by one element: the 8-lanes-per-leaf kernel

@@ -9,7 +9,8 @@ pytestmark = pytest.mark.gpu
 
 
 @pytest.mark.parametrize("sizes", [(1000, 1000), (4097, 1, 0, 300, 129), (100_003, 50_000, 77), (5, 3), (3_000_001, 7, 999_992),
-                                   (128, 128, 128, 128), (127, 130)])
+                                   (128, 128, 128, 128), (127, 130),
+                                   (0, 300, 500), (400, 129, 0), (5, 20, 0, 17, 3, 11, 0, 9)])
 def test_sharded_mean_std_matches_numpy(sizes, cuda, gsx_lib):
     import torch
     from gsx._abi import lib, check
