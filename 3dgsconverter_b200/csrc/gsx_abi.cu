@@ -22,6 +22,7 @@
 #include "gsx_sog_decode.cuh"
 #include "gsx_sor.cuh"
 #include "gsx_splat_codecs.cuh"
+#include "gsx_webp.cuh"
 
 #include <atomic>
 #include <math.h>
@@ -502,6 +503,26 @@ int gsx_sog_labels(const int32_t* labels_dev, int64_t n, int64_t chunk_size, int
 int gsx_sog_centroids(const float* palette_dev, int64_t P, int32_t coeffs, const float* cb_dev, int32_t m,
                       int64_t pixels, uint8_t* out_dev, void* stream) {
     return sog_centroids(palette_dev, P, coeffs, cb_dev, m, pixels, out_dev, (cudaStream_t)stream);
+}
+
+/* ------------------------------------------------------------------ lossless WebP */
+
+int64_t gsx_webp_workspace_bytes(int64_t width, int64_t height) { return webp_workspace_bytes(width, height); }
+
+int gsx_webp_analyze(const uint8_t* rgba_dev, int64_t width, int64_t height, void* ws_dev, int64_t ws_bytes,
+                     uint32_t* hist_dev, uint8_t* modes_dev, void* stream) {
+    return webp_analyze(rgba_dev, width, height, ws_dev, ws_bytes, hist_dev, modes_dev, (cudaStream_t)stream);
+}
+
+int gsx_webp_emit(int64_t width, int64_t height, int32_t image, const uint32_t* table_dev, uint64_t bit_offset,
+                  void* ws_dev, int64_t ws_bytes, uint32_t* words_dev, int64_t nwords,
+                  unsigned long long* total_bits_dev, void* stream) {
+    return webp_emit(width, height, image, table_dev, bit_offset, ws_dev, ws_bytes, words_dev, nwords, total_bits_dev,
+                     (cudaStream_t)stream);
+}
+
+int gsx_webp_patch(uint32_t* words_dev, int64_t nwords, const uint32_t* patches_dev, int64_t npatches, void* stream) {
+    return webp_patch(words_dev, nwords, patches_dev, npatches, (cudaStream_t)stream);
 }
 
 /* ------------------------------------------------------------------ K-Means */

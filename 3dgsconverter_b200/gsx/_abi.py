@@ -122,6 +122,10 @@ _SIGS = {
     "gsx_ply_transcode": (C.c_int, [_vp, _i64, _i32, _vp, _i32, C.POINTER(_i32), _i32, _vp]),
     "gsx_sog_decode_palette":(C.c_int, [_vp, _i64, _i32, _vp, _i32, _vp, _vp, _vp]),
     "gsx_sog_decode": (C.c_int, [C.POINTER(_vp), _i64, _vp, _vp, _i32, _i32, _vp, _i64, _i32, _vp, _vp, _vp]),
+    "gsx_webp_workspace_bytes": (_i64, [_i64, _i64]),
+    "gsx_webp_analyze": (C.c_int, [_vp, _i64, _i64, _vp, _i64, _vp, _vp, _vp]),
+    "gsx_webp_emit": (C.c_int, [_i64, _i64, _i32, _vp, C.c_uint64, _vp, _i64, _vp, _i64, _vp, _vp]),
+    "gsx_webp_patch": (C.c_int, [_vp, _i64, _vp, _i64, _vp]),
     "gsx_copy_h2d": (C.c_int, [_vp, _vp, _i64, _vp]),
     "gsx_copy_d2h": (C.c_int, [_vp, _vp, _i64, _vp]),
     "gsx_host_gather_rows": (C.c_int, [_vp, _i64, _i64, _vp, _i64, _vp]),

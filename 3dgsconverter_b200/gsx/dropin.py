@@ -11,7 +11,9 @@ and, when ``gsconverter.formats.compressed_ply`` imports, ``CompressedPlyFormat.
 and packing on the device, the file still written by the class's own ``_write_ply_file``; records gsx refuses go to
 the original ``write``).  With ``patch(sog="device")`` also ``SogFormat.write`` (gsx.sog.encode: every texture,
 codebook and the chunked SH palette built on the device; opt-in because its position bytes can differ from NumPy's
-log by one count on a small fraction of the splats).  With ``patch(codecs="device")`` also ``SplatFormat.write``,
+log by one count on a small fraction of the splats); ``patch(sog="device", sog_webp="device")`` also encodes its
+WebP members on the device (gsx.webp: lossless VP8L that decodes to the same pixels, in gsx's bytes, not libwebp's).
+With ``patch(codecs="device")`` also ``SplatFormat.write``,
 ``KSplatFormat.write`` and ``SpzFormat.write`` (gsx.splat / gsx.ksplat / gsx.spz: sort, bucket bounds and packing on the
 device, gzip and the file on the host; records gsx refuses go to the original ``write``).  With
 ``patch(readers="device")`` also the ``read`` of ``SplatFormat``, ``KSplatFormat``, ``SpzFormat`` and
@@ -63,11 +65,15 @@ class _GsxCodebookKMeans:
 
 
 def patch(verbose: bool = False, defer: bool = True, codebook: str = "sklearn", require_cuda: bool = True,
-          sog: str = "host", codecs: str = "host", readers: str = "host", sog_reader: str = "host", ply: str = "host"):
+          sog: str = "host", codecs: str = "host", readers: str = "host", sog_reader: str = "host", ply: str = "host",
+          sog_webp: str = "host"):
     """require_cuda: refuse (return False, leave the reference untouched) when no CUDA device is usable, so that a
     CPU-only host keeps the reference's own SciPy / scikit-learn paths (there is no CPU fallback inside gsx).
     sog: "host" keeps the reference's SogFormat.write (with the patched gpu_ops.kmeans and its batch-ahead);
     "device" replaces it with gsx.sog's device encoder (records gsx refuses go to the original write).
+    sog_webp: with sog="device" only.  "host" writes the bundle's WebP members with Pillow, as the reference does;
+    "device" encodes them from HBM with gsx.webp.  The files then hold gsx's lossless bytes rather than libwebp's
+    (same pixels, a different size), so this chooses the output, not only the speed.
     codecs: "host" keeps the reference's .splat / .ksplat / .spz writers; "device" installs gsx's device writers on
     them (records gsx refuses go to the original write).
     readers: "host" keeps the reference's .splat / .ksplat / .spz / compressed PLY readers; "device" installs gsx's
@@ -78,6 +84,10 @@ def patch(verbose: bool = False, defer: bool = True, codebook: str = "sklearn", 
     reader and writer on Ply3DGSFormat and PlyCCFormat (files and records gsx refuses go to the original method)."""
     if sog not in ("host", "device"):
         raise ValueError(f"sog must be 'host' or 'device', not {sog!r}")
+    if sog_webp not in ("host", "device"):
+        raise ValueError(f"sog_webp must be 'host' or 'device', not {sog_webp!r}")
+    if sog_webp == "device" and sog != "device":
+        raise ValueError("sog_webp='device' needs sog='device': the reference writer has no device textures to encode")
     if codecs not in ("host", "device"):
         raise ValueError(f"codecs must be 'host' or 'device', not {codecs!r}")
     if readers not in ("host", "device"):
@@ -135,7 +145,7 @@ def patch(verbose: bool = False, defer: bool = True, codebook: str = "sklearn", 
         sog_mod.MiniBatchKMeans = _GsxCodebookKMeans  # sog.py:561 -> exact 1-D Lloyd on the GPU
     if sog_mod is not None and sog == "device" and hasattr(sog_mod, "SogFormat"):
         from .sog import install as install_sog
-        install_sog(sog_mod.SogFormat)                # sog.py:249-639 -> textures and palette on the GPU
+        install_sog(sog_mod.SogFormat, webp=sog_webp)  # sog.py:249-639 -> textures and palette on the GPU
     if sog_mod is not None and sog_reader == "device" and hasattr(sog_mod, "SogFormat"):
         from .sog_reader import install_reader as install_sog_reader
         install_sog_reader(sog_mod.SogFormat)         # sog.py:23-247 -> palette and rows on the GPU

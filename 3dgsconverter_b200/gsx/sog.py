@@ -8,12 +8,14 @@
 and the whole writer, SogFormat.write (sog.py:249-639), over device-resident records:
 
     tex = encode(records, compression_level=0)  # DeviceRecords -> SogTextures (device uint8 [pixels, 4] textures)
-    write_sog("out.sog", tex.to_host(), tex.meta)
+    write_sog("out.sog", tex.to_host(), tex.meta)   # members by Pillow (libwebp's bytes)
+    write_sog("out.sog", tex, tex.meta)              # members by gsx.webp from HBM
 
 encode() runs the lexsort, the position / quaternion / scale / colour textures, the two 1-D codebook fits and the
 chunked SH palette on the GPU.  What stays on the host: the reference's NumPy RNG draws (consumed from the global RNG
 in the reference's order, so np.random.seed reproduces a run), the fit of the 256-entry SH codebook on the palette
-(scikit-learn's MiniBatchKMeans by default, at most 65 536 x 45 values), and WebP + ZIP in write_sog.
+(scikit-learn's MiniBatchKMeans by default, at most 65 536 x 45 values), and ZIP in write_sog, with
+the WebP members by Pillow or, given the SogTextures themselves, by gsx.webp on the device.
 
 Parity with the reference writer: every byte is exact except those that go through a transcendental.  The position
 logarithm is computed in double and rounded once, NumPy uses a SIMD float32 log, so a means u16 can differ by one on
@@ -399,12 +401,24 @@ def encode(records, compression_level=0, codebook_fit=None, profile: dict | None
     return SogTextures(textures, {k: sizes[k] for k in textures}, meta, order)
 
 
-def write_sog(path, textures: dict, meta: dict) -> None:
-    """The .sog bundle of sog.py:268-276, 637-638: every texture (uint8 [height, width, 4], as SogTextures.to_host
-    returns them) as a lossless WebP with the reference's arguments, in the reference's member order, then
-    meta.json, in a ZIP_STORED archive."""
-    from PIL import Image
+def write_sog(path, textures, meta: dict) -> None:
+    """The .sog bundle of sog.py:268-276, 637-638: every texture as a lossless WebP, in the reference's member order,
+    then meta.json, in a ZIP_STORED archive.  `textures` picks the encoder:
+      * a dict of uint8 [height, width, 4] (as SogTextures.to_host returns them): Pillow with the reference's
+        arguments, so the members are libwebp's bytes;
+      * a SogTextures: gsx.webp encodes each member from HBM and only the compressed bytes come back.  The members
+        decode to the same pixels (RGB wherever alpha is not 0; neither encoder keeps RGB under alpha 0) but are
+        not libwebp's bytes."""
     names = list(MAIN_FILES) + (list(SHN_FILES) if "shN" in meta else [])
+    if isinstance(textures, SogTextures):
+        from .webp import encode_lossless
+        with zipfile.ZipFile(path, "w", zipfile.ZIP_STORED) as zf:
+            for name in names:
+                w, h = textures.sizes[name]
+                zf.writestr(name, encode_lossless(textures.textures[name], w, h))
+            zf.writestr("meta.json", json.dumps(meta))
+        return
+    from PIL import Image
     with zipfile.ZipFile(path, "w", zipfile.ZIP_STORED) as zf:
         for name in names:
             a = np.ascontiguousarray(textures[name], dtype=np.uint8)
@@ -428,7 +442,8 @@ def _module_codebook_fit(cls):
 
 
 def dropin_write(self, data: np.ndarray, path, **kwargs) -> None:
-    """Replacement for SogFormat.write: packed-float32 records are encoded on the device and bundled by write_sog;
+    """Replacement for SogFormat.write: packed-float32 records are encoded on the device and bundled by write_sog
+    (its WebP members by Pillow, or by gsx.webp from HBM when the class was installed with webp="device");
     anything gsx refuses or fails on goes to the original write with the global NumPy RNG as it was on entry."""
     from .records import DeviceRecords, is_packed_f32
     state = np.random.get_state()
@@ -438,15 +453,19 @@ def dropin_write(self, data: np.ndarray, path, **kwargs) -> None:
         import PIL.Image  # noqa: F401  (the reference refuses without Pillow)
         tex = encode(DeviceRecords.from_structured(data), kwargs.get("compression_level", 0),
                      codebook_fit=_module_codebook_fit(type(self)))
-        host = tex.to_host()
+        textures = tex if getattr(type(self), "_gsx_sog_webp", "host") == "device" else tex.to_host()
     except Exception:  # noqa: BLE001  (the reference's convention: exception => CPU path)
         np.random.set_state(state)
         return self._gsx_reference_write(data, path, **kwargs)
-    write_sog(path, host, tex.meta)
+    write_sog(path, textures, tex.meta)
 
 
-def install(cls) -> None:
-    """Make cls.write the device writer, keeping the original as cls._gsx_reference_write (idempotent)."""
+def install(cls, webp: str = "host") -> None:
+    """Make cls.write the device writer, keeping the original as cls._gsx_reference_write (idempotent).
+    webp: "host" bundles the members through Pillow (libwebp's bytes); "device" encodes them with gsx.webp."""
+    if webp not in ("host", "device"):
+        raise ValueError(f"webp must be 'host' or 'device', not {webp!r}")
     if "_gsx_reference_write" not in cls.__dict__:
         cls._gsx_reference_write = cls.write
         cls.write = dropin_write
+    cls._gsx_sog_webp = webp

@@ -275,6 +275,26 @@ int gsx_sog_labels(const int32_t* labels_dev, int64_t n, int64_t chunk_size, int
 int gsx_sog_centroids(const float* palette_dev, int64_t P, int32_t coeffs, const float* cb_dev, int32_t m,
                       int64_t pixels, uint8_t* out_dev, void* stream);
 
+/* ---- lossless WebP (VP8L, RFC 9649) on the device: the SOG bundle's members (gsx/webp.py) ------------------------
+ * The input is an RGBA uint8 image in HBM, [height * width, 4], 1 <= width, height <= 16384 (else GSX_ERR_ARG).
+ * gsx_webp_analyze builds five entropy-coded images in the workspace: 0 = the pixels with RGB cleared where alpha is
+ * 0, 1 = predictor residuals (16x16 tiles, per tile the mode 0..13 with the least sum of |residual as int8|, lowest
+ * on a tie), 2 = subtract-green then the same, 3 / 4 = the predictor sub-images of 1 / 2 (alpha 255, mode in green);
+ * their run copies of the left pixel (greedy, 3..4096 pixels) and their histograms: hist_dev uint32
+ * [5 * 1088 + 1] = per image green + 24 length codes (280), red, blue, alpha (256 each), distance (40), then 1 when
+ * some alpha is not 255.  modes_dev (nullable): uint8 [2 * tiles], the tile modes of images 1 and 2.
+ * gsx_webp_emit writes the tokens of one image as LSB-first bits at bit_offset into words_dev (zeroed by the
+ * caller; a token past nwords is dropped) with table_dev uint32 [1088] = bit-reversed code | length << 16 per
+ * symbol, and stores the image's bit count in *total_bits_dev.  The workspace must hold what analyze left there.
+ * gsx_webp_patch ORs npatches (word index, bits) pairs of uint32 into words_dev (the host-written headers). */
+int64_t gsx_webp_workspace_bytes(int64_t width, int64_t height);
+int gsx_webp_analyze(const uint8_t* rgba_dev, int64_t width, int64_t height, void* ws_dev, int64_t ws_bytes,
+                     uint32_t* hist_dev, uint8_t* modes_dev, void* stream);
+int gsx_webp_emit(int64_t width, int64_t height, int32_t image, const uint32_t* table_dev, uint64_t bit_offset,
+                  void* ws_dev, int64_t ws_bytes, uint32_t* words_dev, int64_t nwords,
+                  unsigned long long* total_bits_dev, void* stream);
+int gsx_webp_patch(uint32_t* words_dev, int64_t nwords, const uint32_t* patches_dev, int64_t npatches, void* stream);
+
 /* ---- K-Means: gpu_ops.py:57-96 (kernels) + :186-188 (Lloyd loop) ---------------------- */
 /* Batched over `nprob` independent problems stored back to back (SOG shN chunks, sog.py:527-549):
  * problem p has rows [row_off[p], row_off[p+1]) of X[*,D] and K centroids at C[p*K*D].
