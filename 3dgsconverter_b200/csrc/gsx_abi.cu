@@ -7,6 +7,7 @@
 #include "gsx_common.cuh"
 #include "gsx_compact.cuh"
 #include "gsx_compressed_ply.cuh"
+#include "gsx_deflate.cuh"
 #include "gsx_density.cuh"
 #include "gsx_hostcopy.cuh"
 #include "gsx_hostrows.cuh"
@@ -523,6 +524,31 @@ int gsx_webp_emit(int64_t width, int64_t height, int32_t image, const uint32_t* 
 
 int gsx_webp_patch(uint32_t* words_dev, int64_t nwords, const uint32_t* patches_dev, int64_t npatches, void* stream) {
     return webp_patch(words_dev, nwords, patches_dev, npatches, (cudaStream_t)stream);
+}
+
+/* ------------------------------------------------------------------ DEFLATE and CRC-32 */
+
+int64_t gsx_deflate_workspace_bytes(int64_t nblocks) { return deflate_workspace_bytes(nblocks); }
+
+int gsx_crc32(const uint8_t* data_dev, int64_t n, void* ws_dev, int64_t ws_bytes, uint8_t* trailer_dev, void* stream) {
+    return crc32_trailer(data_dev, n, ws_dev, ws_bytes, trailer_dev, (cudaStream_t)stream);
+}
+
+int gsx_deflate_stored(const uint8_t* data_dev, int64_t n, uint8_t* out_dev, void* stream) {
+    return deflate_stored(data_dev, n, out_dev, (cudaStream_t)stream);
+}
+
+int gsx_deflate_plan(const uint8_t* data_dev, int64_t n, const int64_t* starts_dev, int64_t nblocks, void* ws_dev,
+                     int64_t ws_bytes, uint64_t bit_offset, unsigned long long* total_bits_dev, void* stream) {
+    return deflate_plan(data_dev, n, starts_dev, nblocks, ws_dev, ws_bytes, bit_offset, total_bits_dev,
+                        (cudaStream_t)stream);
+}
+
+int gsx_deflate_emit(const uint8_t* data_dev, int64_t n, const int64_t* starts_dev, int64_t nblocks, void* ws_dev,
+                     int64_t ws_bytes, uint32_t* words_dev, int64_t nwords, unsigned long long* mismatches_dev,
+                     void* stream) {
+    return deflate_emit(data_dev, n, starts_dev, nblocks, ws_dev, ws_bytes, words_dev, nwords, mismatches_dev,
+                        (cudaStream_t)stream);
 }
 
 /* ------------------------------------------------------------------ K-Means */

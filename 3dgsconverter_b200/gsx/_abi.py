@@ -126,6 +126,11 @@ _SIGS = {
     "gsx_webp_analyze": (C.c_int, [_vp, _i64, _i64, _vp, _i64, _vp, _vp, _vp]),
     "gsx_webp_emit": (C.c_int, [_i64, _i64, _i32, _vp, C.c_uint64, _vp, _i64, _vp, _i64, _vp, _vp]),
     "gsx_webp_patch": (C.c_int, [_vp, _i64, _vp, _i64, _vp]),
+    "gsx_deflate_workspace_bytes": (_i64, [_i64]),
+    "gsx_crc32": (C.c_int, [_vp, _i64, _vp, _i64, _vp, _vp]),
+    "gsx_deflate_stored": (C.c_int, [_vp, _i64, _vp, _vp]),
+    "gsx_deflate_plan": (C.c_int, [_vp, _i64, _vp, _i64, _vp, _i64, C.c_uint64, _vp, _vp]),
+    "gsx_deflate_emit": (C.c_int, [_vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64, _vp, _vp]),
     "gsx_copy_h2d": (C.c_int, [_vp, _vp, _i64, _vp]),
     "gsx_copy_d2h": (C.c_int, [_vp, _vp, _i64, _vp]),
     "gsx_host_gather_rows": (C.c_int, [_vp, _i64, _i64, _vp, _i64, _vp]),

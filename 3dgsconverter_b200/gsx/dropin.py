@@ -15,7 +15,9 @@ log by one count on a small fraction of the splats); ``patch(sog="device", sog_w
 WebP members on the device (gsx.webp: lossless VP8L that decodes to the same pixels, in gsx's bytes, not libwebp's).
 With ``patch(codecs="device")`` also ``SplatFormat.write``,
 ``KSplatFormat.write`` and ``SpzFormat.write`` (gsx.splat / gsx.ksplat / gsx.spz: sort, bucket bounds and packing on the
-device, gzip and the file on the host; records gsx refuses go to the original ``write``).  With
+device, gzip and the file on the host; records gsx refuses go to the original ``write``);
+``patch(codecs="device", spz_gzip="device")`` also gzips the .spz payload on the device (gsx.deflate: a file that
+decompresses to the same payload, in gsx's bytes, not zlib's).  With
 ``patch(readers="device")`` also the ``read`` of ``SplatFormat``, ``KSplatFormat``, ``SpzFormat`` and
 ``CompressedPlyFormat`` (gsx.splat / gsx.ksplat / gsx.spz / gsx.compressed_ply ``decode``: headers and gunzip on the
 host, every splat decoded on the device, byte for byte as the reference readers; files gsx refuses go to the original
@@ -66,7 +68,7 @@ class _GsxCodebookKMeans:
 
 def patch(verbose: bool = False, defer: bool = True, codebook: str = "sklearn", require_cuda: bool = True,
           sog: str = "host", codecs: str = "host", readers: str = "host", sog_reader: str = "host", ply: str = "host",
-          sog_webp: str = "host"):
+          sog_webp: str = "host", spz_gzip: str = "host"):
     """require_cuda: refuse (return False, leave the reference untouched) when no CUDA device is usable, so that a
     CPU-only host keeps the reference's own SciPy / scikit-learn paths (there is no CPU fallback inside gsx).
     sog: "host" keeps the reference's SogFormat.write (with the patched gpu_ops.kmeans and its batch-ahead);
@@ -76,6 +78,9 @@ def patch(verbose: bool = False, defer: bool = True, codebook: str = "sklearn", 
     (same pixels, a different size), so this chooses the output, not only the speed.
     codecs: "host" keeps the reference's .splat / .ksplat / .spz writers; "device" installs gsx's device writers on
     them (records gsx refuses go to the original write).
+    spz_gzip: with codecs="device" only.  "host" gzips the .spz payload with gzip.compress, as the reference does;
+    "device" compresses it in HBM with gsx.deflate and copies back only the file.  The file then holds gsx's DEFLATE
+    bytes rather than zlib's (the same payload inside), so this chooses the output, not only the speed.
     readers: "host" keeps the reference's .splat / .ksplat / .spz / compressed PLY readers; "device" installs gsx's
     device readers on them (files gsx refuses go to the original read).
     sog_reader: "host" keeps the reference's SogFormat.read; "device" installs gsx.sog_reader's device reader on it
@@ -90,6 +95,10 @@ def patch(verbose: bool = False, defer: bool = True, codebook: str = "sklearn", 
         raise ValueError("sog_webp='device' needs sog='device': the reference writer has no device textures to encode")
     if codecs not in ("host", "device"):
         raise ValueError(f"codecs must be 'host' or 'device', not {codecs!r}")
+    if spz_gzip not in ("host", "device"):
+        raise ValueError(f"spz_gzip must be 'host' or 'device', not {spz_gzip!r}")
+    if spz_gzip == "device" and codecs != "device":
+        raise ValueError("spz_gzip='device' needs codecs='device': the reference writer has no device payload to gzip")
     if readers not in ("host", "device"):
         raise ValueError(f"readers must be 'host' or 'device', not {readers!r}")
     if sog_reader not in ("host", "device"):
@@ -168,8 +177,11 @@ def patch(verbose: bool = False, defer: bool = True, codebook: str = "sklearn", 
                     fmt = importlib.import_module(f"gsconverter.formats.{modname}")
                 except Exception:  # noqa: BLE001  (writer not importable: nothing to patch there)
                     continue
-            if hasattr(fmt, clsname):
-                ours.install(getattr(fmt, clsname))   # splat.py:82-166, ksplat.py:319-544, spz.py:49-173
+            if hasattr(fmt, clsname):                 # splat.py:82-166, ksplat.py:319-544, spz.py:49-173
+                if ours is spz:
+                    ours.install(getattr(fmt, clsname), where=spz_gzip)
+                else:
+                    ours.install(getattr(fmt, clsname))
     if readers == "device":
         from . import compressed_ply, ksplat, splat, spz
         for modname, clsname, ours in (("splat", "SplatFormat", splat), ("ksplat", "KSplatFormat", ksplat),

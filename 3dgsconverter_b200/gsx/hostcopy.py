@@ -3,6 +3,8 @@ pageable host buffers are moved by several host threads through pinned chunks, s
 (torch's `.to(device)` / `.cpu()` of a pageable array run on one thread)."""
 from __future__ import annotations
 
+import ctypes
+
 import numpy as np
 import torch
 
@@ -32,4 +34,25 @@ def to_host(t: torch.Tensor) -> np.ndarray:
     if out.nbytes:
         with torch.cuda.device(t.device):
             check(lib.gsx_copy_d2h(out.ctypes.data, _ptr(t), out.nbytes, _stream()), "gsx_copy_d2h")
+    return out
+
+
+# a new bytes object of n uninitialised bytes, and the address of its contents: the C API's way to fill a bytes object
+# before anyone else holds it, so that a device buffer lands in the returned bytes without a second host copy
+_new_bytes = ctypes.pythonapi.PyBytes_FromStringAndSize
+_new_bytes.restype, _new_bytes.argtypes = ctypes.py_object, [ctypes.c_void_p, ctypes.c_ssize_t]
+_bytes_at = ctypes.pythonapi.PyBytes_AsString
+_bytes_at.restype, _bytes_at.argtypes = ctypes.c_void_p, [ctypes.py_object]
+
+
+def to_bytes(t: torch.Tensor) -> bytes:
+    """The bytes of a uint8 CUDA tensor, copied once, straight into the returned object (blocks until they are
+    there)."""
+    t = t.contiguous()
+    if t.dtype != torch.uint8:
+        raise ValueError(f"to_bytes needs a uint8 tensor, not {t.dtype}")
+    out = _new_bytes(None, t.numel())
+    if t.numel():
+        with torch.cuda.device(t.device):
+            check(lib.gsx_copy_d2h(_bytes_at(out), _ptr(t), t.numel(), _stream()), "gsx_copy_d2h")
     return out

@@ -2,10 +2,12 @@
 and the 16-byte header on the host, the planar body on the GPU (gsx_spz_decode).  encode: formats/spz.py:49-173
 (SpzFormat.write, _pack_v3) over DeviceRecords.  The SH degree
 rule reads one non-zero mask of the f_rest columns (gsx_codec_sh_mask); the planar body is packed on the GPU
-(gsx_spz_pack) behind the 16-byte header; the host runs gzip.
+(gsx_spz_pack) behind the 16-byte header; the host runs gzip, or with where="device" gsx.deflate does, cutting its
+blocks at the section boundaries.
 
     enc = encode(records)                           # DeviceRecords -> Spz (device payload: header + body)
     write_spz("out.spz", enc, compression_level=0)
+    write_spz("out.spz", enc, 6, where="device")    # gzip on the GPU: only the compressed file crosses PCIe
     dec = decode("in.spz")                          # -> readers.Decoded: dec.to_host() is what SpzFormat.read returns
 """
 from __future__ import annotations
@@ -36,6 +38,17 @@ class Spz:
         """The payload the reference hands to gzip.compress."""
         from .hostcopy import to_host
         return to_host(self.payload).tobytes()
+
+    def sections(self) -> list:
+        """Offsets where the payload's sections start: the 16-byte header, then positions 9n, alphas n, colours 3n,
+        scales 3n, rotations 4n and SH 3 * dim * n."""
+        n = (self.payload.numel() - 16) // (20 + 3 * SH_DIM[self.sh_degree])
+        return list(np.cumsum([16, 9 * n, n, 3 * n, 3 * n, 4 * n]))
+
+    def compress(self, compression_level: int, mtime: int | None = None) -> bytes:
+        """The .spz file: the payload gzipped on the device (gsx.deflate) with its blocks cut at the sections."""
+        from .deflate import gzip as device_gzip
+        return device_gzip(self.payload, compression_level, mtime=mtime, breaks=self.sections())
 
 
 def sh_degree(records) -> int:
@@ -75,30 +88,49 @@ def encode(records) -> Spz:
     return Spz(payload, degree)
 
 
-def write_spz(path, enc: Spz, compression_level=0) -> None:
-    """gzip at `compression_level` (0 = stored), as spz.py:97-102."""
+def _where(where: str) -> str:
+    if where not in ("host", "device"):
+        raise ValueError(f"gzip must run on the 'host' or the 'device', not {where!r}")
+    return where
+
+
+def write_spz(path, enc: Spz, compression_level=0, where: str = "host") -> None:
+    """gzip at `compression_level` (0 = stored): where="host" copies the payload back and runs gzip.compress, as
+    spz.py:97-102; where="device" runs gsx.deflate (Spz.compress) and copies back only the file."""
+    if _where(where) == "device":
+        blob = enc.compress(compression_level)
+    else:
+        blob = gzip.compress(enc.to_host(), compresslevel=compression_level)
     with open(path, "wb") as fh:
-        fh.write(gzip.compress(enc.to_host(), compresslevel=compression_level))
+        fh.write(blob)
 
 
 def dropin_write(self, data: np.ndarray, path, **kwargs) -> None:
-    """Replacement for SpzFormat.write: the payload is packed on the device and gzipped on the host; anything gsx
-    refuses or fails on goes to the original write with the original arguments."""
+    """Replacement for SpzFormat.write: the payload is packed on the device and gzipped on the host (or on the device
+    when installed with where="device"); anything gsx refuses or fails on goes to the original write with the
+    original arguments."""
     from .records import DeviceRecords
     try:
-        payload = encode(DeviceRecords.from_writer_input(data)).to_host()
-        blob = gzip.compress(payload, compresslevel=kwargs.get("compression_level", 0))
+        enc = encode(DeviceRecords.from_writer_input(data))
+        level = kwargs.get("compression_level", 0)
+        if getattr(self, "_gsx_spz_gzip", "host") == "device":
+            blob = enc.compress(level)
+        else:
+            blob = gzip.compress(enc.to_host(), compresslevel=level)
     except Exception:  # noqa: BLE001  (the reference's convention: exception => CPU path)
         return self._gsx_reference_write(data, path, **kwargs)
     with open(path, "wb") as fh:
         fh.write(blob)
 
 
-def install(cls) -> None:
-    """Make cls.write the device writer, keeping the original as cls._gsx_reference_write (idempotent)."""
+def install(cls, where: str = "host") -> None:
+    """Make cls.write the device writer, keeping the original as cls._gsx_reference_write (idempotent).
+    where: "host" gzips with gzip.compress (the reference's bytes); "device" with gsx.deflate."""
+    _where(where)
     if "_gsx_reference_write" not in cls.__dict__:
         cls._gsx_reference_write = cls.write
         cls.write = dropin_write
+    cls._gsx_spz_gzip = where
 
 
 def read_tables():

@@ -295,6 +295,33 @@ int gsx_webp_emit(int64_t width, int64_t height, int32_t image, const uint32_t* 
                   unsigned long long* total_bits_dev, void* stream);
 int gsx_webp_patch(uint32_t* words_dev, int64_t nwords, const uint32_t* patches_dev, int64_t npatches, void* stream);
 
+/* ---- raw DEFLATE (RFC 1951) and CRC-32 on the device: the body and trailer of .gz files (gsx/deflate.py) ---------
+ * data_dev is n bytes of HBM (64-bit n).  Every pointer is a device pointer; every entry runs on `stream`.
+ * gsx_deflate_workspace_bytes(nblocks): the workspace of gsx_crc32 (nblocks 0), gsx_deflate_plan and
+ * gsx_deflate_emit: 4 KiB + about 1.6 KiB per block, independent of n.
+ * gsx_crc32 writes the 8-byte gzip trailer at trailer_dev: zlib's crc32 of the n bytes, then n mod 2^32, both
+ * little-endian (the CRC of each 4 KiB chunk is shifted by x^(8 * bytes after it) mod P and XORed).
+ * gsx_deflate_stored writes 5 * max(1, ceil(n / 65535)) + n bytes at out_dev: stored blocks of 65535 bytes, the
+ * last one shorter and final (an empty input: one empty final block).
+ * gsx_deflate_plan plans the dynamic blocks starts_dev int64 [nblocks] (block b is [starts[b], starts[b + 1]) or up
+ * to n; starts[0] = 0, ascending, each block at most 1 MiB; one empty block when n = 0).  Per block: the
+ * histograms of literals only and of literals plus distance-1 copies (a run of r >= 4 equal bytes -> one literal,
+ * then copies of 258, then one copy of the remainder when it is >= 3, else that many literals), Huffman code lengths
+ * (15 bits, 7 for the code-length code; the rule of gsx/webp.py code_lengths), the run-length-coded header, and the
+ * candidate with fewer bits (literals on a tie).  Writes the body's bit count to *total_bits_dev; block b starts at
+ * bit bit_offset + the bits of the blocks before it.
+ * gsx_deflate_emit ORs the planned blocks' bits into words_dev (uint32 LSB-first, zeroed by the caller and sized
+ * from the total; bits past nwords are dropped) and adds 1 to *mismatches_dev for every block whose emitted bits
+ * differ from its plan.  The workspace must hold what gsx_deflate_plan left there. */
+int64_t gsx_deflate_workspace_bytes(int64_t nblocks);
+int gsx_crc32(const uint8_t* data_dev, int64_t n, void* ws_dev, int64_t ws_bytes, uint8_t* trailer_dev, void* stream);
+int gsx_deflate_stored(const uint8_t* data_dev, int64_t n, uint8_t* out_dev, void* stream);
+int gsx_deflate_plan(const uint8_t* data_dev, int64_t n, const int64_t* starts_dev, int64_t nblocks, void* ws_dev,
+                     int64_t ws_bytes, uint64_t bit_offset, unsigned long long* total_bits_dev, void* stream);
+int gsx_deflate_emit(const uint8_t* data_dev, int64_t n, const int64_t* starts_dev, int64_t nblocks, void* ws_dev,
+                     int64_t ws_bytes, uint32_t* words_dev, int64_t nwords, unsigned long long* mismatches_dev,
+                     void* stream);
+
 /* ---- K-Means: gpu_ops.py:57-96 (kernels) + :186-188 (Lloyd loop) ---------------------- */
 /* Batched over `nprob` independent problems stored back to back (SOG shN chunks, sog.py:527-549):
  * problem p has rows [row_off[p], row_off[p+1]) of X[*,D] and K centroids at C[p*K*D].
