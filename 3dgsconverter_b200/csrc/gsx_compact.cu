@@ -7,8 +7,9 @@
 // Stable (order-preserving), like NumPy boolean indexing: one pass with decoupled look-back over per-tile survivor
 // counts (k_cmp_onepass) when n < 2^30, where its 30-bit look-back counts cannot overflow; from 2^30 rows on,
 // count -> multi-level scan -> scatter (k_cmp_count, k_cmp_scatter), which reads the mask twice.
+#include "../../include/gsx.h"
+
 #include "gsx_common.cuh"
-#include "gsx_compact.cuh"
 #include "gsx_radix.cuh"
 
 namespace gsx {
@@ -161,15 +162,22 @@ __global__ void __launch_bounds__(kOpThreads)
     }
 }
 
-int64_t compact_workspace_bytes(int64_t n) {
+}  // namespace gsx
+
+using namespace gsx;
+
+extern "C" {
+
+int64_t gsx_compact_workspace_bytes(int64_t n) {
     if (n < 1) n = 1;
     int64_t blocks = (n + kCmpBlock - 1) / kCmpBlock;
     return (int64_t)((size_t)(blocks + 64) * 4 + scan_workspace_bytes(blocks) + 1024);
 }
 
-int compact_points(const uint8_t* mask, int64_t n, const float* xyz, const float* opacity, const int32_t* idx,
-                   float* xyz_out, float* opacity_out, int32_t* idx_out, int64_t* count_host, void* ws,
-                   int64_t ws_bytes, cudaStream_t st) {
+int gsx_compact_points(const uint8_t* mask, int64_t n, const float* xyz, const float* opacity, const int32_t* idx,
+                       float* xyz_out, float* opacity_out, int32_t* idx_out, int64_t* count_host, void* ws,
+                       int64_t ws_bytes, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
     GSX_NVTX("gsx::compact_points");
     if (n == 0) {
         *count_host = 0;
@@ -178,7 +186,7 @@ int compact_points(const uint8_t* mask, int64_t n, const float* xyz, const float
     // the surviving row indices are int32 (a row >= 2^31 would wrap) and the two-pass positions uint32
     GSX_REQUIRE(n < (1ll << 31), GSX_ERR_UNSUPPORTED, "compact: n = %lld rows, int32 row indices need n < 2^31",
                 (long long)n);
-    GSX_REQUIRE(ws_bytes >= compact_workspace_bytes(n), GSX_ERR_WORKSPACE, "compact: workspace too small");
+    GSX_REQUIRE(ws_bytes >= gsx_compact_workspace_bytes(n), GSX_ERR_WORKSPACE, "compact: workspace too small");
     GSX_REQUIRE((opacity == nullptr) == (opacity_out == nullptr), GSX_ERR_ARG, "compact: opacity in/out mismatch");
     if (n < (1ll << 30)) {   // the look-back words carry 30-bit survivor counts (kLbVal)
         const int64_t tiles = (n + kOpTile - 1) / kOpTile;   // (fits the two-pass workspace: fewer tiles than blocks)
@@ -211,4 +219,4 @@ int compact_points(const uint8_t* mask, int64_t n, const float* xyz, const float
     return GSX_OK;
 }
 
-}  // namespace gsx
+}  // extern "C"

@@ -12,9 +12,10 @@
 // Arithmetic follows NumPy-2 float32 semantics (Python float constants are weak scalars, i.e. rounded to float32 first):
 // every step is one __f*_rn operation in the reference's order, with no contraction.  The alpha channel goes through
 // expf and can differ from NumPy's SIMD exp by one count on ~1e-5 of the splats; everything else is bit-exact.
+#include "../../include/gsx.h"
+
 #include "gsx_common.cuh"
 #include "gsx_sh_mask.cuh"
-#include "gsx_compressed_ply.cuh"
 
 namespace gsx {
 
@@ -175,10 +176,17 @@ __global__ void __launch_bounds__(256) k_cply_narrow_sh(const uint8_t* __restric
 
 }  // namespace
 
-int cply_pack(const float* rows, int64_t n, int F, const int32_t* order, const int32_t* cols14_host,
-              const int32_t* rest_cols_host, int n_rest, const float* lo_pos_dc, const float* hi_pos_dc,
-              const float* lo_scale, const float* hi_scale, float* chunk_out, uint32_t* vertex_out, uint8_t* sh_out,
-              unsigned long long* rest_nonzero_out, cudaStream_t st) {
+}  // namespace gsx
+
+using namespace gsx;
+
+extern "C" {
+
+int gsx_cply_pack(const float* rows, int64_t n, int32_t F, const int32_t* order, const int32_t* cols14_host,
+                  const int32_t* rest_cols_host, int32_t n_rest, const float* lo_pos_dc, const float* hi_pos_dc,
+                  const float* lo_scale, const float* hi_scale, float* chunk_out, uint32_t* vertex_out, uint8_t* sh_out,
+                  uint64_t* rest_nonzero_out, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
     GSX_NVTX("gsx::cply_pack");
     GSX_REQUIRE(n >= 0 && n < 2147483648ll, GSX_ERR_ARG, "cply_pack: n=%lld out of range [0, 2^31)", (long long)n);
     if (n == 0) return GSX_OK;
@@ -207,12 +215,13 @@ int cply_pack(const float* rows, int64_t n, int F, const int32_t* order, const i
     const int64_t nchunk = (n + kChunk - 1) / kChunk;
     k_cply_pack<<<(int)nchunk, kChunk, 0, st>>>(rows, n, F, order, cols, lo_pos_dc, hi_pos_dc, lo_scale, hi_scale,
                                                 chunk_out, reinterpret_cast<uint4*>(vertex_out), sh_out,
-                                                rest_nonzero_out);
+                                                (unsigned long long*)rest_nonzero_out);
     GSX_KERNEL_CHECK();
     return GSX_OK;
 }
 
-int cply_narrow_sh(const uint8_t* sh, int64_t n, int width, int keep, uint8_t* out, cudaStream_t st) {
+int gsx_cply_narrow_sh(const uint8_t* sh, int64_t n, int32_t width, int32_t keep, uint8_t* out, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
     GSX_REQUIRE(n >= 0 && n < 2147483648ll, GSX_ERR_ARG, "cply_narrow_sh: n=%lld out of range [0, 2^31)", (long long)n);
     GSX_REQUIRE(keep >= 0 && keep <= width && width <= kMaxRest, GSX_ERR_ARG,
                 "cply_narrow_sh: keep=%d width=%d (need 0 <= keep <= width <= %d)", keep, width, kMaxRest);
@@ -226,4 +235,4 @@ int cply_narrow_sh(const uint8_t* sh, int64_t n, int width, int keep, uint8_t* o
     return GSX_OK;
 }
 
-}  // namespace gsx
+}  // extern "C"

@@ -13,7 +13,9 @@
 //                    (shared with the neighbouring tiles or blocks), the words between them are stored
 // Stored blocks (level 0) are k_deflate_stored.  The CRC is k_crc_chunks (the CRC of each 4 KiB chunk, shifted by
 // x^(8 * bytes after it) mod P, XORed per CTA) and k_crc_finish (the init / final XOR of zlib's crc32).
-#include "gsx_deflate.cuh"
+#include "../../include/gsx.h"
+
+#include "gsx_common.cuh"
 
 #include <algorithm>
 #include <climits>
@@ -21,6 +23,7 @@
 namespace gsx {
 namespace {
 
+constexpr int64_t kDeflateStoredBlock = 65535;
 constexpr int kThreads = 512;
 constexpr int kPer = 8;                             // consecutive bytes per thread in a tile
 constexpr int kTile = kThreads * kPer;              // 4096 bytes
@@ -645,7 +648,13 @@ bool carve(Carver& cv, int64_t nblocks, Layout& L) {
 
 }  // namespace
 
-int64_t deflate_workspace_bytes(int64_t nblocks) {
+}  // namespace gsx
+
+using namespace gsx;
+
+extern "C" {
+
+int64_t gsx_deflate_workspace_bytes(int64_t nblocks) {
     if (nblocks < 0) return 0;
     Carver cv(nullptr, 0);
     Layout L;
@@ -653,7 +662,8 @@ int64_t deflate_workspace_bytes(int64_t nblocks) {
     return int64_t(cv.off) + 256;
 }
 
-int crc32_trailer(const uint8_t* data, int64_t n, void* ws, int64_t ws_bytes, uint8_t* trailer, cudaStream_t st) {
+int gsx_crc32(const uint8_t* data, int64_t n, void* ws, int64_t ws_bytes, uint8_t* trailer, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
     GSX_NVTX("gsx_crc32");
     GSX_REQUIRE(n >= 0 && (data || n == 0) && ws && trailer, GSX_ERR_ARG, "crc32: bad arguments");
     Carver cv(ws, size_t(ws_bytes));
@@ -669,7 +679,8 @@ int crc32_trailer(const uint8_t* data, int64_t n, void* ws, int64_t ws_bytes, ui
     return GSX_OK;
 }
 
-int deflate_stored(const uint8_t* data, int64_t n, uint8_t* out, cudaStream_t st) {
+int gsx_deflate_stored(const uint8_t* data, int64_t n, uint8_t* out, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
     GSX_NVTX("gsx_deflate_stored");
     GSX_REQUIRE(n >= 0 && (data || n == 0) && out, GSX_ERR_ARG, "deflate_stored: bad arguments");
     const int64_t nb = std::max<int64_t>(1, (n + kDeflateStoredBlock - 1) / kDeflateStoredBlock);
@@ -679,8 +690,9 @@ int deflate_stored(const uint8_t* data, int64_t n, uint8_t* out, cudaStream_t st
     return GSX_OK;
 }
 
-int deflate_plan(const uint8_t* data, int64_t n, const int64_t* starts, int64_t nblocks, void* ws, int64_t ws_bytes,
-                 uint64_t bit_offset, unsigned long long* total_bits, cudaStream_t st) {
+int gsx_deflate_plan(const uint8_t* data, int64_t n, const int64_t* starts, int64_t nblocks, void* ws, int64_t ws_bytes,
+                     uint64_t bit_offset, unsigned long long* total_bits, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
     GSX_NVTX("gsx_deflate_plan");
     GSX_REQUIRE(n >= 0 && (data || n == 0) && starts && ws && total_bits, GSX_ERR_ARG, "deflate_plan: bad arguments");
     GSX_REQUIRE(nblocks >= 1 && nblocks < (int64_t(1) << 31), GSX_ERR_ARG,
@@ -695,8 +707,9 @@ int deflate_plan(const uint8_t* data, int64_t n, const int64_t* starts, int64_t 
     return GSX_OK;
 }
 
-int deflate_emit(const uint8_t* data, int64_t n, const int64_t* starts, int64_t nblocks, void* ws, int64_t ws_bytes,
-                 uint32_t* words, int64_t nwords, unsigned long long* mismatches, cudaStream_t st) {
+int gsx_deflate_emit(const uint8_t* data, int64_t n, const int64_t* starts, int64_t nblocks, void* ws, int64_t ws_bytes,
+                     uint32_t* words, int64_t nwords, unsigned long long* mismatches, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
     GSX_NVTX("gsx_deflate_emit");
     GSX_REQUIRE(n >= 0 && (data || n == 0) && starts && ws && words && mismatches, GSX_ERR_ARG,
                 "deflate_emit: bad arguments");
@@ -711,4 +724,4 @@ int deflate_emit(const uint8_t* data, int64_t n, const int64_t* starts, int64_t 
     return GSX_OK;
 }
 
-}  // namespace gsx
+}  // extern "C"

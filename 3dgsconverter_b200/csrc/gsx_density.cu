@@ -11,7 +11,9 @@
 // The thread whose increment makes a voxel reach the density threshold appends it to the
 // dense list, so no pass over the grid is needed.  q = floor(x / f32(voxel)) uses the float32
 // division of the reference (NumPy-2 weak-scalar semantics).
-#include "gsx_density.cuh"
+#include "../../include/gsx.h"
+
+#include "gsx_common.cuh"
 #include "gsx_sor.cuh"
 
 #include <limits.h>
@@ -114,15 +116,6 @@ __device__ __forceinline__ void dense_rule(int old, int c, int thr, unsigned lon
                                            long long* dense_vox, int64_t cap, VoxelOf voxel) {
     if (old == 0) atomicAdd(counters + kDistinct, 1ull);
     if (old < thr && old + c >= thr) dense_append(counters, dense_vox, cap, voxel);
-}
-
-int64_t density_workspace_bytes(int64_t n, int64_t cap) {
-    if (n < 1) n = 1;
-    if (cap < 1) cap = 1;
-    // hash path: table of >= 2n slots (power of two), 8-byte key + 4-byte count; plus minmax scratch
-    size_t slots = 64;
-    while (slots < (size_t)2 * n) slots <<= 1;
-    return (int64_t)(slots * 12 + 6 * 1024 * 4 + (size_t)cap * 28 + 8192);
 }
 
 // ---------------------------------------------------------------- counter tables
@@ -355,113 +348,6 @@ __global__ void k_vox_dense_counts(const long long* __restrict__ dense_vox, int6
     dense_cnt[t] = tab.find(g, dense_vox[3 * t], dense_vox[3 * t + 1], dense_vox[3 * t + 2]);
 }
 
-int density_voxel_count(const float* xyz, int64_t n, float voxel, int64_t min_points, int64_t* dense_vox_host,
-                        int32_t* dense_cnt_host, int64_t cap, int64_t* n_dense_host, int64_t* n_voxels_host, void* ws,
-                        int64_t ws_bytes, cudaStream_t st) {
-    GSX_NVTX("gsx::density_voxel_count");
-    GSX_REQUIRE(n >= 1, GSX_ERR_ARG, "density: n must be >= 1");
-    GSX_REQUIRE(voxel > 0.f, GSX_ERR_ARG, "density: voxel size must be > 0");
-    GSX_REQUIRE(ws_bytes >= density_workspace_bytes(n, cap), GSX_ERR_WORKSPACE, "density: workspace too small");
-    GSX_REQUIRE(cap >= 1, GSX_ERR_ARG, "density: cap must be >= 1");
-    Carver c(ws, (size_t)ws_bytes);
-    float* partial = c.take<float>(6 * 1024);
-    float* minmax = c.take<float>(8);
-    unsigned long long* counters = c.take<unsigned long long>(4);
-    long long* dvox = c.take<long long>(3 * (size_t)cap);
-    int* dcnt = c.take<int>((size_t)cap);
-    size_t used = align_up(c.off, 256);
-    GSX_REQUIRE(c.ok() && used < (size_t)ws_bytes, GSX_ERR_WORKSPACE, "density: workspace too small for cap=%lld",
-                (long long)cap);
-    char* blob = (char*)ws + used;
-    size_t blob_bytes = (size_t)ws_bytes - used;
-
-    int rc = sor_minmax(xyz, n, minmax, partial, st);
-    if (rc) return rc;
-    float mm[6];
-    GSX_CUDA_CHECK(cudaMemcpyAsync(mm, minmax, sizeof(mm), cudaMemcpyDeviceToHost, st));
-    GSX_CUDA_CHECK(cudaStreamSynchronize(st));
-    VoxGrid g;
-    double cells = 1.0;
-    bool wide = false;
-    for (int a = 0; a < 3; ++a) {
-        g.q0[a] = voxel_of(mm[a], voxel);  // floor(x/voxel) is monotone in x: min/max commute with it
-        long long q1 = voxel_of(mm[3 + a], voxel);
-        GSX_REQUIRE(g.q0[a] != LLONG_MIN && q1 != LLONG_MIN, GSX_ERR_UNSUPPORTED,
-                    "density: non-finite or out-of-range coordinates on axis %d", a);
-        // q1 >= q0; the unsigned difference is exact where the signed one could overflow
-        GSX_REQUIRE((unsigned long long)q1 - (unsigned long long)g.q0[a] < (1ull << 31) - 1, GSX_ERR_UNSUPPORTED,
-                    "density: voxel grid extent on axis %d exceeds 2^31 voxels", a);
-        g.dim[a] = q1 - g.q0[a] + 1;
-        if (g.dim[a] >= kAxisLim) wide = true;  // the packed 3 x 21-bit key does not fit: two-word keys
-        cells *= (double)g.dim[a];
-    }
-    long long thr_ll = min_points < 1 ? 1 : min_points;
-    GSX_REQUIRE(thr_ll < 2147483647ll, GSX_ERR_ARG, "density: min_points too large");
-    int thr = (int)thr_ll;
-    GSX_CUDA_CHECK(cudaMemsetAsync(counters, 0, 4 * sizeof(unsigned long long), st));
-    auto count_rows = [&](const auto& tab) {
-        k_vox_count<true><<<(int)((n + 255) / 256), 256, 0, st>>>(xyz, n, voxel, g, tab, thr, counters, dvox, cap,
-                                                                  counters + kOutside);
-    };
-    // After the histogram: the refusals, then the counts of the dense voxels looked up in `tab`.
-    auto read_dense = [&](const auto& tab) -> int {
-        GSX_KERNEL_CHECK();
-        unsigned long long hc[3];   // counters[kDense], [kDistinct], [kOutside]
-        GSX_CUDA_CHECK(cudaMemcpyAsync(hc, counters, sizeof(hc), cudaMemcpyDeviceToHost, st));
-        GSX_CUDA_CHECK(cudaStreamSynchronize(st));
-        *n_dense_host = (int64_t)hc[kDense];
-        if (n_voxels_host) *n_voxels_host = (int64_t)hc[kDistinct];
-        // The reference puts a NaN row in a voxel outside the finite box.  Fewer than thr such rows make no dense
-        // voxel, so dropping them is exact; with thr or more, one of those voxels may be dense, and that is refused.
-        GSX_REQUIRE(hc[kOutside] < (unsigned long long)thr, GSX_ERR_UNSUPPORTED,
-                    "density: %llu points have non-finite (NaN) coordinates, at least min_points = %d", hc[kOutside],
-                    thr);
-        GSX_REQUIRE((int64_t)hc[kDense] <= cap, GSX_ERR_WORKSPACE, "density: %llu dense voxels exceed cap %lld",
-                    hc[kDense], (long long)cap);
-        const int64_t nd = (int64_t)hc[kDense];
-        if (nd > 0) {
-            k_vox_dense_counts<<<(int)((nd + 127) / 128), 128, 0, st>>>(dvox, nd, g, tab, dcnt);
-            GSX_KERNEL_CHECK();
-            GSX_CUDA_CHECK(cudaMemcpyAsync(dense_vox_host, dvox, (size_t)nd * 24, cudaMemcpyDeviceToHost, st));
-            GSX_CUDA_CHECK(cudaMemcpyAsync(dense_cnt_host, dcnt, (size_t)nd * 4, cudaMemcpyDeviceToHost, st));
-            GSX_CUDA_CHECK(cudaStreamSynchronize(st));
-        }
-        return GSX_OK;
-    };
-
-    if (cells * 4.0 <= (double)blob_bytes) {
-        const GridTable tab{(int*)blob};
-        const size_t ncell = (size_t)g.dim[0] * g.dim[1] * g.dim[2];
-        GSX_CUDA_CHECK(cudaMemsetAsync(blob, 0, ncell * 4, st));
-        if (ncell <= (size_t)kSmemCells) {
-            rc = launch_vox_count_smem(xyz, n, voxel, g, ncell, thr, tab.cnt, counters, dvox, cap, counters + kOutside,
-                                       st);
-            if (rc) return rc;
-        } else if (ncell < 0xfffffff0ull) {
-            const int ablocks = (int)((n + 256 * kAggItems - 1) / (256 * kAggItems));
-            k_vox_count_grid_agg<<<ablocks, 256, 0, st>>>(xyz, n, voxel, g, thr, tab.cnt, counters, dvox, cap);
-        } else {
-            count_rows(tab);
-        }
-        return read_dense(tab);
-    }
-    size_t slots = 64;
-    while (slots < (size_t)2 * n) slots <<= 1;
-    GSX_REQUIRE(slots * 12 <= blob_bytes, GSX_ERR_WORKSPACE, "density: workspace too small for the hash table");
-    if (!wide) {
-        const HashTable tab{(unsigned long long*)blob, (int*)(blob + slots * 8), slots - 1};
-        GSX_CUDA_CHECK(cudaMemsetAsync(blob, 0, slots * 12, st));
-        count_rows(tab);
-        return read_dense(tab);
-    }
-    slots >>= 1;   // two-word keys in the same budget: half the slots (still >= n), 20 bytes each
-    const WideHashTable tab{(unsigned long long*)blob, (unsigned long long*)blob + slots, (int*)(blob + slots * 16),
-                            slots - 1};
-    GSX_CUDA_CHECK(cudaMemsetAsync(blob, 0, slots * 20, st));
-    count_rows(tab);
-    return read_dense(tab);
-}
-
 // ---------------------------------------------------------------- staged dense-grid API (multi-GPU)
 // Rank-local histogram into a caller-owned int32 grid over a caller-chosen voxel box (the global one);
 // the caller all-reduces the grid and then extracts the dense voxels.
@@ -489,66 +375,6 @@ static int make_grid(const int64_t* q0, const int64_t* dim, VoxGrid& g, size_t& 
     }
     GSX_REQUIRE(cells < 4.0e9, GSX_ERR_UNSUPPORTED, "density: grid too large for the dense path");
     ncell = (size_t)dim[0] * dim[1] * dim[2];
-    return GSX_OK;
-}
-
-void density_voxel_range(const float* minmax_host, float voxel, int64_t* q0, int64_t* dim) {
-    for (int a = 0; a < 3; ++a) {
-        q0[a] = voxel_of(minmax_host[a], voxel);
-        dim[a] = voxel_of(minmax_host[3 + a], voxel) - q0[a] + 1;
-    }
-}
-
-int density_grid_count(const float* xyz, int64_t n, float voxel, const int64_t* q0, const int64_t* dim, int* grid_dev,
-                       unsigned long long* oob_dev, cudaStream_t st) {
-    if (n == 0) return GSX_OK;
-    GSX_REQUIRE(voxel > 0.f, GSX_ERR_ARG, "density: voxel size must be > 0");
-    VoxGrid g;
-    size_t ncell;
-    int rc = make_grid(q0, dim, g, ncell);
-    if (rc) return rc;
-    if (ncell <= (size_t)kSmemCells) {
-        rc = launch_vox_count_smem(xyz, n, voxel, g, ncell, 0, grid_dev, nullptr, nullptr, 0, oob_dev, st);
-        if (rc) return rc;
-    } else {
-        k_vox_count<false><<<(int)((n + 255) / 256), 256, 0, st>>>(xyz, n, voxel, g, GridTable{grid_dev}, 0, nullptr,
-                                                                   nullptr, 0, oob_dev);
-    }
-    GSX_KERNEL_CHECK();
-    return GSX_OK;
-}
-
-int density_grid_dense(const int* grid_dev, const int64_t* q0, const int64_t* dim, int64_t min_points,
-                       int64_t* dense_vox_host, int32_t* dense_cnt_host, int64_t cap, int64_t* n_dense_host,
-                       int64_t* n_voxels_host, void* ws, int64_t ws_bytes, cudaStream_t st) {
-    VoxGrid g;
-    size_t ncell;
-    int rc = make_grid(q0, dim, g, ncell);
-    if (rc) return rc;
-    GSX_REQUIRE(cap >= 1, GSX_ERR_ARG, "density: cap must be >= 1");
-    Carver c(ws, (size_t)ws_bytes);
-    unsigned long long* counters = c.take<unsigned long long>(4);
-    long long* dvox = c.take<long long>(3 * (size_t)cap);
-    int* dcnt = c.take<int>((size_t)cap);
-    GSX_REQUIRE(c.ok(), GSX_ERR_WORKSPACE, "density: workspace too small for cap=%lld", (long long)cap);
-    long long thr_ll = min_points < 1 ? 1 : min_points;
-    GSX_REQUIRE(thr_ll < 2147483647ll, GSX_ERR_ARG, "density: min_points too large");
-    GSX_CUDA_CHECK(cudaMemsetAsync(counters, 0, 4 * sizeof(unsigned long long), st));
-    k_vox_grid_dense<<<(unsigned)((ncell + 255) / 256), 256, 0, st>>>(grid_dev, ncell, g, (int)thr_ll, counters, dvox,
-                                                                      dcnt, cap);
-    GSX_KERNEL_CHECK();
-    unsigned long long hc[2];   // counters[kDense], [kDistinct]
-    GSX_CUDA_CHECK(cudaMemcpyAsync(hc, counters, sizeof(hc), cudaMemcpyDeviceToHost, st));
-    GSX_CUDA_CHECK(cudaStreamSynchronize(st));
-    *n_dense_host = (int64_t)hc[kDense];
-    if (n_voxels_host) *n_voxels_host = (int64_t)hc[kDistinct];
-    GSX_REQUIRE((int64_t)hc[kDense] <= cap, GSX_ERR_WORKSPACE, "density: %llu dense voxels exceed cap %lld",
-                hc[kDense], (long long)cap);
-    if (hc[kDense] > 0) {
-        GSX_CUDA_CHECK(cudaMemcpyAsync(dense_vox_host, dvox, (size_t)hc[kDense] * 24, cudaMemcpyDeviceToHost, st));
-        GSX_CUDA_CHECK(cudaMemcpyAsync(dense_cnt_host, dcnt, (size_t)hc[kDense] * 4, cudaMemcpyDeviceToHost, st));
-        GSX_CUDA_CHECK(cudaStreamSynchronize(st));
-    }
     return GSX_OK;
 }
 
@@ -653,8 +479,194 @@ static int launch_member(const float* xyz, int64_t n, float voxel, const Set& se
 
 constexpr unsigned long long kMaxKeepBits = 1ull << 27;   // 16 MiB of bitmap at most; larger boxes use the hash set
 
-int density_member_mask(const float* xyz, int64_t n, float voxel, const int64_t* keep, int64_t n_keep, uint8_t* mask,
-                        void* ws, int64_t ws_bytes, cudaStream_t st) {
+}  // namespace gsx
+
+using namespace gsx;
+
+extern "C" {
+
+int64_t gsx_density_workspace_bytes(int64_t n, int64_t cap) {
+    if (n < 1) n = 1;
+    if (cap < 1) cap = 1;
+    // hash path: table of >= 2n slots (power of two), 8-byte key + 4-byte count; plus minmax scratch
+    size_t slots = 64;
+    while (slots < (size_t)2 * n) slots <<= 1;
+    return (int64_t)(slots * 12 + 6 * 1024 * 4 + (size_t)cap * 28 + 8192);
+}
+
+int gsx_density_voxel_count(const float* xyz, int64_t n, float voxel, int64_t min_points, int64_t* dense_vox_host,
+                            int32_t* dense_cnt_host, int64_t cap, int64_t* n_dense_host, int64_t* n_voxels_host,
+                            void* ws, int64_t ws_bytes, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
+    GSX_NVTX("gsx::density_voxel_count");
+    GSX_REQUIRE(n >= 1, GSX_ERR_ARG, "density: n must be >= 1");
+    GSX_REQUIRE(voxel > 0.f, GSX_ERR_ARG, "density: voxel size must be > 0");
+    GSX_REQUIRE(ws_bytes >= gsx_density_workspace_bytes(n, cap), GSX_ERR_WORKSPACE, "density: workspace too small");
+    GSX_REQUIRE(cap >= 1, GSX_ERR_ARG, "density: cap must be >= 1");
+    Carver c(ws, (size_t)ws_bytes);
+    float* partial = c.take<float>(6 * 1024);
+    float* minmax = c.take<float>(8);
+    unsigned long long* counters = c.take<unsigned long long>(4);
+    long long* dvox = c.take<long long>(3 * (size_t)cap);
+    int* dcnt = c.take<int>((size_t)cap);
+    size_t used = align_up(c.off, 256);
+    GSX_REQUIRE(c.ok() && used < (size_t)ws_bytes, GSX_ERR_WORKSPACE, "density: workspace too small for cap=%lld",
+                (long long)cap);
+    char* blob = (char*)ws + used;
+    size_t blob_bytes = (size_t)ws_bytes - used;
+
+    int rc = sor_minmax(xyz, n, minmax, partial, st);
+    if (rc) return rc;
+    float mm[6];
+    GSX_CUDA_CHECK(cudaMemcpyAsync(mm, minmax, sizeof(mm), cudaMemcpyDeviceToHost, st));
+    GSX_CUDA_CHECK(cudaStreamSynchronize(st));
+    VoxGrid g;
+    double cells = 1.0;
+    bool wide = false;
+    for (int a = 0; a < 3; ++a) {
+        g.q0[a] = voxel_of(mm[a], voxel);  // floor(x/voxel) is monotone in x: min/max commute with it
+        long long q1 = voxel_of(mm[3 + a], voxel);
+        GSX_REQUIRE(g.q0[a] != LLONG_MIN && q1 != LLONG_MIN, GSX_ERR_UNSUPPORTED,
+                    "density: non-finite or out-of-range coordinates on axis %d", a);
+        // q1 >= q0; the unsigned difference is exact where the signed one could overflow
+        GSX_REQUIRE((unsigned long long)q1 - (unsigned long long)g.q0[a] < (1ull << 31) - 1, GSX_ERR_UNSUPPORTED,
+                    "density: voxel grid extent on axis %d exceeds 2^31 voxels", a);
+        g.dim[a] = q1 - g.q0[a] + 1;
+        if (g.dim[a] >= kAxisLim) wide = true;  // the packed 3 x 21-bit key does not fit: two-word keys
+        cells *= (double)g.dim[a];
+    }
+    long long thr_ll = min_points < 1 ? 1 : min_points;
+    GSX_REQUIRE(thr_ll < 2147483647ll, GSX_ERR_ARG, "density: min_points too large");
+    int thr = (int)thr_ll;
+    GSX_CUDA_CHECK(cudaMemsetAsync(counters, 0, 4 * sizeof(unsigned long long), st));
+    auto count_rows = [&](const auto& tab) {
+        k_vox_count<true><<<(int)((n + 255) / 256), 256, 0, st>>>(xyz, n, voxel, g, tab, thr, counters, dvox, cap,
+                                                                  counters + kOutside);
+    };
+    // After the histogram: the refusals, then the counts of the dense voxels looked up in `tab`.
+    auto read_dense = [&](const auto& tab) -> int {
+        GSX_KERNEL_CHECK();
+        unsigned long long hc[3];   // counters[kDense], [kDistinct], [kOutside]
+        GSX_CUDA_CHECK(cudaMemcpyAsync(hc, counters, sizeof(hc), cudaMemcpyDeviceToHost, st));
+        GSX_CUDA_CHECK(cudaStreamSynchronize(st));
+        *n_dense_host = (int64_t)hc[kDense];
+        if (n_voxels_host) *n_voxels_host = (int64_t)hc[kDistinct];
+        // The reference puts a NaN row in a voxel outside the finite box.  Fewer than thr such rows make no dense
+        // voxel, so dropping them is exact; with thr or more, one of those voxels may be dense, and that is refused.
+        GSX_REQUIRE(hc[kOutside] < (unsigned long long)thr, GSX_ERR_UNSUPPORTED,
+                    "density: %llu points have non-finite (NaN) coordinates, at least min_points = %d", hc[kOutside],
+                    thr);
+        GSX_REQUIRE((int64_t)hc[kDense] <= cap, GSX_ERR_WORKSPACE, "density: %llu dense voxels exceed cap %lld",
+                    hc[kDense], (long long)cap);
+        const int64_t nd = (int64_t)hc[kDense];
+        if (nd > 0) {
+            k_vox_dense_counts<<<(int)((nd + 127) / 128), 128, 0, st>>>(dvox, nd, g, tab, dcnt);
+            GSX_KERNEL_CHECK();
+            GSX_CUDA_CHECK(cudaMemcpyAsync(dense_vox_host, dvox, (size_t)nd * 24, cudaMemcpyDeviceToHost, st));
+            GSX_CUDA_CHECK(cudaMemcpyAsync(dense_cnt_host, dcnt, (size_t)nd * 4, cudaMemcpyDeviceToHost, st));
+            GSX_CUDA_CHECK(cudaStreamSynchronize(st));
+        }
+        return GSX_OK;
+    };
+
+    if (cells * 4.0 <= (double)blob_bytes) {
+        const GridTable tab{(int*)blob};
+        const size_t ncell = (size_t)g.dim[0] * g.dim[1] * g.dim[2];
+        GSX_CUDA_CHECK(cudaMemsetAsync(blob, 0, ncell * 4, st));
+        if (ncell <= (size_t)kSmemCells) {
+            rc = launch_vox_count_smem(xyz, n, voxel, g, ncell, thr, tab.cnt, counters, dvox, cap, counters + kOutside,
+                                       st);
+            if (rc) return rc;
+        } else if (ncell < 0xfffffff0ull) {
+            const int ablocks = (int)((n + 256 * kAggItems - 1) / (256 * kAggItems));
+            k_vox_count_grid_agg<<<ablocks, 256, 0, st>>>(xyz, n, voxel, g, thr, tab.cnt, counters, dvox, cap);
+        } else {
+            count_rows(tab);
+        }
+        return read_dense(tab);
+    }
+    size_t slots = 64;
+    while (slots < (size_t)2 * n) slots <<= 1;
+    GSX_REQUIRE(slots * 12 <= blob_bytes, GSX_ERR_WORKSPACE, "density: workspace too small for the hash table");
+    if (!wide) {
+        const HashTable tab{(unsigned long long*)blob, (int*)(blob + slots * 8), slots - 1};
+        GSX_CUDA_CHECK(cudaMemsetAsync(blob, 0, slots * 12, st));
+        count_rows(tab);
+        return read_dense(tab);
+    }
+    slots >>= 1;   // two-word keys in the same budget: half the slots (still >= n), 20 bytes each
+    const WideHashTable tab{(unsigned long long*)blob, (unsigned long long*)blob + slots, (int*)(blob + slots * 16),
+                            slots - 1};
+    GSX_CUDA_CHECK(cudaMemsetAsync(blob, 0, slots * 20, st));
+    count_rows(tab);
+    return read_dense(tab);
+}
+
+void gsx_density_voxel_range(const float* minmax_host, float voxel, int64_t* q0, int64_t* dim) {
+    for (int a = 0; a < 3; ++a) {
+        q0[a] = voxel_of(minmax_host[a], voxel);
+        dim[a] = voxel_of(minmax_host[3 + a], voxel) - q0[a] + 1;
+    }
+}
+
+int gsx_density_grid_count(const float* xyz, int64_t n, float voxel, const int64_t* q0, const int64_t* dim,
+                           int32_t* grid_dev, unsigned long long* oob_dev, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
+    if (n == 0) return GSX_OK;
+    GSX_REQUIRE(voxel > 0.f, GSX_ERR_ARG, "density: voxel size must be > 0");
+    VoxGrid g;
+    size_t ncell;
+    int rc = make_grid(q0, dim, g, ncell);
+    if (rc) return rc;
+    if (ncell <= (size_t)kSmemCells) {
+        rc = launch_vox_count_smem(xyz, n, voxel, g, ncell, 0, grid_dev, nullptr, nullptr, 0, oob_dev, st);
+        if (rc) return rc;
+    } else {
+        k_vox_count<false><<<(int)((n + 255) / 256), 256, 0, st>>>(xyz, n, voxel, g, GridTable{grid_dev}, 0, nullptr,
+                                                                   nullptr, 0, oob_dev);
+    }
+    GSX_KERNEL_CHECK();
+    return GSX_OK;
+}
+
+int gsx_density_grid_dense(const int32_t* grid_dev, const int64_t* q0, const int64_t* dim, int64_t min_points,
+                           int64_t* dense_vox_host, int32_t* dense_cnt_host, int64_t cap, int64_t* n_dense_host,
+                           int64_t* n_voxels_host, void* ws, int64_t ws_bytes, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
+    VoxGrid g;
+    size_t ncell;
+    int rc = make_grid(q0, dim, g, ncell);
+    if (rc) return rc;
+    GSX_REQUIRE(cap >= 1, GSX_ERR_ARG, "density: cap must be >= 1");
+    Carver c(ws, (size_t)ws_bytes);
+    unsigned long long* counters = c.take<unsigned long long>(4);
+    long long* dvox = c.take<long long>(3 * (size_t)cap);
+    int* dcnt = c.take<int>((size_t)cap);
+    GSX_REQUIRE(c.ok(), GSX_ERR_WORKSPACE, "density: workspace too small for cap=%lld", (long long)cap);
+    long long thr_ll = min_points < 1 ? 1 : min_points;
+    GSX_REQUIRE(thr_ll < 2147483647ll, GSX_ERR_ARG, "density: min_points too large");
+    GSX_CUDA_CHECK(cudaMemsetAsync(counters, 0, 4 * sizeof(unsigned long long), st));
+    k_vox_grid_dense<<<(unsigned)((ncell + 255) / 256), 256, 0, st>>>(grid_dev, ncell, g, (int)thr_ll, counters, dvox,
+                                                                      dcnt, cap);
+    GSX_KERNEL_CHECK();
+    unsigned long long hc[2];   // counters[kDense], [kDistinct]
+    GSX_CUDA_CHECK(cudaMemcpyAsync(hc, counters, sizeof(hc), cudaMemcpyDeviceToHost, st));
+    GSX_CUDA_CHECK(cudaStreamSynchronize(st));
+    *n_dense_host = (int64_t)hc[kDense];
+    if (n_voxels_host) *n_voxels_host = (int64_t)hc[kDistinct];
+    GSX_REQUIRE((int64_t)hc[kDense] <= cap, GSX_ERR_WORKSPACE, "density: %llu dense voxels exceed cap %lld",
+                hc[kDense], (long long)cap);
+    if (hc[kDense] > 0) {
+        GSX_CUDA_CHECK(cudaMemcpyAsync(dense_vox_host, dvox, (size_t)hc[kDense] * 24, cudaMemcpyDeviceToHost, st));
+        GSX_CUDA_CHECK(cudaMemcpyAsync(dense_cnt_host, dcnt, (size_t)hc[kDense] * 4, cudaMemcpyDeviceToHost, st));
+        GSX_CUDA_CHECK(cudaStreamSynchronize(st));
+    }
+    return GSX_OK;
+}
+
+int gsx_density_member_mask(const float* xyz, int64_t n, float voxel, const int64_t* keep, int64_t n_keep,
+                            uint8_t* mask, void* ws, int64_t ws_bytes, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
     GSX_NVTX("gsx::density_member_mask");
     if (n == 0) return GSX_OK;
     GSX_REQUIRE(voxel > 0.f, GSX_ERR_ARG, "density: voxel size must be > 0");
@@ -721,4 +733,4 @@ int density_member_mask(const float* xyz, int64_t n, float voxel, const int64_t*
     return launch_member(xyz, n, voxel, KeepHash<false>{o[0], o[1], o[2], set, slots - 1}, mask, st);
 }
 
-}  // namespace gsx
+}  // extern "C"

@@ -9,6 +9,8 @@
 // the user's buffer into a free pinned chunk and enqueues the DMA itself, so T memcpys and the DMAs of earlier
 // chunks overlap.  D2H is the mirror image (DMA into a pinned chunk, memcpy out while the next DMA runs).
 // A buffer that is already pinned / registered / managed goes straight to cudaMemcpyAsync.
+#include "../../include/gsx.h"
+
 #include "gsx_hostcopy.cuh"
 
 #include <algorithm>
@@ -303,3 +305,17 @@ int copy_d2h(void* dst_host, const void* src_dev, size_t bytes, cudaStream_t st)
 }
 
 }  // namespace gsx
+
+extern "C" {
+
+int gsx_copy_h2d(void* dst_dev, const void* src_host, int64_t bytes, void* stream) {
+    GSX_REQUIRE(bytes >= 0 && (bytes == 0 || (dst_dev && src_host)), GSX_ERR_ARG, "copy_h2d: bad arguments");
+    return gsx::copy_h2d(dst_dev, src_host, (size_t)bytes, (cudaStream_t)stream);
+}
+
+int gsx_copy_d2h(void* dst_host, const void* src_dev, int64_t bytes, void* stream) {
+    GSX_REQUIRE(bytes >= 0 && (bytes == 0 || (dst_host && src_dev)), GSX_ERR_ARG, "copy_d2h: bad arguments");
+    return gsx::copy_d2h(dst_host, src_dev, (size_t)bytes, (cudaStream_t)stream);
+}
+
+}  // extern "C"

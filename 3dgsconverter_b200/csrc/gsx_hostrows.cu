@@ -5,7 +5,9 @@
 // (:114,149,209,224) -- both single-threaded NumPy passes over 2.5 GB per 10 M splats.  The device-resident record
 // mode (gsx_records.cu) avoids them; when the records stay on the host (the default wiring) these two entry points do
 // the same passes with every core's memory bandwidth instead of one's.
-#include "gsx_hostrows.cuh"
+#include "../../include/gsx.h"
+
+#include "gsx_common.cuh"
 
 #include <algorithm>
 #include <atomic>
@@ -44,7 +46,13 @@ void parallel_rows(int64_t m, int T, F&& body) {   // body(begin, end) on T thre
 
 }  // namespace
 
-int host_gather_rows(const void* src, int64_t n_rows, int64_t row_bytes, const int64_t* idx, int64_t m, void* dst) {
+}  // namespace gsx
+
+using namespace gsx;
+
+extern "C" {
+
+int gsx_host_gather_rows(const void* src, int64_t n_rows, int64_t row_bytes, const int64_t* idx, int64_t m, void* dst) {
     GSX_REQUIRE(n_rows >= 0 && m >= 0 && row_bytes > 0, GSX_ERR_ARG, "host_gather_rows: bad sizes");
     if (m == 0) return GSX_OK;
     GSX_REQUIRE(src && idx && dst, GSX_ERR_ARG, "host_gather_rows: null pointer");
@@ -67,8 +75,8 @@ int host_gather_rows(const void* src, int64_t n_rows, int64_t row_bytes, const i
     return GSX_OK;
 }
 
-int host_extract_xyz_opacity(const void* src, int64_t n_rows, int64_t row_bytes, int64_t off_x, int64_t off_y,
-                             int64_t off_z, int64_t off_op, float* xyz_out, float* op_out) {
+int gsx_host_extract_xyz_opacity(const void* src, int64_t n_rows, int64_t row_bytes, int64_t off_x, int64_t off_y,
+                                 int64_t off_z, int64_t off_op, float* xyz_out, float* op_out) {
     GSX_REQUIRE(n_rows >= 0 && row_bytes >= 4, GSX_ERR_ARG, "host_extract: bad sizes");
     if (n_rows == 0) return GSX_OK;
     GSX_REQUIRE(src && xyz_out, GSX_ERR_ARG, "host_extract: null pointer");
@@ -96,4 +104,4 @@ int host_extract_xyz_opacity(const void* src, int64_t n_rows, int64_t row_bytes,
     return GSX_OK;
 }
 
-}  // namespace gsx
+}  // extern "C"

@@ -18,6 +18,8 @@
 //     order with 8 row loads in flight and accumulates lane-per-dimension.  This reproduces the
 //     oracle's serial index-order float32 sum bit-for-bit and is run-to-run deterministic (the
 //     reference's float atomics are neither).  K > 2047 falls back to a per-cluster label scan.
+#include "../../include/gsx.h"
+
 #include "gsx_common.cuh"
 #include "gsx_kmeans.cuh"
 
@@ -415,16 +417,6 @@ static KmWs km_carve(void* ws, size_t bytes, int64_t n_total, int nprob, int K, 
     return w;
 }
 
-int64_t kmeans_workspace_bytes(int64_t n_total, int nprob, int K, int D) {
-    (void)D;
-    if (nprob < 1) nprob = 1;
-    if (n_total < 1) n_total = 1;
-    // worst case number of sub-tiles: every problem adds at most one partial tile
-    long long nsub = n_total / kSubTile + nprob + 1;
-    KmWs w = km_carve(nullptr, 0, n_total, nprob, K, nsub);
-    return (int64_t)w.total + 1024;
-}
-
 template <int D>
 static void launch_assign(const float* X, const float* C, int* labels, const KmProb* probs, int nprob, int K,
                           int tiles, cudaStream_t st) {
@@ -445,9 +437,26 @@ static int points_per_thread(int D) {
     }
 }
 
-int kmeans_lloyd(const float* X, const int64_t* row_off, int nprob, int K, int D, int max_iter, float* C, int* labels,
-                 int* counts, void* ws, int64_t ws_bytes, int assign_mode, unsigned long long* tc_stats,
-                 cudaStream_t st) {
+}  // namespace gsx
+
+using namespace gsx;
+
+extern "C" {
+
+int64_t gsx_kmeans_workspace_bytes(int64_t n_total, int32_t nprob, int32_t K, int32_t D) {
+    (void)D;
+    if (nprob < 1) nprob = 1;
+    if (n_total < 1) n_total = 1;
+    // worst case number of sub-tiles: every problem adds at most one partial tile
+    long long nsub = n_total / kSubTile + nprob + 1;
+    KmWs w = km_carve(nullptr, 0, n_total, nprob, K, nsub);
+    return (int64_t)w.total + 1024;
+}
+
+int gsx_kmeans_lloyd_device(const float* X, const int64_t* row_off, int32_t nprob, int32_t K, int32_t D,
+                            int32_t max_iter, float* C, int32_t* labels, int32_t* counts, void* ws, int64_t ws_bytes,
+                            int32_t assign_mode, unsigned long long* tc_stats, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
     GSX_NVTX("gsx::kmeans_lloyd");
     GSX_REQUIRE(assign_mode == GSX_KM_ASSIGN_AUTO || assign_mode == GSX_KM_ASSIGN_STRICT ||
                     assign_mode == GSX_KM_ASSIGN_TENSOR,
@@ -460,7 +469,7 @@ int kmeans_lloyd(const float* X, const int64_t* row_off, int nprob, int K, int D
     GSX_REQUIRE(nprob >= 1 && K >= 1 && D >= 1 && max_iter >= 0, GSX_ERR_ARG, "kmeans: bad shape");
     const int64_t n_total = row_off[nprob] - row_off[0];
     GSX_REQUIRE(row_off[0] == 0, GSX_ERR_ARG, "kmeans: row_off[0] must be 0");
-    GSX_REQUIRE(ws_bytes >= kmeans_workspace_bytes(n_total, nprob, K, D), GSX_ERR_WORKSPACE,
+    GSX_REQUIRE(ws_bytes >= gsx_kmeans_workspace_bytes(n_total, nprob, K, D), GSX_ERR_WORKSPACE,
                 "kmeans: workspace too small");
     const int per_tile = kAssignThreads * points_per_thread(D);
     std::vector<KmProb> hp(nprob);
@@ -539,8 +548,9 @@ int kmeans_lloyd(const float* X, const int64_t* row_off, int nprob, int K, int D
 }
 
 // debug / test hook: raw tensor-core scores of the first 128 rows against K centroids (one problem)
-int kmeans_tc_debug_scores(const float* X, int64_t rows, const float* C, int K, int D, float* scores,
-                           void* ws, int64_t ws_bytes, cudaStream_t st) {
+int gsx_kmeans_tc_debug_scores(const float* X, int64_t rows, const float* C, int32_t K, int32_t D, float* scores,
+                               void* ws, int64_t ws_bytes, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
     GSX_REQUIRE(kmeans_tc_supported(K, D) && rows >= 1, GSX_ERR_UNSUPPORTED, "kmeans_tc_debug: unsupported shape");
     GSX_REQUIRE(ws_bytes >= 1024, GSX_ERR_WORKSPACE, "kmeans_tc_debug: workspace too small");
     KmProb hp;
@@ -561,4 +571,4 @@ int kmeans_tc_debug_scores(const float* X, int64_t rows, const float* C, int K, 
     return GSX_OK;
 }
 
-}  // namespace gsx
+}  // extern "C"

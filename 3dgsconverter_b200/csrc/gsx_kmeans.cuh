@@ -12,15 +12,9 @@ struct KmProb {
     int sub0;            // first label sub-tile (kSubTile points, one warp each) of the problem
 };
 
-int64_t kmeans_workspace_bytes(int64_t n_total, int nprob, int K, int D);
-int kmeans_lloyd(const float* X, const int64_t* row_off, int nprob, int K, int D, int max_iter, float* C, int* labels,
-                 int* counts, void* ws, int64_t ws_bytes, int assign_mode, unsigned long long* tc_stats,
-                 cudaStream_t st);
 // gsx_kmeans_tc.cu
 bool kmeans_tc_supported(int K, int D);
 int kmeans_assign_tc(const float* X, long long x_floats, const float* C, int* labels, const KmProb* probs_dev, int nprob,
                      int K, int D, long long tiles, int mode, float* dump, unsigned long long* stats,
                      int* err_flag_dev, cudaStream_t st);
-int kmeans_tc_debug_scores(const float* X, int64_t rows, const float* C, int K, int D, float* scores,
-                           void* ws, int64_t ws_bytes, cudaStream_t st);
 }

@@ -26,6 +26,8 @@
 // Data movement: a tile is 128 consecutive rows of X = 128*D*4 contiguous bytes; one elected thread moves it
 // global -> shared with a 1-D TMA bulk copy (cp.async.bulk, completion on an mbarrier) one tile ahead of the
 // MMA, then every thread re-lays its half row into the GMMA canonical K-major layout (no swizzle).
+#include "../../include/gsx.h"
+
 #include "gsx_common.cuh"
 #include "gsx_kmeans.cuh"
 
@@ -457,3 +459,7 @@ int kmeans_assign_tc(const float* X, long long x_floats, const float* C, int* la
 }
 
 }  // namespace gsx
+
+extern "C" int32_t gsx_kmeans_tensor_core_supported(int32_t K, int32_t D) {
+    return gsx::kmeans_tc_supported(K, D) ? 1 : 0;
+}

@@ -12,8 +12,9 @@
 // 32 / 1024 / 32768 / 1048576 sorted points; one warp per query walks the 4-level hierarchy nearest
 // box first and prunes with lb >= tau, where lb is evaluated with the same monotone float64 op
 // sequence as d^2 (so lb <= d^2 of every point in the box, exactly).
+#include "../../include/gsx.h"
+
 #include "gsx_common.cuh"
-#include "gsx_knn_exact.cuh"
 #include "gsx_sor.cuh"
 
 #include "gsx_radix.cuh"
@@ -65,12 +66,6 @@ static ExWs ex_carve(void* ws, size_t bytes, int64_t n, size_t sort_ws_bytes) {
     w.total = align_up(c.off, 256);
     w.ok = c.ok();
     return w;
-}
-
-int64_t knn_exact_workspace_bytes(int64_t n) {
-    if (n < 1) n = 1;
-    ExWs w = ex_carve(nullptr, 0, n, ex_sort_ws_bytes(n));
-    return (int64_t)w.total + 1024;
 }
 
 __device__ __forceinline__ uint64_t spread16(uint32_t v) {  // 16 bits -> every third bit of 48
@@ -299,8 +294,21 @@ __global__ void __launch_bounds__(256, 4)
     }
 }
 
-int knn_exact_mean_dists(const float* xyz, int64_t n, int k, float* means, void* ws, int64_t ws_bytes,
-                         cudaStream_t st) {
+}  // namespace gsx
+
+using namespace gsx;
+
+extern "C" {
+
+int64_t gsx_knn_exact_workspace_bytes(int64_t n) {
+    if (n < 1) n = 1;
+    ExWs w = ex_carve(nullptr, 0, n, ex_sort_ws_bytes(n));
+    return (int64_t)w.total + 1024;
+}
+
+int gsx_knn_exact_mean_dists(const float* xyz, int64_t n, int32_t k, float* means, void* ws, int64_t ws_bytes,
+                             void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
     GSX_REQUIRE(n >= 1 && n < 2147483584ll, GSX_ERR_ARG, "knn_exact: n out of range");
     GSX_REQUIRE(k >= 1 && k <= 63, GSX_ERR_UNSUPPORTED, "knn_exact: k must be in [1,63] (got %d)", k);
     ExWs w = ex_carve(ws, (size_t)ws_bytes, n, ex_sort_ws_bytes(n));
@@ -345,4 +353,4 @@ int knn_exact_mean_dists(const float* xyz, int64_t n, int k, float* means, void*
     return GSX_OK;
 }
 
-}  // namespace gsx
+}  // extern "C"

@@ -4,8 +4,11 @@
 // per SURVEY A.4: bbox = six closed-interval float32 compares (the Python-float bounds are NumPy-2
 // weak scalars, i.e. rounded to float32 by the caller); alpha = float64 compare of the float32
 // opacity against the float64 logit threshold.
+#include "../../include/gsx.h"
+
 #include "gsx_common.cuh"
-#include "gsx_masks.cuh"
+
+#include <math.h>
 
 namespace gsx {
 
@@ -34,7 +37,29 @@ __global__ void __launch_bounds__(256) k_bbox_mask1(const float* __restrict__ xy
     mask[i] = x >= lx && x <= hx && y >= ly && y <= hy && z >= lz && z <= hz;
 }
 
-int bbox_mask(const float* xyz, int64_t n, const float* lohi, uint8_t* mask, cudaStream_t st) {
+__global__ void __launch_bounds__(256) k_alpha_mask(const float* __restrict__ op, int64_t begin, int64_t n, double t,
+                                                    uint8_t* __restrict__ mask) {
+    int64_t i = begin + (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) mask[i] = (double)op[i] >= t;
+}
+
+__global__ void __launch_bounds__(256) k_alpha_mask4(const float4* __restrict__ op4, int64_t n4, double t,
+                                                     uchar4* __restrict__ mask4) {
+    int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n4) return;
+    float4 v = ld_stream_f4(op4 + i);
+    mask4[i] = make_uchar4((double)v.x >= t, (double)v.y >= t, (double)v.z >= t, (double)v.w >= t);
+}
+
+}  // namespace gsx
+
+using namespace gsx;
+
+extern "C" {
+
+int gsx_bbox_mask(const float* xyz, int64_t n, const float* lohi, uint8_t* mask, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
+    GSX_REQUIRE(n >= 0, GSX_ERR_ARG, "bbox: n < 0");
     if (n == 0) return GSX_OK;
     int64_t n4 = 0;
     if (((uintptr_t)xyz % 16 == 0) && ((uintptr_t)mask % 4 == 0)) {
@@ -54,21 +79,9 @@ int bbox_mask(const float* xyz, int64_t n, const float* lohi, uint8_t* mask, cud
     return GSX_OK;
 }
 
-__global__ void __launch_bounds__(256) k_alpha_mask(const float* __restrict__ op, int64_t begin, int64_t n, double t,
-                                                    uint8_t* __restrict__ mask) {
-    int64_t i = begin + (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) mask[i] = (double)op[i] >= t;
-}
-
-__global__ void __launch_bounds__(256) k_alpha_mask4(const float4* __restrict__ op4, int64_t n4, double t,
-                                                     uchar4* __restrict__ mask4) {
-    int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n4) return;
-    float4 v = ld_stream_f4(op4 + i);
-    mask4[i] = make_uchar4((double)v.x >= t, (double)v.y >= t, (double)v.z >= t, (double)v.w >= t);
-}
-
-int alpha_mask(const float* opacity, int64_t n, double logit_thresh, uint8_t* mask, cudaStream_t st) {
+int gsx_alpha_mask(const float* opacity, int64_t n, double logit_thresh, uint8_t* mask, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
+    GSX_REQUIRE(n >= 0, GSX_ERR_ARG, "alpha: n < 0");
     if (n == 0) return GSX_OK;
     int64_t n4 = 0;
     if (((uintptr_t)opacity % 16 == 0) && ((uintptr_t)mask % 4 == 0)) {
@@ -86,4 +99,11 @@ int alpha_mask(const float* opacity, int64_t n, double logit_thresh, uint8_t* ma
     return GSX_OK;
 }
 
-}  // namespace gsx
+double gsx_alpha_logit_threshold(double min_opacity_u8) {
+    double a = min_opacity_u8 / 255.0;
+    if (a < 1e-6) a = 1e-6;
+    if (a > 1.0 - 1e-6) a = 1.0 - 1e-6;
+    return log(a / (1.0 - a));
+}
+
+}  // extern "C"

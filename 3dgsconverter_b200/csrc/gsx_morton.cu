@@ -17,8 +17,9 @@
 //                      float32 matrix over consecutive chunks of the (optionally permuted) rows.
 // Float arithmetic of the codes follows NumPy-2 float32 semantics: (c - min) * (1024.0 / len), clip to [0,1023],
 // truncation to uint32.
+#include "../../include/gsx.h"
+
 #include "gsx_common.cuh"
-#include "gsx_morton.cuh"
 #include "gsx_radix.cuh"
 #include "gsx_sor.cuh"
 
@@ -189,7 +190,56 @@ __global__ void k_mo_iota(int32_t* __restrict__ order, int64_t n) {
     if (i < n) order[i] = (int32_t)i;
 }
 
-int64_t morton_workspace_bytes(int64_t n) {
+// ---------------------------------------------------------------------------------------------------------
+// chunk min/max: one block per chunk, `ncol` (<= 8) columns of a row-major [n, F] matrix, rows optionally permuted.
+// A NaN makes its chunk's min and max NaN (np.minimum.reduceat); of two zeros the min is -0.0 and the max +0.0.
+__global__ void __launch_bounds__(256) k_chunk_minmax(const float* __restrict__ rows, int F, const int32_t* __restrict__ order,
+                                                      int64_t n, int chunk, int ncol, const int* __restrict__ cols,
+                                                      float clip_lo, float clip_hi, float* __restrict__ lo_out,
+                                                      float* __restrict__ hi_out) {
+    const int64_t c0 = (int64_t)blockIdx.x * chunk;
+    const int64_t c1 = c0 + chunk < n ? c0 + chunk : n;
+    float lo[8], hi[8];
+#pragma unroll
+    for (int a = 0; a < 8; ++a) lo[a] = INFINITY, hi[a] = -INFINITY;
+    for (int64_t j = c0 + threadIdx.x; j < c1; j += blockDim.x) {
+        const float* r = rows + (size_t)(order ? order[j] : j) * F;
+#pragma unroll
+        for (int a = 0; a < 8; ++a)
+            if (a < ncol) {
+                float v = __ldg(r + cols[a]);
+                v = v != v ? v : fminf(fmaxf(v, clip_lo), clip_hi);   // np.clip keeps NaN
+                lo[a] = nan_min(lo[a], v);
+                hi[a] = nan_max(hi[a], v);
+            }
+    }
+    __shared__ float slo[8][8], shi[8][8];
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+#pragma unroll
+    for (int a = 0; a < 8; ++a) {
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            lo[a] = nan_min(lo[a], __shfl_xor_sync(GSX_FULL, lo[a], o));
+            hi[a] = nan_max(hi[a], __shfl_xor_sync(GSX_FULL, hi[a], o));
+        }
+        if (lane == 0) slo[a][w] = lo[a], shi[a][w] = hi[a];
+    }
+    __syncthreads();
+    if (threadIdx.x < ncol) {
+        float l = slo[threadIdx.x][0], h = shi[threadIdx.x][0];
+        for (int k = 1; k < 8; ++k) l = nan_min(l, slo[threadIdx.x][k]), h = nan_max(h, shi[threadIdx.x][k]);
+        lo_out[(size_t)blockIdx.x * ncol + threadIdx.x] = l;
+        hi_out[(size_t)blockIdx.x * ncol + threadIdx.x] = h;
+    }
+}
+
+}  // namespace gsx
+
+using namespace gsx;
+
+extern "C" {
+
+int64_t gsx_morton_workspace_bytes(int64_t n) {
     if (n < 1) n = 1;
     size_t b = 2 * align_up((size_t)n * 8, 256) + 2 * align_up((size_t)n * 4, 256) + radix_ws_bytes(n);
     b += align_up((size_t)(n + 1) * 4, 256) + scan_workspace_bytes(n + 1) + align_up((size_t)n * 4, 256);  // flags, starts
@@ -198,14 +248,15 @@ int64_t morton_workspace_bytes(int64_t n) {
     return (int64_t)b;
 }
 
-int morton_order(const float* xyz, int64_t n, int32_t* order, int limit, int* levels_out, void* ws, int64_t ws_bytes,
-                 cudaStream_t st) {
+int gsx_morton_order(const float* xyz, int64_t n, int32_t* order, int32_t limit, int32_t* levels_out, void* ws,
+                     int64_t ws_bytes, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
     GSX_NVTX("gsx::morton_order");
-    GSX_REQUIRE(n >= 0 && n < 2147483584ll, GSX_ERR_ARG, "morton: n out of range");
     if (levels_out) *levels_out = 0;
+    GSX_REQUIRE(n >= 0 && n < 2147483584ll, GSX_ERR_ARG, "morton: n out of range");
     if (n == 0) return GSX_OK;
     GSX_REQUIRE(limit >= 1, GSX_ERR_ARG, "morton: limit must be >= 1");
-    GSX_REQUIRE(ws_bytes >= morton_workspace_bytes(n), GSX_ERR_WORKSPACE, "morton: workspace too small");
+    GSX_REQUIRE(ws_bytes >= gsx_morton_workspace_bytes(n), GSX_ERR_WORKSPACE, "morton: workspace too small");
     Carver c(ws, (size_t)ws_bytes);
     uint64_t* k0 = c.take<uint64_t>((size_t)n);
     uint64_t* k1 = c.take<uint64_t>((size_t)n);
@@ -288,51 +339,10 @@ int morton_order(const float* xyz, int64_t n, int32_t* order, int limit, int* le
     return GSX_OK;
 }
 
-// ---------------------------------------------------------------------------------------------------------
-// chunk min/max: one block per chunk, `ncol` (<= 8) columns of a row-major [n, F] matrix, rows optionally permuted.
-// A NaN makes its chunk's min and max NaN (np.minimum.reduceat); of two zeros the min is -0.0 and the max +0.0.
-__global__ void __launch_bounds__(256) k_chunk_minmax(const float* __restrict__ rows, int F, const int32_t* __restrict__ order,
-                                                      int64_t n, int chunk, int ncol, const int* __restrict__ cols,
-                                                      float clip_lo, float clip_hi, float* __restrict__ lo_out,
-                                                      float* __restrict__ hi_out) {
-    const int64_t c0 = (int64_t)blockIdx.x * chunk;
-    const int64_t c1 = c0 + chunk < n ? c0 + chunk : n;
-    float lo[8], hi[8];
-#pragma unroll
-    for (int a = 0; a < 8; ++a) lo[a] = INFINITY, hi[a] = -INFINITY;
-    for (int64_t j = c0 + threadIdx.x; j < c1; j += blockDim.x) {
-        const float* r = rows + (size_t)(order ? order[j] : j) * F;
-#pragma unroll
-        for (int a = 0; a < 8; ++a)
-            if (a < ncol) {
-                float v = __ldg(r + cols[a]);
-                v = v != v ? v : fminf(fmaxf(v, clip_lo), clip_hi);   // np.clip keeps NaN
-                lo[a] = nan_min(lo[a], v);
-                hi[a] = nan_max(hi[a], v);
-            }
-    }
-    __shared__ float slo[8][8], shi[8][8];
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-#pragma unroll
-    for (int a = 0; a < 8; ++a) {
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            lo[a] = nan_min(lo[a], __shfl_xor_sync(GSX_FULL, lo[a], o));
-            hi[a] = nan_max(hi[a], __shfl_xor_sync(GSX_FULL, hi[a], o));
-        }
-        if (lane == 0) slo[a][w] = lo[a], shi[a][w] = hi[a];
-    }
-    __syncthreads();
-    if (threadIdx.x < ncol) {
-        float l = slo[threadIdx.x][0], h = shi[threadIdx.x][0];
-        for (int k = 1; k < 8; ++k) l = nan_min(l, slo[threadIdx.x][k]), h = nan_max(h, shi[threadIdx.x][k]);
-        lo_out[(size_t)blockIdx.x * ncol + threadIdx.x] = l;
-        hi_out[(size_t)blockIdx.x * ncol + threadIdx.x] = h;
-    }
-}
-
-int chunk_minmax(const float* rows, int64_t n, int F, const int32_t* order, int chunk, const int* cols_host, int ncol,
-                 float clip_lo, float clip_hi, float* lo_out, float* hi_out, void* ws, int64_t ws_bytes, cudaStream_t st) {
+int gsx_chunk_minmax(const float* rows, int64_t n, int32_t F, const int32_t* order, int32_t chunk,
+                     const int32_t* cols_host, int32_t ncol, float clip_lo, float clip_hi, float* lo_out, float* hi_out,
+                     void* ws, int64_t ws_bytes, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
     if (n == 0) return GSX_OK;
     GSX_REQUIRE(ncol >= 1 && ncol <= 8 && chunk >= 1 && F >= 1, GSX_ERR_ARG, "chunk_minmax: bad shape");
     GSX_REQUIRE(ws_bytes >= 64, GSX_ERR_WORKSPACE, "chunk_minmax: needs 64 bytes of scratch");
@@ -345,4 +355,4 @@ int chunk_minmax(const float* rows, int64_t n, int F, const int32_t* order, int 
     return GSX_OK;
 }
 
-}  // namespace gsx
+}  // extern "C"

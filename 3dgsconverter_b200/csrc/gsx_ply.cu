@@ -17,9 +17,10 @@
 //                               outside int32 give 0.  NumPy's strided and contiguous loops agree on every float32
 //                               pattern and on the float64 edges (DESIGN 4.8).
 // Every other pairing is refused.  Field offsets may be any byte; rows up to kRowMax bytes.
+#include "../../include/gsx.h"
+
 #include "gsx_common.cuh"
 #include "gsx_numpy_scalar.cuh"
-#include "gsx_ply.cuh"
 #include "gsx_staged.cuh"
 
 namespace gsx {
@@ -116,8 +117,15 @@ __global__ void __launch_bounds__(kThreads) k_ply_transcode(const uint8_t* __res
 
 }  // namespace
 
-int ply_transcode(const uint8_t* src, int64_t n, int32_t src_row, uint8_t* dst, int32_t dst_row, const int32_t* fields,
-                  int32_t nf, cudaStream_t st) {
+}  // namespace gsx
+
+using namespace gsx;
+
+extern "C" {
+
+int gsx_ply_transcode(const uint8_t* src, int64_t n, int32_t src_row, uint8_t* dst, int32_t dst_row,
+                      const int32_t* fields, int32_t nf, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
     GSX_REQUIRE(n >= 0, GSX_ERR_ARG, "ply_transcode: n=%lld < 0", (long long)n);
     GSX_REQUIRE(n < 2147483648ll, GSX_ERR_UNSUPPORTED, "ply_transcode: n=%lld needs n < 2^31", (long long)n);
     GSX_REQUIRE(src_row >= 1 && src_row <= kRowMax && dst_row >= 1 && dst_row <= kRowMax, GSX_ERR_ARG,
@@ -150,4 +158,4 @@ int ply_transcode(const uint8_t* src, int64_t n, int32_t src_row, uint8_t* dst, 
     return GSX_OK;
 }
 
-}  // namespace gsx
+}  // extern "C"

@@ -13,6 +13,8 @@
 // Only the bits [begin_bit, end_bit) are sorted (the hash needs ceil(log2 N) bits, not 32): the last pass's digit is
 // masked to the bits below end_bit, so bits at and above end_bit do not take part.
 // HBM traffic per pass: 8 B (hist) + 12 B read + 12 B written per pair.
+#include "../../include/gsx.h"
+
 #include "gsx_common.cuh"
 #include "gsx_radix.cuh"
 
@@ -482,3 +484,36 @@ int radix_sort_keys(uint64_t* keys0, uint64_t* keys1, int64_t n, int begin_bit, 
 }
 
 }  // namespace gsx
+
+using namespace gsx;
+
+extern "C" {
+
+int64_t gsx_sort_pairs_workspace_bytes(int64_t n) {
+    if (n < 1) n = 1;
+    return (int64_t)(align_up((size_t)n * 8, 256) + align_up((size_t)n * 4, 256) + radix_ws_bytes(n) + 1024);
+}
+
+int gsx_sort_pairs(uint64_t* keys_dev, int32_t* vals_dev, int64_t n, int32_t begin_bit, int32_t end_bit, void* ws,
+                   int64_t ws_bytes, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
+    if (n == 0) return GSX_OK;
+    GSX_REQUIRE(ws_bytes >= gsx_sort_pairs_workspace_bytes(n), GSX_ERR_WORKSPACE, "sort: workspace too small");
+    Carver c(ws, (size_t)ws_bytes);
+    uint64_t* k1 = c.take<uint64_t>((size_t)n);
+    int32_t* v1 = c.take<int32_t>((size_t)n);
+    char* rws = c.take<char>(radix_ws_bytes(n));
+    uint64_t* ks = nullptr;
+    int32_t* vs = nullptr;
+    int rc = vals_dev ? radix_sort_pairs(keys_dev, k1, vals_dev, v1, n, begin_bit, end_bit, rws, radix_ws_bytes(n), &ks,
+                                         &vs, st)
+                      : radix_sort_keys(keys_dev, k1, n, begin_bit, end_bit, rws, radix_ws_bytes(n), &ks, st);
+    if (rc) return rc;
+    if (ks != keys_dev) {
+        GSX_CUDA_CHECK(cudaMemcpyAsync(keys_dev, ks, (size_t)n * 8, cudaMemcpyDeviceToDevice, st));
+        if (vals_dev) GSX_CUDA_CHECK(cudaMemcpyAsync(vals_dev, vs, (size_t)n * 4, cudaMemcpyDeviceToDevice, st));
+    }
+    return GSX_OK;
+}
+
+}  // extern "C"

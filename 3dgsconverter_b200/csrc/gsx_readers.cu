@@ -22,9 +22,10 @@
 // with the reference's own NumPy expression on the host, so NumPy's float32 and float64 log are reproduced without
 // restating them.  All other arithmetic is one __f*_rn / __d*_rn operation per NumPy operation in the reference's
 // order and precision (gsx_numpy_scalar.cuh), with x86's NaN results where NaN inputs can reach the output.
+#include "../../include/gsx.h"
+
 #include "gsx_common.cuh"
 #include "gsx_numpy_scalar.cuh"
-#include "gsx_readers.cuh"
 #include "gsx_staged.cuh"
 
 namespace gsx {
@@ -356,7 +357,14 @@ int grid(int64_t n) { return (int)((n + kRows - 1) / kRows); }
 
 }  // namespace
 
-int splat_decode(const uint8_t* data, int64_t n, const float* tables, uint8_t* rows, cudaStream_t st) {
+}  // namespace gsx
+
+using namespace gsx;
+
+extern "C" {
+
+int gsx_splat_decode(const uint8_t* data, int64_t n, const float* tables, uint8_t* rows, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
     int rc = check_rows(n, "splat_decode");
     if (rc) return rc;
     if (n == 0) return GSX_OK;
@@ -367,10 +375,11 @@ int splat_decode(const uint8_t* data, int64_t n, const float* tables, uint8_t* r
     return GSX_OK;
 }
 
-int ksplat_decode_section(const uint8_t* rec, int64_t n, int level, int sh_count, float sr, float sf,
-                          const uint8_t* centres, int64_t ncentres, int64_t full_buckets, int64_t bucket_size,
-                          const int64_t* partial_end, int32_t npartial, const float* tables, int32_t row_bytes,
-                          uint8_t* rows, cudaStream_t st) {
+int gsx_ksplat_decode_section(const uint8_t* rec, int64_t n, int32_t level, int32_t sh_count, float sr, float sf,
+                              const uint8_t* centres, int64_t ncentres, int64_t full_buckets, int64_t bucket_size,
+                              const int64_t* partial_end, int32_t npartial, const float* tables, int32_t row_bytes,
+                              uint8_t* rows, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
     int rc = check_rows(n, "ksplat_decode_section");
     if (rc) return rc;
     GSX_REQUIRE(level >= 0 && level <= 2, GSX_ERR_ARG, "ksplat_decode_section: level %d (0, 1, or 2 for any >= 2)",
@@ -409,8 +418,9 @@ int ksplat_decode_section(const uint8_t* rec, int64_t n, int level, int sh_count
     return GSX_OK;
 }
 
-int spz_decode(const uint8_t* body, int64_t n, int version, int sh_dim, int frac_bits, const float* tables,
-               int32_t row_bytes, uint8_t* rows, cudaStream_t st) {
+int gsx_spz_decode(const uint8_t* body, int64_t n, int32_t version, int32_t sh_dim, int32_t frac_bits,
+                   const float* tables, int32_t row_bytes, uint8_t* rows, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
     int rc = check_rows(n, "spz_decode");
     if (rc) return rc;
     GSX_REQUIRE(version >= 1 && version <= 3, GSX_ERR_ARG, "spz_decode: version %d", version);
@@ -433,10 +443,11 @@ int spz_decode(const uint8_t* body, int64_t n, int version, int sh_dim, int frac
     return GSX_OK;
 }
 
-int cply_decode(const uint8_t* chunk, int64_t nchunk, int32_t chunk_row, const int32_t* chunk_offs,
-                const uint8_t* vertex, int64_t n, int32_t vertex_row, const int32_t* vertex_offs, const uint8_t* sh,
-                int32_t sh_row, const int32_t* sh_offs, int32_t nsh, const float* tables, uint8_t* rows,
-                cudaStream_t st) {
+int gsx_cply_decode(const uint8_t* chunk, int64_t nchunk, int32_t chunk_row, const int32_t* chunk_offs,
+                    const uint8_t* vertex, int64_t n, int32_t vertex_row, const int32_t* vertex_offs, const uint8_t* sh,
+                    int32_t sh_row, const int32_t* sh_offs, int32_t nsh, const float* tables, uint8_t* rows,
+                    void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
     int rc = check_rows(n, "cply_decode");
     if (rc) return rc;
     GSX_REQUIRE(nchunk >= 0, GSX_ERR_ARG, "cply_decode: nchunk < 0");
@@ -474,4 +485,4 @@ int cply_decode(const uint8_t* chunk, int64_t nchunk, int32_t chunk_row, const i
     return GSX_OK;
 }
 
-}  // namespace gsx
+}  // extern "C"

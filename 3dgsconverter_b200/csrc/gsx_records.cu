@@ -14,8 +14,9 @@
 //                      -> RGBA8 (float32 ops in NumPy's order; the colour channels are bit-exact, the alpha channel
 //                      goes through expf and can differ from NumPy's SIMD exp by one count on ~1e-5 of the splats)
 //   k_scale_exp      : exp(scale_0..2) -> float32 [n,3]
+#include "../../include/gsx.h"
+
 #include "gsx_common.cuh"
-#include "gsx_records.cuh"
 
 namespace gsx {
 
@@ -78,8 +79,15 @@ static int check_cols(int F, std::initializer_list<int> cols) {
     return GSX_OK;
 }
 
-int records_extract_xyz_opacity(const float* rows, int64_t n, int F, int cx, int cy, int cz, int cop, float* xyz,
-                                float* opacity, cudaStream_t st) {
+}  // namespace gsx
+
+using namespace gsx;
+
+extern "C" {
+
+int gsx_records_extract_xyz_opacity(const float* rows, int64_t n, int32_t F, int32_t cx, int32_t cy, int32_t cz,
+                                    int32_t cop, float* xyz, float* opacity, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
     if (n == 0) return GSX_OK;
     GSX_REQUIRE(F >= 3, GSX_ERR_ARG, "records: bad row width %d", F);
     int rc = check_cols(F, {cx, cy, cz});
@@ -90,7 +98,8 @@ int records_extract_xyz_opacity(const float* rows, int64_t n, int F, int cx, int
     return GSX_OK;
 }
 
-int records_gather_rows(const float* rows, const int32_t* idx, int64_t m, int F, float* out, cudaStream_t st) {
+int gsx_records_gather_rows(const float* rows, const int32_t* idx, int64_t m, int32_t F, float* out, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
     if (m == 0) return GSX_OK;
     GSX_REQUIRE(F >= 1, GSX_ERR_ARG, "records: bad row width %d", F);
     k_gather_rows<<<(int)((m * 32 + 255) / 256), 256, 0, st>>>(rows, idx, m, F, out);
@@ -98,8 +107,9 @@ int records_gather_rows(const float* rows, const int32_t* idx, int64_t m, int F,
     return GSX_OK;
 }
 
-int records_color_rgba8(const float* rows, int64_t n, int F, int c0, int c1, int c2, int cop, float scale, uint8_t* rgba,
-                        cudaStream_t st) {
+int gsx_records_color_rgba8(const float* rows, int64_t n, int32_t F, int32_t c0, int32_t c1, int32_t c2, int32_t cop,
+                            float scale, uint8_t* rgba, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
     if (n == 0) return GSX_OK;
     int rc = check_cols(F, {c0, c1, c2, cop});
     if (rc) return rc;
@@ -108,7 +118,9 @@ int records_color_rgba8(const float* rows, int64_t n, int F, int c0, int c1, int
     return GSX_OK;
 }
 
-int records_scale_exp(const float* rows, int64_t n, int F, int s0, int s1, int s2, float* out, cudaStream_t st) {
+int gsx_records_scale_exp(const float* rows, int64_t n, int32_t F, int32_t s0, int32_t s1, int32_t s2, float* out,
+                          void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
     if (n == 0) return GSX_OK;
     int rc = check_cols(F, {s0, s1, s2});
     if (rc) return rc;
@@ -117,4 +129,4 @@ int records_scale_exp(const float* rows, int64_t n, int F, int s0, int s1, int s
     return GSX_OK;
 }
 
-}  // namespace gsx
+}  // extern "C"

@@ -8,10 +8,11 @@
 // NumPy compares them equal; every NaN, whatever its sign and payload, gets one key above +inf because NumPy sorts
 // NaN last and treats NaNs as equal, so they keep index order).  quantize: lower_bound in the (<= 4096-entry) codebook held in shared memory,
 // clip, then the reference's left-neighbour test |v - cb[left]| < |v - cb[idx]| in float32.
+#include "../../include/gsx.h"
+
 #include "gsx_common.cuh"
 #include "gsx_sh_mask.cuh"
 #include "gsx_radix.cuh"
-#include "gsx_sog.cuh"
 
 namespace gsx {
 
@@ -36,42 +37,6 @@ __global__ void __launch_bounds__(256) k_lex_keys_xy(const float* __restrict__ x
     if (j >= n) return;
     int64_t i = order[j];
     keys[j] = ((uint64_t)float_key(xyz[3 * i]) << 32) | (uint64_t)float_key(xyz[3 * i + 1]);
-}
-
-int64_t lexsort_workspace_bytes(int64_t n) {
-    if (n < 1) n = 1;
-    return (int64_t)(2 * align_up((size_t)n * 8, 256) + 2 * align_up((size_t)n * 4, 256) + radix_ws_bytes(n) + 1024);
-}
-
-int lexsort_zyx(const float* xyz, int64_t n, int32_t* order_out, void* ws, int64_t ws_bytes, cudaStream_t st) {
-    if (n == 0) return GSX_OK;
-    GSX_REQUIRE(n < 2147483584ll, GSX_ERR_ARG, "lexsort: n out of range");
-    GSX_REQUIRE(ws_bytes >= lexsort_workspace_bytes(n), GSX_ERR_WORKSPACE, "lexsort: workspace too small");
-    Carver c(ws, (size_t)ws_bytes);
-    uint64_t* k0 = c.take<uint64_t>((size_t)n);
-    uint64_t* k1 = c.take<uint64_t>((size_t)n);
-    int32_t* v0 = c.take<int32_t>((size_t)n);
-    int32_t* v1 = c.take<int32_t>((size_t)n);
-    char* rws = c.take<char>(radix_ws_bytes(n));
-    int blocks = (int)((n + 255) / 256);
-    k_lex_keys_z<<<blocks, 256, 0, st>>>(xyz, n, k0, v0);
-    GSX_KERNEL_CHECK();
-    uint64_t* ks = nullptr;
-    int32_t* vs = nullptr;
-    int rc = radix_sort_pairs(k0, k1, v0, v1, n, 0, 32, rws, radix_ws_bytes(n), &ks, &vs, st);
-    if (rc) return rc;
-    // second (more significant) key pair, gathered in the current order; reuse the buffer vs does not occupy
-    uint64_t* kin = (ks == k0) ? k0 : k1;  // keys are dead: overwrite the buffer that pairs with vs
-    uint64_t* kalt = (ks == k0) ? k1 : k0;
-    int32_t* valt = (vs == v0) ? v1 : v0;
-    k_lex_keys_xy<<<blocks, 256, 0, st>>>(xyz, vs, n, kin);
-    GSX_KERNEL_CHECK();
-    uint64_t* ks2 = nullptr;
-    int32_t* vs2 = nullptr;
-    rc = radix_sort_pairs(kin, kalt, vs, valt, n, 0, 64, rws, radix_ws_bytes(n), &ks2, &vs2, st);
-    if (rc) return rc;
-    GSX_CUDA_CHECK(cudaMemcpyAsync(order_out, vs2, (size_t)n * 4, cudaMemcpyDeviceToDevice, st));
-    return GSX_OK;
 }
 
 constexpr int kMaxCodebook = 4096;
@@ -102,26 +67,6 @@ __global__ void __launch_bounds__(256) k_quantize_codebook(const float* __restri
     int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride)
         labels[i] = codebook_index(scb, m, vals[i]);
-}
-
-int quantize_to_codebook(const float* vals, int64_t n, const float* codebook_host, int m, uint8_t* labels, void* ws,
-                         int64_t ws_bytes, cudaStream_t st) {
-    if (n == 0) return GSX_OK;
-    GSX_REQUIRE(m >= 1 && m <= kMaxCodebook, GSX_ERR_UNSUPPORTED, "quantize: codebook size must be in [1,%d]",
-                kMaxCodebook);
-    GSX_REQUIRE(ws_bytes >= (int64_t)m * 4, GSX_ERR_WORKSPACE, "quantize: workspace too small");
-    if (m == 1) {  // sog.py:410
-        GSX_CUDA_CHECK(cudaMemsetAsync(labels, 0, (size_t)n, st));
-        return GSX_OK;
-    }
-    GSX_CUDA_CHECK(cudaMemcpyAsync(ws, codebook_host, (size_t)m * 4, cudaMemcpyHostToDevice, st));
-    GSX_CUDA_CHECK(cudaStreamSynchronize(st));  // codebook_host may be a temporary
-    int blocks = sm_count() * 8;
-    int64_t need = (n + 255) / 256;
-    if ((int64_t)blocks > need) blocks = (int)need;
-    k_quantize_codebook<<<blocks, 256, 0, st>>>(vals, n, (const float*)ws, m, labels);
-    GSX_KERNEL_CHECK();
-    return GSX_OK;
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -413,8 +358,73 @@ int load_cols(SogCols* cols, const int32_t* host, int ncols, int F, const char* 
 
 }  // namespace
 
-int sog_means_minmax(const float* rows, int64_t n, int F, const int32_t* cols3_host, float* ws, int64_t ws_bytes,
-                     float* minmax, cudaStream_t st) {
+}  // namespace gsx
+
+using namespace gsx;
+
+extern "C" {
+
+int64_t gsx_lexsort_workspace_bytes(int64_t n) {
+    if (n < 1) n = 1;
+    return (int64_t)(2 * align_up((size_t)n * 8, 256) + 2 * align_up((size_t)n * 4, 256) + radix_ws_bytes(n) + 1024);
+}
+
+int gsx_lexsort_zyx(const float* xyz, int64_t n, int32_t* order_out, void* ws, int64_t ws_bytes, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
+    if (n == 0) return GSX_OK;
+    GSX_REQUIRE(n < 2147483584ll, GSX_ERR_ARG, "lexsort: n out of range");
+    GSX_REQUIRE(ws_bytes >= gsx_lexsort_workspace_bytes(n), GSX_ERR_WORKSPACE, "lexsort: workspace too small");
+    Carver c(ws, (size_t)ws_bytes);
+    uint64_t* k0 = c.take<uint64_t>((size_t)n);
+    uint64_t* k1 = c.take<uint64_t>((size_t)n);
+    int32_t* v0 = c.take<int32_t>((size_t)n);
+    int32_t* v1 = c.take<int32_t>((size_t)n);
+    char* rws = c.take<char>(radix_ws_bytes(n));
+    int blocks = (int)((n + 255) / 256);
+    k_lex_keys_z<<<blocks, 256, 0, st>>>(xyz, n, k0, v0);
+    GSX_KERNEL_CHECK();
+    uint64_t* ks = nullptr;
+    int32_t* vs = nullptr;
+    int rc = radix_sort_pairs(k0, k1, v0, v1, n, 0, 32, rws, radix_ws_bytes(n), &ks, &vs, st);
+    if (rc) return rc;
+    // second (more significant) key pair, gathered in the current order; reuse the buffer vs does not occupy
+    uint64_t* kin = (ks == k0) ? k0 : k1;  // keys are dead: overwrite the buffer that pairs with vs
+    uint64_t* kalt = (ks == k0) ? k1 : k0;
+    int32_t* valt = (vs == v0) ? v1 : v0;
+    k_lex_keys_xy<<<blocks, 256, 0, st>>>(xyz, vs, n, kin);
+    GSX_KERNEL_CHECK();
+    uint64_t* ks2 = nullptr;
+    int32_t* vs2 = nullptr;
+    rc = radix_sort_pairs(kin, kalt, vs, valt, n, 0, 64, rws, radix_ws_bytes(n), &ks2, &vs2, st);
+    if (rc) return rc;
+    GSX_CUDA_CHECK(cudaMemcpyAsync(order_out, vs2, (size_t)n * 4, cudaMemcpyDeviceToDevice, st));
+    return GSX_OK;
+}
+
+int gsx_quantize_to_codebook(const float* vals, int64_t n, const float* codebook_host, int32_t m, uint8_t* labels,
+                             void* ws, int64_t ws_bytes, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
+    if (n == 0) return GSX_OK;
+    GSX_REQUIRE(m >= 1 && m <= kMaxCodebook, GSX_ERR_UNSUPPORTED, "quantize: codebook size must be in [1,%d]",
+                kMaxCodebook);
+    GSX_REQUIRE(ws_bytes >= (int64_t)m * 4, GSX_ERR_WORKSPACE, "quantize: workspace too small");
+    if (m == 1) {  // sog.py:410
+        GSX_CUDA_CHECK(cudaMemsetAsync(labels, 0, (size_t)n, st));
+        return GSX_OK;
+    }
+    GSX_CUDA_CHECK(cudaMemcpyAsync(ws, codebook_host, (size_t)m * 4, cudaMemcpyHostToDevice, st));
+    GSX_CUDA_CHECK(cudaStreamSynchronize(st));  // codebook_host may be a temporary
+    int blocks = sm_count() * 8;
+    int64_t need = (n + 255) / 256;
+    if ((int64_t)blocks > need) blocks = (int)need;
+    k_quantize_codebook<<<blocks, 256, 0, st>>>(vals, n, (const float*)ws, m, labels);
+    GSX_KERNEL_CHECK();
+    return GSX_OK;
+}
+
+int gsx_sog_means_minmax(const float* rows, int64_t n, int32_t F, const int32_t* cols3_host, float* ws,
+                         int64_t ws_bytes, float* minmax, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
     GSX_NVTX("gsx::sog_means_minmax");
     SOG_REQUIRE_N("sog_means_minmax");
     GSX_REQUIRE(n >= 1, GSX_ERR_ARG, "sog_means_minmax: the min and max of no splats are undefined");
@@ -432,8 +442,9 @@ int sog_means_minmax(const float* rows, int64_t n, int F, const int32_t* cols3_h
     return GSX_OK;
 }
 
-int sog_means(const float* rows, int64_t n, int F, const int32_t* order, const int32_t* cols3_host,
-              const float* minmax, int64_t pixels, uint8_t* means_l, uint8_t* means_u, cudaStream_t st) {
+int gsx_sog_means(const float* rows, int64_t n, int32_t F, const int32_t* order, const int32_t* cols3_host,
+                  const float* minmax, int64_t pixels, uint8_t* means_l, uint8_t* means_u, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
     GSX_NVTX("gsx::sog_means");
     SOG_REQUIRE_N("sog_means");
     GSX_REQUIRE(pixels >= n, GSX_ERR_ARG, "sog_means: %lld pixels < n", (long long)pixels);
@@ -450,8 +461,9 @@ int sog_means(const float* rows, int64_t n, int F, const int32_t* order, const i
     return GSX_OK;
 }
 
-int sog_quats(const float* rows, int64_t n, int F, const int32_t* order, const int32_t* cols4_host, int64_t pixels,
-              uint8_t* quats, cudaStream_t st) {
+int gsx_sog_quats(const float* rows, int64_t n, int32_t F, const int32_t* order, const int32_t* cols4_host,
+                  int64_t pixels, uint8_t* quats, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
     GSX_NVTX("gsx::sog_quats");
     SOG_REQUIRE_N("sog_quats");
     GSX_REQUIRE(pixels >= n, GSX_ERR_ARG, "sog_quats: %lld pixels < n", (long long)pixels);
@@ -467,8 +479,9 @@ int sog_quats(const float* rows, int64_t n, int F, const int32_t* order, const i
     return GSX_OK;
 }
 
-int sog_gather_values(const float* rows, int64_t n, int F, const int32_t* order, const int32_t* cols_host, int ncols,
-                      const int64_t* sel, int64_t m, float* out, cudaStream_t st) {
+int gsx_sog_gather_values(const float* rows, int64_t n, int32_t F, const int32_t* order, const int32_t* cols_host,
+                          int32_t ncols, const int64_t* sel, int64_t m, float* out, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
     GSX_NVTX("gsx::sog_gather_values");
     SOG_REQUIRE_N("sog_gather_values");
     GSX_REQUIRE(m >= 0 && (sel != nullptr || m <= n * ncols), GSX_ERR_ARG, "sog_gather_values: m=%lld out of range",
@@ -483,9 +496,10 @@ int sog_gather_values(const float* rows, int64_t n, int F, const int32_t* order,
     return GSX_OK;
 }
 
-int sog_scales_sh0(const float* rows, int64_t n, int F, const int32_t* order, const int32_t* cols7_host,
-                   const float* scale_cb, int m_scale, const float* color_cb, int m_color, int64_t pixels,
-                   uint8_t* scales, uint8_t* sh0, cudaStream_t st) {
+int gsx_sog_scales_sh0(const float* rows, int64_t n, int32_t F, const int32_t* order, const int32_t* cols7_host,
+                       const float* scale_cb, int32_t m_scale, const float* color_cb, int32_t m_color, int64_t pixels,
+                       uint8_t* scales, uint8_t* sh0, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
     GSX_NVTX("gsx::sog_scales_sh0");
     SOG_REQUIRE_N("sog_scales_sh0");
     GSX_REQUIRE(pixels >= n, GSX_ERR_ARG, "sog_scales_sh0: %lld pixels < n", (long long)pixels);
@@ -505,8 +519,9 @@ int sog_scales_sh0(const float* rows, int64_t n, int F, const int32_t* order, co
     return GSX_OK;
 }
 
-int sog_sh_gather(const float* rows, int64_t n, int F, const int32_t* order, const int32_t* cols_host, int ncols,
-                  float* out, unsigned long long* nonzero, cudaStream_t st) {
+int gsx_sog_sh_gather(const float* rows, int64_t n, int32_t F, const int32_t* order, const int32_t* cols_host,
+                      int32_t ncols, float* out, unsigned long long* nonzero, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
     GSX_NVTX("gsx::sog_sh_gather");
     SOG_REQUIRE_N("sog_sh_gather");
     SogCols c{};
@@ -522,8 +537,9 @@ int sog_sh_gather(const float* rows, int64_t n, int F, const int32_t* order, con
     return GSX_OK;
 }
 
-int sog_labels(const int32_t* labels, int64_t n, int64_t chunk_size, int nchunks, const int32_t* offsets_host,
-               const int32_t* passthrough_host, int64_t pixels, uint8_t* out, cudaStream_t st) {
+int gsx_sog_labels(const int32_t* labels, int64_t n, int64_t chunk_size, int32_t nchunks, const int32_t* offsets_host,
+                   const int32_t* passthrough_host, int64_t pixels, uint8_t* out, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
     GSX_NVTX("gsx::sog_labels");
     GSX_REQUIRE(n >= 0 && n < 2147483648ll && pixels >= n, GSX_ERR_ARG, "sog_labels: n=%lld pixels=%lld",
                 (long long)n, (long long)pixels);
@@ -549,8 +565,9 @@ int sog_labels(const int32_t* labels, int64_t n, int64_t chunk_size, int nchunks
     return GSX_OK;
 }
 
-int sog_centroids(const float* palette, int64_t P, int coeffs, const float* cb, int m, int64_t pixels, uint8_t* out,
-                  cudaStream_t st) {
+int gsx_sog_centroids(const float* palette, int64_t P, int32_t coeffs, const float* cb, int32_t m, int64_t pixels,
+                      uint8_t* out, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
     GSX_NVTX("gsx::sog_centroids");
     GSX_REQUIRE(P >= 0 && coeffs >= 3 && coeffs <= kSogMaxCols && coeffs % 3 == 0, GSX_ERR_ARG,
                 "sog_centroids: P=%lld coeffs=%d", (long long)P, coeffs);
@@ -566,4 +583,4 @@ int sog_centroids(const float* palette, int64_t P, int coeffs, const float* cb, 
     return GSX_OK;
 }
 
-}  // namespace gsx
+}  // extern "C"

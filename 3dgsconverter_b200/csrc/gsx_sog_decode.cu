@@ -16,13 +16,21 @@
 // reference rejects with IndexError (a codebook index past the codebook's length, a label >= P) sets a bit of *err;
 // the row gets 0 there and the caller refuses the file.  128 threads per CTA; rows are built in shared memory and
 // stored as 16-byte words (gsx_staged.cuh): SH-3 rows are 248 bytes, not a multiple of 16.
+#include "../../include/gsx.h"
+
 #include "gsx_common.cuh"
-#include "gsx_sog_decode.cuh"
 #include "gsx_staged.cuh"
 
 #include <algorithm>
 
 namespace gsx {
+
+// bits of the error word: the index the reference reader rejects with IndexError
+constexpr int32_t kSogErrScaleCodebook = 1, kSogErrSh0Codebook = 2, kSogErrShCodebook = 4, kSogErrLabel = 8;
+
+struct SogTextures {   // RGBA pixels, 4-byte aligned; labels null without shN
+    const uint8_t *means_l, *means_u, *quats, *scales, *sh0, *labels;
+};
 
 namespace {
 
@@ -111,8 +119,15 @@ __global__ void __launch_bounds__(kRows) k_sog_decode(const SogTextures tx, int6
 
 }  // namespace
 
-int sog_decode_palette(const uint8_t* centroids, int64_t P, int coeffs, const float* codebook, int ncb, float* palette,
-                       int32_t* err, cudaStream_t st) {
+}  // namespace gsx
+
+using namespace gsx;
+
+extern "C" {
+
+int gsx_sog_decode_palette(const uint8_t* centroids, int64_t P, int32_t coeffs, const float* codebook, int32_t ncb,
+                           float* palette, int32_t* err, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
     GSX_REQUIRE(coeffs == 0 || coeffs == 9 || coeffs == 24 || coeffs == 45, GSX_ERR_ARG,
                 "sog_decode_palette: coeffs %d (0, 9, 24 or 45)", coeffs);
     GSX_REQUIRE(P >= 0 && P * coeffs < 2147483648ll, GSX_ERR_UNSUPPORTED,
@@ -128,8 +143,13 @@ int sog_decode_palette(const uint8_t* centroids, int64_t P, int coeffs, const fl
     return GSX_OK;
 }
 
-int sog_decode(const SogTextures& tx, int64_t n, const float* pos_tables, const float* tables, int nscb, int nccb,
-               const float* palette, int64_t P, int coeffs, uint8_t* rows, int32_t* err, cudaStream_t st) {
+int gsx_sog_decode(const uint8_t* const* textures_host, int64_t n, const float* pos_tables, const float* tables,
+                   int32_t nscb, int32_t nccb, const float* palette, int64_t P, int32_t coeffs, uint8_t* rows,
+                   int32_t* err, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
+    GSX_REQUIRE(textures_host, GSX_ERR_ARG, "gsx_sog_decode: no texture table");
+    const SogTextures tx{textures_host[0], textures_host[1], textures_host[2],
+                         textures_host[3], textures_host[4], textures_host[5]};
     GSX_REQUIRE(n >= 0, GSX_ERR_ARG, "sog_decode: n=%lld < 0", (long long)n);
     GSX_REQUIRE(n < 2147483648ll, GSX_ERR_UNSUPPORTED, "sog_decode: n=%lld needs n < 2^31", (long long)n);
     GSX_REQUIRE(coeffs == 0 || coeffs == 9 || coeffs == 24 || coeffs == 45, GSX_ERR_ARG,
@@ -152,4 +172,4 @@ int sog_decode(const SogTextures& tx, int64_t n, const float* pos_tables, const 
     return GSX_OK;
 }
 
-}  // namespace gsx
+}  // extern "C"

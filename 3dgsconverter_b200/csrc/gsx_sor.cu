@@ -28,6 +28,8 @@
 //     probes is scanned twice, int32-wrapping probe hash (GSX_HASH_I32WRAP), self/duplicate
 //     skip by d^2 > 1e-12, K capped at 50, 1e10 "empty" sentinel and the < 0.9e10 validity
 //     test, mean = 0 when no candidate was found.
+#include "../../include/gsx.h"
+
 #include "gsx_common.cuh"
 #include "gsx_sor.cuh"
 
@@ -100,18 +102,6 @@ SorWs sor_carve(void* ws, int64_t ws_bytes, int64_t n, size_t sort_ws_bytes) {
 }
 
 size_t sor_sort_ws_bytes(int64_t n) { return radix_ws_bytes(n) + 256; }  // scratch of the pair sort
-
-int64_t sor_workspace_bytes(int64_t n) {
-    if (n < 1) n = 1;
-    SorWs w = sor_carve(nullptr, 0, n, sor_sort_ws_bytes(n));
-    return (int64_t)w.total + 1024;
-}
-
-int64_t sor_grid_workspace_bytes(int64_t n) {
-    if (n < 1) n = 1;
-    SorWs w = sor_carve(nullptr, 0, n, sor_sort_ws_bytes(n));
-    return (int64_t)w.grid_total;
-}
 
 // ------------------------------------------------------------------ min / max
 
@@ -1343,4 +1333,180 @@ int sor_mean_dists(SorWs& w, int64_t q_begin, int64_t q_end, int q_stride, int q
     return GSX_OK;
 }
 
+// grid-only functions (build_from_sorted, mean_dists) accept the shorter gsx_sor_grid_workspace_bytes blob
+static int carve_grid_checked(void* ws, int64_t ws_bytes, int64_t n, SorWs& w) {
+    GSX_REQUIRE(n >= 1 && n < 2147483584ll, GSX_ERR_ARG, "sor: n=%lld out of range [1, 2^31-64)", (long long)n);
+    GSX_REQUIRE(ws != nullptr, GSX_ERR_WORKSPACE, "sor: null workspace");
+    w = sor_carve(ws, ws_bytes, n, sor_sort_ws_bytes(n));
+    GSX_REQUIRE(w.grid_ok, GSX_ERR_WORKSPACE, "sor: grid workspace too small (%lld < %zu)", (long long)ws_bytes,
+                w.grid_total);
+    return GSX_OK;
+}
+
+static int carve_checked(void* ws, int64_t ws_bytes, int64_t n, SorWs& w) {
+    GSX_REQUIRE(n >= 1 && n < 2147483584ll, GSX_ERR_ARG, "sor: n=%lld out of range [1, 2^31-64)", (long long)n);
+    GSX_REQUIRE(ws != nullptr, GSX_ERR_WORKSPACE, "sor: null workspace");
+    w = sor_carve(ws, ws_bytes, n, sor_sort_ws_bytes(n));
+    GSX_REQUIRE(w.ok, GSX_ERR_WORKSPACE, "sor: workspace too small (%lld < %zu)", (long long)ws_bytes, w.total);
+    return GSX_OK;
+}
+
 }  // namespace gsx
+
+using namespace gsx;
+
+extern "C" {
+
+int64_t gsx_sor_workspace_bytes(int64_t n) {
+    if (n < 1) n = 1;
+    SorWs w = sor_carve(nullptr, 0, n, sor_sort_ws_bytes(n));
+    return (int64_t)w.total + 1024;
+}
+
+int64_t gsx_sor_grid_workspace_bytes(int64_t n) {
+    if (n < 1) n = 1;
+    SorWs w = sor_carve(nullptr, 0, n, sor_sort_ws_bytes(n));
+    return (int64_t)w.grid_total;
+}
+
+
+int gsx_sor_minmax(const float* xyz_dev, int64_t n, float* minmax_dev, void* ws, int64_t ws_bytes, void* stream) {
+    GSX_REQUIRE(n >= 1, GSX_ERR_ARG, "sor: minmax of an empty cloud");
+    GSX_REQUIRE(ws != nullptr && ws_bytes >= 6 * 1024 * (int64_t)sizeof(float), GSX_ERR_WORKSPACE,
+                "sor: minmax needs 24 KiB of scratch");
+    return sor_minmax(xyz_dev, n, minmax_dev, (float*)ws, (cudaStream_t)stream);  // scratch = the head of ws
+}
+
+/* gpu_ops.py:203-213 with NumPy-2 semantics: extent/vol in float32; vol<=0 -> python float 1.0 (then
+ * float64 arithmetic); avg = max(1e-8, vol/N) keeps the float32 unless the python float wins; the
+ * cube root is float32 powf for a float32 base, float64 pow otherwise; floor of 1e-4. */
+float gsx_sor_cell_size(const float* mm, int64_t n) {
+    float ex = mm[3] - mm[0], ey = mm[4] - mm[1], ez = mm[5] - mm[2];
+    float vol = (ex * ey) * ez;
+    double cell;
+    if (vol <= 0.0f || vol != vol) {
+        if (vol != vol) {
+            cell = NAN;
+        } else {
+            double avg = 1.0 / (double)n;
+            if (!(avg > 1e-8)) avg = 1e-8;
+            cell = pow(avg * 32.0, 1.0 / 3.0);
+        }
+    } else {
+        float avgf = vol / (float)n;
+        if ((double)avgf > 1e-8) {  /* python max(1e-8, avgf) returns avgf only if avgf > 1e-8 */
+            float cv = avgf * 32.0f;
+            cell = (double)powf(cv, (float)(1.0 / 3.0));
+        } else {
+            cell = pow(1e-8 * 32.0, 1.0 / 3.0);
+        }
+    }
+    if (!(cell > 1e-4)) cell = 1e-4; /* max(cell_size, 1e-4) */
+    return (float)cell;
+}
+
+int gsx_sor_build(const float* xyz_dev, int64_t n, const float* bmin_host, float cell, void* ws, int64_t ws_bytes,
+                  void* stream) {
+    SorWs w;
+    int rc = carve_checked(ws, ws_bytes, n, w);
+    if (rc) return rc;
+    GSX_REQUIRE(cell > 0.f, GSX_ERR_ARG, "sor: cell size must be > 0");
+    return sor_build(xyz_dev, n, bmin_host, cell, w, (cudaStream_t)stream);
+}
+
+int gsx_sor_dist_local_run(const float* xyz_local_dev, int64_t n_local, int64_t idx_base, int64_t n_global,
+                           int32_t world, const float* bmin_host, float cell, float* pos4_out_dev,
+                           int64_t* cuts_dev, void* ws, int64_t ws_bytes, void* stream) {
+    SorWs w;
+    int rc = carve_checked(ws, ws_bytes, n_local > 0 ? n_local : 1, w);
+    if (rc) return rc;
+    GSX_REQUIRE(n_global >= n_local && n_global >= 1 && n_global < 2147483584ll, GSX_ERR_ARG, "sor: bad n_global");
+    return sor_dist_local_run(xyz_local_dev, n_local, idx_base, n_global, world, bmin_host, cell,
+                              (float4*)pos4_out_dev, (long long*)cuts_dev, w, (cudaStream_t)stream);
+}
+
+int gsx_sor_dist_merge(const float* pos4_dev, int64_t m, int64_t n_global, int64_t bucket_lo, int64_t bucket_hi,
+                       const float* bmin_host, float cell, float* pos4_sorted_dev, uint8_t* flags_sorted_dev, void* ws,
+                       int64_t ws_bytes, void* stream) {
+    if (m == 0) return GSX_OK;
+    SorWs w;
+    int rc = carve_checked(ws, ws_bytes, m, w);
+    if (rc) return rc;
+    return sor_dist_merge((const float4*)pos4_dev, m, n_global, bucket_lo, bucket_hi, bmin_host, cell,
+                          (float4*)pos4_sorted_dev, flags_sorted_dev, w, (cudaStream_t)stream);
+}
+
+int64_t gsx_sor_spos_offset(int64_t n) {
+    if (n < 1) return -1;
+    SorWs w = sor_carve(nullptr, 0, n, sor_sort_ws_bytes(n));
+    return (int64_t)((char*)w.spos - (char*)nullptr);
+}
+
+int gsx_sor_build_from_sorted(const float* spos4_dev, const uint8_t* flags_dev, int64_t n, const float* bmin_host,
+                              float cell, void* ws, int64_t ws_bytes, void* stream) {
+    SorWs w;
+    int rc = carve_grid_checked(ws, ws_bytes, n, w);
+    if (rc) return rc;
+    GSX_REQUIRE(cell > 0.f, GSX_ERR_ARG, "sor: cell size must be > 0");
+    return sor_build_from_sorted((const float4*)spos4_dev, flags_dev, n, bmin_host, cell, w, (cudaStream_t)stream);
+}
+
+int gsx_sor_mean_dists_range(int64_t n, int64_t q_begin, int64_t q_end, int32_t k, int32_t hash_mode,
+                             const float* bmin_host, float cell, void* ws, int64_t ws_bytes, float* final_means_dev,
+                             unsigned long long* stats_dev, void* stream) {
+    SorWs w;
+    int rc = carve_grid_checked(ws, ws_bytes, n, w);
+    if (rc) return rc;
+    return sor_mean_dists(w, q_begin, q_end, 1, 0, k, hash_mode, bmin_host, cell, final_means_dev, stats_dev,
+                          (cudaStream_t)stream);
+}
+
+int gsx_sor_mean_dists_strided(int64_t n, int32_t stride, int32_t phase, int32_t k, int32_t hash_mode,
+                               const float* bmin_host, float cell, void* ws, int64_t ws_bytes, float* final_means_dev,
+                               unsigned long long* stats_dev, void* stream) {
+    SorWs w;
+    int rc = carve_grid_checked(ws, ws_bytes, n, w);
+    if (rc) return rc;
+    return sor_mean_dists(w, 0, n, stride, phase, k, hash_mode, bmin_host, cell, final_means_dev, stats_dev,
+                          (cudaStream_t)stream);
+}
+
+int gsx_sor_mean_dists(int64_t n, int32_t k, int32_t hash_mode, const float* bmin_host, float cell, void* ws,
+                       int64_t ws_bytes, float* final_means_dev, unsigned long long* stats_dev, void* stream) {
+    return gsx_sor_mean_dists_range(n, 0, n, k, hash_mode, bmin_host, cell, ws, ws_bytes, final_means_dev, stats_dev,
+                                    stream);
+}
+
+int gsx_sor_query_counters(int64_t n, void* ws, int64_t ws_bytes, unsigned long long* out8_host, void* stream) {
+    SorWs w;
+    int rc = carve_grid_checked(ws, ws_bytes, n, w);
+    if (rc) return rc;
+    GSX_REQUIRE(out8_host != nullptr, GSX_ERR_ARG, "sor: null counter buffer");
+    GSX_CUDA_CHECK(cudaMemcpyAsync(out8_host, w.stats, 8 * sizeof(unsigned long long), cudaMemcpyDeviceToHost,
+                                   (cudaStream_t)stream));
+    GSX_CUDA_CHECK(cudaStreamSynchronize((cudaStream_t)stream));
+    return GSX_OK;
+}
+
+int gsx_sor_filter_device(const float* xyz_dev, int64_t n, int32_t k, float threshold_factor, int32_t hash_mode,
+                          uint8_t* mask_dev, float* means_dev, void* ws, int64_t ws_bytes, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
+    SorWs w;
+    int rc = carve_checked(ws, ws_bytes, n, w);
+    if (rc) return rc;
+    GSX_REQUIRE(k >= 1, GSX_ERR_ARG, "sor: k must be >= 1 (got %d)", k);
+    if ((rc = sor_minmax(xyz_dev, n, w.minmax, w.partial, st))) return rc;
+    float mm[6];
+    GSX_CUDA_CHECK(cudaMemcpyAsync(mm, w.minmax, sizeof(mm), cudaMemcpyDeviceToHost, st));
+    GSX_CUDA_CHECK(cudaStreamSynchronize(st));
+    float cell = gsx_sor_cell_size(mm, n);
+    GSX_REQUIRE(cell == cell, GSX_ERR_ARG, "sor: non-finite coordinates");
+    if ((rc = sor_build(xyz_dev, n, mm, cell, w, st))) return rc;
+    // the keys buffers are dead after the build: park the means there when the caller wants none
+    float* means = means_dev ? means_dev : reinterpret_cast<float*>(w.keys0);
+    if ((rc = sor_mean_dists(w, 0, n, 1, 0, k, hash_mode, mm, cell, means, nullptr, st))) return rc;
+    if ((rc = mean_std_f32(means, n, w.meanstd, w.ms_ws, w.ms_bytes, st))) return rc;
+    return threshold_mask(means, n, w.meanstd, threshold_factor, mask_dev, st);
+}
+
+}  // extern "C"

@@ -1,4 +1,4 @@
-// gsx_sor.cuh -- internal declarations shared by the SOR translation units and the C ABI.
+// gsx_sor.cuh -- internal declarations shared by the SOR translation units.
 #pragma once
 #include "gsx_common.cuh"
 
@@ -33,8 +33,6 @@ struct SorWs {
 };
 
 SorWs sor_carve(void* ws, int64_t ws_bytes, int64_t n, size_t sort_ws_bytes);
-int64_t sor_workspace_bytes(int64_t n);
-int64_t sor_grid_workspace_bytes(int64_t n);
 size_t sor_sort_ws_bytes(int64_t n);
 int sor_minmax(const float* xyz, int64_t n, float* minmax_dev, float* partial, cudaStream_t st);
 int sor_build(const float* xyz, int64_t n, const float* bmin, float cell, SorWs& w, cudaStream_t st);
@@ -54,10 +52,6 @@ const char* sor_build_info();
 
 size_t mean_std_ws_bytes(int64_t n);
 int mean_std_f32(const float* a, int64_t n, float* out_dev, void* ws, size_t ws_bytes, cudaStream_t st);
-int64_t pairwise_slots(int64_t n);
-int pairwise_leaves_dist(const float* a_local, int64_t base, int64_t n_local, int64_t n, int sq, const float* meanstd,
-                         const float* halo, const long long* bases_dev, int world, float* slot, cudaStream_t st);
-int pairwise_finish(float* slot, int64_t n, int sq, float* meanstd, cudaStream_t st);
 int threshold_mask(const float* a, int64_t n, const float* meanstd_dev, float tf, uint8_t* mask, cudaStream_t st);
 
 }  // namespace gsx

@@ -20,10 +20,11 @@
 // the destination (records of 33 or 65 bytes, planar sections at any offset).  Arithmetic follows NumPy-2 float32
 // semantics on x86-64 (gsx_numpy_scalar.cuh): Python float constants are weak scalars, one __f*_rn operation per NumPy
 // operation in the reference's order.
+#include "../../include/gsx.h"
+
 #include "gsx_common.cuh"
 #include "gsx_numpy_scalar.cuh"
 #include "gsx_sh_mask.cuh"
-#include "gsx_splat_codecs.cuh"
 #include "gsx_staged.cuh"
 
 namespace gsx {
@@ -338,8 +339,15 @@ size_t tile_bytes(int ncol) { return (size_t)kThreads * ncol * 4; }
 
 }  // namespace
 
-int codec_sh_mask(const float* rows, int64_t n, int F, const int32_t* sh_cols, int nsh, unsigned long long* mask,
-                  cudaStream_t st) {
+}  // namespace gsx
+
+using namespace gsx;
+
+extern "C" {
+
+int gsx_codec_sh_mask(const float* rows, int64_t n, int32_t F, const int32_t* sh_cols, int32_t nsh, uint64_t* mask,
+                      void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
     int rc = check_n(n, F, "codec_sh_mask");
     if (rc) return rc;
     GSX_REQUIRE(nsh >= 0 && nsh <= kMaxSh && (nsh == 0 || sh_cols), GSX_ERR_ARG, "codec_sh_mask: %d SH columns", nsh);
@@ -354,17 +362,18 @@ int codec_sh_mask(const float* rows, int64_t n, int F, const int32_t* sh_cols, i
     GSX_CUDA_CHECK(cudaMemsetAsync(mask, 0, sizeof(unsigned long long), st));
     if (n == 0 || nsh == 0) return GSX_OK;
     GSX_REQUIRE(rows, GSX_ERR_ARG, "codec_sh_mask: null rows");
-    k_codec_sh_mask<<<(int)((n + 255) / 256), 256, 0, st>>>(rows, n, F, cols, mask);
+    k_codec_sh_mask<<<(int)((n + 255) / 256), 256, 0, st>>>(rows, n, F, cols, (unsigned long long*)mask);
     GSX_KERNEL_CHECK();
     return GSX_OK;
 }
 
-int ksplat_record_bytes(int level, int sh_count) {
+int32_t gsx_ksplat_record_bytes(int32_t level, int32_t sh_count) {
     if (level < 0 || sh_count < 0) return -1;
     return level == 0 ? 44 + 4 * sh_count : 24 + (level == 1 ? 2 : 1) * sh_count;
 }
 
-int ksplat_centres(const float* lo, const float* hi, int64_t nbucket, float* centres, cudaStream_t st) {
+int gsx_ksplat_centres(const float* lo, const float* hi, int64_t nbucket, float* centres, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
     GSX_REQUIRE(nbucket >= 0, GSX_ERR_ARG, "ksplat_centres: nbucket < 0");
     if (nbucket == 0) return GSX_OK;
     GSX_REQUIRE(lo && hi && centres, GSX_ERR_ARG, "ksplat_centres: null pointer");
@@ -374,8 +383,10 @@ int ksplat_centres(const float* lo, const float* hi, int64_t nbucket, float* cen
     return GSX_OK;
 }
 
-int ksplat_pack(const float* rows, int64_t n, int F, const int32_t* cols14, const int32_t* sh_cols, int sh_count,
-                int level, int64_t bucket_size, float sf_inv, const float* centres, uint8_t* out, cudaStream_t st) {
+int gsx_ksplat_pack(const float* rows, int64_t n, int32_t F, const int32_t* cols14, const int32_t* sh_cols,
+                    int32_t sh_count, int32_t level, int64_t bucket_size, float sf_inv, const float* centres,
+                    uint8_t* out, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
     int rc = check_n(n, F, "ksplat_pack");
     if (rc) return rc;
     GSX_REQUIRE(level >= 0 && level <= 65535, GSX_ERR_ARG, "ksplat_pack: level %d", level);
@@ -386,7 +397,7 @@ int ksplat_pack(const float* rows, int64_t n, int F, const int32_t* cols14, cons
     if ((rc = fill_cols(cols14, sh_cols, sh_count, F, cols, "ksplat_pack"))) return rc;
     GSX_REQUIRE(rows && out && (level == 0 || centres), GSX_ERR_ARG, "ksplat_pack: null device pointer");
     const int lv = level < 3 ? level : 3;
-    const int rec = ksplat_record_bytes(lv, sh_count);
+    const int rec = gsx_ksplat_record_bytes(lv, sh_count);
     const size_t smem = tile_bytes(cols.ncol) + (size_t)kThreads * rec + 16;
     k_ksplat_pack<<<(int)((n + kThreads - 1) / kThreads), kThreads, smem, st>>>(rows, n, F, cols, lv, bucket_size, sf_inv,
                                                                                  centres, rec, out);
@@ -394,8 +405,9 @@ int ksplat_pack(const float* rows, int64_t n, int F, const int32_t* cols14, cons
     return GSX_OK;
 }
 
-int spz_pack(const float* rows, int64_t n, int F, const int32_t* cols14, const int32_t* sh_cols, int sh_dim,
-             uint8_t* body, cudaStream_t st) {
+int gsx_spz_pack(const float* rows, int64_t n, int32_t F, const int32_t* cols14, const int32_t* sh_cols, int32_t sh_dim,
+                 uint8_t* body, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
     int rc = check_n(n, F, "spz_pack");
     if (rc) return rc;
     GSX_REQUIRE(sh_dim == 0 || sh_dim == 3 || sh_dim == 8 || sh_dim == 15, GSX_ERR_ARG, "spz_pack: sh_dim %d", sh_dim);
@@ -409,8 +421,9 @@ int spz_pack(const float* rows, int64_t n, int F, const int32_t* cols14, const i
     return GSX_OK;
 }
 
-int splat_sort_keys(const float* rows, int64_t n, int F, const int32_t* cols4, uint64_t* keys, int32_t* vals,
-                    cudaStream_t st) {
+int gsx_splat_sort_keys(const float* rows, int64_t n, int32_t F, const int32_t* cols4, uint64_t* keys, int32_t* vals,
+                        void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
     int rc = check_n(n, F, "splat_sort_keys");
     if (rc) return rc;
     GSX_REQUIRE(cols4, GSX_ERR_ARG, "splat_sort_keys: no column table");
@@ -425,8 +438,9 @@ int splat_sort_keys(const float* rows, int64_t n, int F, const int32_t* cols4, u
     return GSX_OK;
 }
 
-int splat_pack(const float* rows, int64_t n, int F, const int32_t* order, const int32_t* cols14, uint8_t* out,
-               cudaStream_t st) {
+int gsx_splat_pack(const float* rows, int64_t n, int32_t F, const int32_t* order, const int32_t* cols14, uint8_t* out,
+                   void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
     int rc = check_n(n, F, "splat_pack");
     if (rc) return rc;
     if (n == 0) return GSX_OK;
@@ -439,8 +453,9 @@ int splat_pack(const float* rows, int64_t n, int F, const int32_t* order, const 
     return GSX_OK;
 }
 
-int records_from_bytes(const uint8_t* src, int64_t n, int64_t row_bytes, const int32_t* offsets, int nf, float* out,
-                       cudaStream_t st) {
+int gsx_records_from_bytes(const uint8_t* src, int64_t n, int64_t row_bytes, const int32_t* offsets, int32_t nf,
+                           float* out, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
     GSX_REQUIRE(n >= 0 && row_bytes >= 1, GSX_ERR_ARG, "records_from_bytes: bad sizes");
     GSX_REQUIRE(nf >= 1 && nf <= 256 && offsets, GSX_ERR_ARG, "records_from_bytes: %d fields (1..256)", nf);
     ByteFields f{};
@@ -458,4 +473,4 @@ int records_from_bytes(const uint8_t* src, int64_t n, int64_t row_bytes, const i
     return GSX_OK;
 }
 
-}  // namespace gsx
+}  // extern "C"

@@ -8,6 +8,8 @@
 // The split tree depends only on n, so it parallelises exactly: one thread per leaf block walks the
 // tree from the root along the bits of its slot index, sums its <=128 elements in NumPy's order, and
 // the inner nodes are then combined bottom-up in place (left + right, one float add per node).
+#include "../../include/gsx.h"
+
 #include "gsx_common.cuh"
 #include "gsx_sor.cuh"
 
@@ -299,36 +301,6 @@ __global__ void __launch_bounds__(128)
     if (j == 0) slot[t] = res;
 }
 
-int64_t pairwise_slots(int64_t n) {
-    if (n < 1) n = 1;
-    return (int64_t)1 << pairwise_depth(n);
-}
-
-int pairwise_leaves_dist(const float* a_local, int64_t base, int64_t n_local, int64_t n, int sq, const float* meanstd,
-                         const float* halo, const long long* bases_dev, int world, float* slot, cudaStream_t st) {
-    GSX_REQUIRE(n >= 1 && n_local >= 0 && base >= 0 && base + n_local <= n, GSX_ERR_ARG, "pairwise_dist: bad slab");
-    int dmax = pairwise_depth(n);
-    GSX_REQUIRE(dmax <= 31, GSX_ERR_UNSUPPORTED, "pairwise_dist: n too large");
-    uint32_t leaves = 1u << dmax;
-    GSX_CUDA_CHECK(cudaMemsetAsync(slot, 0, (size_t)leaves * sizeof(float), st));
-    if (n_local == 0) return GSX_OK;
-    const unsigned lb = (unsigned)(((uint64_t)leaves * 8 + 127) / 128);
-    if (sq) k_pw_leaves_dist<true><<<lb, 128, 0, st>>>(a_local, base, n_local, n, dmax, meanstd, halo, bases_dev, world, slot);
-    else k_pw_leaves_dist<false><<<lb, 128, 0, st>>>(a_local, base, n_local, n, dmax, meanstd, halo, bases_dev, world, slot);
-    GSX_KERNEL_CHECK();
-    return GSX_OK;
-}
-
-int pairwise_finish(float* slot, int64_t n, int sq, float* meanstd, cudaStream_t st) {
-    int dmax = pairwise_depth(n);
-    const int d = pairwise_mid_levels(n, dmax, slot, st);
-    GSX_KERNEL_CHECK();
-    if (sq) k_pw_top<true><<<1, 1024, 0, st>>>(n, dmax, d, slot, meanstd);
-    else k_pw_top<false><<<1, 1024, 0, st>>>(n, dmax, d, slot, meanstd);
-    GSX_KERNEL_CHECK();
-    return GSX_OK;
-}
-
 // gpu_ops.py:261-263: thresh = mean + f32(tf) * std (float32 mul then add), mask = a < thresh
 __global__ void __launch_bounds__(256) k_threshold_mask(const float* __restrict__ a, int64_t n,
                                                         const float* __restrict__ ms, float tf,
@@ -365,3 +337,58 @@ int threshold_mask(const float* a, int64_t n, const float* meanstd_dev, float tf
 }
 
 }  // namespace gsx
+
+using namespace gsx;
+
+extern "C" {
+
+int64_t gsx_pairwise_slots(int64_t n) {
+    if (n < 1) n = 1;
+    return (int64_t)1 << pairwise_depth(n);
+}
+
+int gsx_pairwise_leaves_dist(const float* a_local, int64_t base, int64_t n_local, int64_t n, int32_t sq,
+                             const float* meanstd, const float* halo, const int64_t* bases_dev, int32_t world,
+                             float* slot, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
+    GSX_REQUIRE(n >= 1 && n_local >= 0 && base >= 0 && base + n_local <= n, GSX_ERR_ARG, "pairwise_dist: bad slab");
+    int dmax = pairwise_depth(n);
+    GSX_REQUIRE(dmax <= 31, GSX_ERR_UNSUPPORTED, "pairwise_dist: n too large");
+    uint32_t leaves = 1u << dmax;
+    GSX_CUDA_CHECK(cudaMemsetAsync(slot, 0, (size_t)leaves * sizeof(float), st));
+    if (n_local == 0) return GSX_OK;
+    const unsigned lb = (unsigned)(((uint64_t)leaves * 8 + 127) / 128);
+    if (sq)
+        k_pw_leaves_dist<true><<<lb, 128, 0, st>>>(a_local, base, n_local, n, dmax, meanstd, halo,
+                                                   (const long long*)bases_dev, world, slot);
+    else
+        k_pw_leaves_dist<false><<<lb, 128, 0, st>>>(a_local, base, n_local, n, dmax, meanstd, halo,
+                                                    (const long long*)bases_dev, world, slot);
+    GSX_KERNEL_CHECK();
+    return GSX_OK;
+}
+
+int gsx_pairwise_finish(float* slot, int64_t n, int32_t sq, float* meanstd, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
+    GSX_REQUIRE(n >= 1, GSX_ERR_ARG, "pairwise_finish: n must be >= 1");
+    int dmax = pairwise_depth(n);
+    const int d = pairwise_mid_levels(n, dmax, slot, st);
+    GSX_KERNEL_CHECK();
+    if (sq) k_pw_top<true><<<1, 1024, 0, st>>>(n, dmax, d, slot, meanstd);
+    else k_pw_top<false><<<1, 1024, 0, st>>>(n, dmax, d, slot, meanstd);
+    GSX_KERNEL_CHECK();
+    return GSX_OK;
+}
+
+int64_t gsx_mean_std_workspace_bytes(int64_t n) { return (int64_t)mean_std_ws_bytes(n); }
+
+int gsx_mean_std_f32(const float* a_dev, int64_t n, float* out_dev, void* ws, int64_t ws_bytes, void* stream) {
+    return mean_std_f32(a_dev, n, out_dev, ws, (size_t)ws_bytes, (cudaStream_t)stream);
+}
+
+int gsx_threshold_mask(const float* a_dev, int64_t n, const float* meanstd_dev, float threshold_factor,
+                       uint8_t* mask_dev, void* stream) {
+    return threshold_mask(a_dev, n, meanstd_dev, threshold_factor, mask_dev, (cudaStream_t)stream);
+}
+
+}  // extern "C"

@@ -14,12 +14,18 @@
 //   k_webp_bases       the 64-bit base of each scanned chunk and the image's total
 //   k_webp_emit        the LSB-first fields of every token ORed into a zeroed word buffer (a token straddles up to
 //                      three 32-bit words)
+#include "../../include/gsx.h"
+
+#include "gsx_common.cuh"
 #include "gsx_radix.cuh"
-#include "gsx_webp.cuh"
 
 #include <algorithm>
 
 namespace gsx {
+
+constexpr int kWebpMaxSide = 16384;
+constexpr int kWebpTreeSyms = 280 + 256 + 256 + 256 + 40;   // green + 24 lengths, red, blue, alpha, distance
+
 namespace {
 
 constexpr int kTile = 16;
@@ -361,7 +367,13 @@ int tokens_of(const uint32_t* sym, int64_t n, uint16_t* tok, uint32_t* hist, con
 
 }  // namespace
 
-int64_t webp_workspace_bytes(int64_t width, int64_t height) {
+}  // namespace gsx
+
+using namespace gsx;
+
+extern "C" {
+
+int64_t gsx_webp_workspace_bytes(int64_t width, int64_t height) {
     if (!side_ok(width, height)) return 0;
     Carver cv(nullptr, 0);
     Layout L;
@@ -369,8 +381,9 @@ int64_t webp_workspace_bytes(int64_t width, int64_t height) {
     return int64_t(cv.off) + 256;
 }
 
-int webp_analyze(const uint8_t* rgba, int64_t width, int64_t height, void* ws, int64_t ws_bytes, uint32_t* hist,
-                 uint8_t* modes, cudaStream_t st) {
+int gsx_webp_analyze(const uint8_t* rgba, int64_t width, int64_t height, void* ws, int64_t ws_bytes, uint32_t* hist,
+                     uint8_t* modes, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
     GSX_NVTX("gsx_webp_analyze");
     GSX_REQUIRE(side_ok(width, height), GSX_ERR_ARG, "webp: width and height must be 1..16384 (got %lld x %lld)",
                 (long long)width, (long long)height);
@@ -398,8 +411,9 @@ int webp_analyze(const uint8_t* rgba, int64_t width, int64_t height, void* ws, i
     return GSX_OK;
 }
 
-int webp_emit(int64_t width, int64_t height, int image, const uint32_t* table, uint64_t bit_offset, void* ws,
-              int64_t ws_bytes, uint32_t* words, int64_t nwords, unsigned long long* total_bits, cudaStream_t st) {
+int gsx_webp_emit(int64_t width, int64_t height, int32_t image, const uint32_t* table, uint64_t bit_offset, void* ws,
+                  int64_t ws_bytes, uint32_t* words, int64_t nwords, unsigned long long* total_bits, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
     GSX_NVTX("gsx_webp_emit");
     GSX_REQUIRE(side_ok(width, height), GSX_ERR_ARG, "webp: width and height must be 1..16384 (got %lld x %lld)",
                 (long long)width, (long long)height);
@@ -425,7 +439,8 @@ int webp_emit(int64_t width, int64_t height, int image, const uint32_t* table, u
     return GSX_OK;
 }
 
-int webp_patch(uint32_t* words, int64_t nwords, const uint32_t* patches, int64_t npatches, cudaStream_t st) {
+int gsx_webp_patch(uint32_t* words, int64_t nwords, const uint32_t* patches, int64_t npatches, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
     GSX_REQUIRE(words && (patches || npatches == 0) && npatches >= 0, GSX_ERR_ARG, "webp_patch: bad arguments");
     if (npatches == 0) return GSX_OK;
     k_webp_patch<<<grid_for(npatches), 256, 0, st>>>(words, nwords, patches, npatches);
@@ -433,4 +448,4 @@ int webp_patch(uint32_t* words, int64_t nwords, const uint32_t* patches, int64_t
     return GSX_OK;
 }
 
-}  // namespace gsx
+}  // extern "C"

@@ -1,13 +1,18 @@
-"""ctypes binding of libgsx.so (include/gsx.h).  No torch types cross this boundary.
+"""ctypes binding of libgsx.so, derived from include/gsx.h.  No torch types cross this boundary.
 
 The library is built in-tree by ``__graft_entry__.build()`` (3dgsconverter_b200/lib/libgsx.so).
-There is NO CPU fallback: if the shared object is missing this module raises at import.
+There is NO CPU fallback: if the shared object or the header is missing this module raises at import.
+Every ``gsx_*`` prototype of the header becomes one ctypes signature: pointers are ``c_void_p`` (a
+``const char*`` return is ``c_char_p``), scalars map through ``_SCALARS``; any other type is an ImportError.
 """
 from __future__ import annotations
 
 import ctypes as C
 import os
+import re
 from pathlib import Path
+
+import torch
 
 _PKG = Path(__file__).resolve().parent.parent
 LIB_PATH = Path(os.environ.get("GSX_LIB", _PKG / "lib" / "libgsx.so"))
@@ -24,119 +29,36 @@ if not LIB_PATH.exists():
 
 lib = C.CDLL(str(LIB_PATH))
 
-_f32p = C.POINTER(C.c_float)
-_vp = C.c_void_p
-_i64 = C.c_int64
-_i32 = C.c_int32
+_HEADER = _PKG.parent / "include" / "gsx.h"
+_SCALARS = {"int": C.c_int32, "int32_t": C.c_int32, "int64_t": C.c_int64, "long long": C.c_int64,
+            "uint64_t": C.c_uint64, "float": C.c_float, "double": C.c_double, "void": None}
 
-_SIGS = {
-    "gsx_last_error": (C.c_char_p, []),
-    "gsx_version": (C.c_int, []),
-    "gsx_build_info": (C.c_char_p, []),
-    "gsx_device_sm_count": (C.c_int, []),
-    "gsx_kernel_launches": (C.c_longlong, []),
-    "gsx_sor_workspace_bytes": (_i64, [_i64]),
-    "gsx_sor_grid_workspace_bytes": (_i64, [_i64]),
-    "gsx_sor_minmax": (C.c_int, [_vp, _i64, _vp, _vp, _i64, _vp]),
-    "gsx_sor_cell_size": (C.c_float, [_f32p, _i64]),
-    "gsx_sor_build": (C.c_int, [_vp, _i64, _f32p, C.c_float, _vp, _i64, _vp]),
-    "gsx_sor_dist_local_run": (C.c_int, [_vp, _i64, _i64, _i64, _i32, _f32p, C.c_float, _vp, _vp, _vp, _i64, _vp]),
-    "gsx_sor_dist_merge": (C.c_int, [_vp, _i64, _i64, _i64, _i64, _f32p, C.c_float, _vp, _vp, _vp, _i64, _vp]),
-    "gsx_sor_spos_offset": (_i64, [_i64]),
-    "gsx_sor_build_from_sorted": (C.c_int, [_vp, _vp, _i64, _f32p, C.c_float, _vp, _i64, _vp]),
-    "gsx_sor_mean_dists": (C.c_int, [_i64, _i32, _i32, _f32p, C.c_float, _vp, _i64, _vp, _vp, _vp]),
-    "gsx_sor_mean_dists_range": (C.c_int, [_i64, _i64, _i64, _i32, _i32, _f32p, C.c_float, _vp, _i64, _vp, _vp, _vp]),
-    "gsx_sor_mean_dists_strided": (C.c_int, [_i64, _i32, _i32, _i32, _i32, _f32p, C.c_float, _vp, _i64, _vp, _vp, _vp]),
-    "gsx_sor_query_counters": (C.c_int, [_i64, _vp, _i64, _vp, _vp]),
-    "gsx_sort_pairs_workspace_bytes": (_i64, [_i64]),
-    "gsx_sort_pairs": (C.c_int, [_vp, _vp, _i64, _i32, _i32, _vp, _i64, _vp]),
-    "gsx_mean_std_workspace_bytes": (_i64, [_i64]),
-    "gsx_mean_std_f32": (C.c_int, [_vp, _i64, _vp, _vp, _i64, _vp]),
-    "gsx_pairwise_slots": (_i64, [_i64]),
-    "gsx_pairwise_leaves_dist": (C.c_int, [_vp, _i64, _i64, _i64, _i32, _vp, _vp, _vp, _i32, _vp, _vp]),
-    "gsx_pairwise_finish": (C.c_int, [_vp, _i64, _i32, _vp, _vp]),
-    "gsx_threshold_mask": (C.c_int, [_vp, _i64, _vp, C.c_float, _vp, _vp]),
-    "gsx_sor_filter_device": (C.c_int, [_vp, _i64, _i32, C.c_float, _i32, _vp, _vp, _vp, _i64, _vp]),
-    "gsx_sor_filter_host": (C.c_int, [_vp, _i64, _i32, C.c_float, _i32, _vp, _vp]),
-    "gsx_knn_exact_workspace_bytes": (_i64, [_i64]),
-    "gsx_knn_exact_mean_dists": (C.c_int, [_vp, _i64, _i32, _vp, _vp, _i64, _vp]),
-    "gsx_sor_ckdtree_filter_host": (C.c_int, [_vp, _i64, _i32, C.c_float, _vp, _vp]),
-    "gsx_bbox_mask": (C.c_int, [_vp, _i64, _f32p, _vp, _vp]),
-    "gsx_alpha_mask": (C.c_int, [_vp, _i64, C.c_double, _vp, _vp]),
-    "gsx_alpha_logit_threshold": (C.c_double, [C.c_double]),
-    "gsx_compact_workspace_bytes": (_i64, [_i64]),
-    "gsx_compact_points": (C.c_int, [_vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, C.POINTER(_i64), _vp, _i64, _vp]),
-    "gsx_density_workspace_bytes": (_i64, [_i64, _i64]),
-    "gsx_density_voxel_count": (C.c_int, [_vp, _i64, C.c_float, _i64, _vp, _vp, _i64, C.POINTER(_i64),
-                                          C.POINTER(_i64), _vp, _i64, _vp]),
-    "gsx_density_member_mask": (C.c_int, [_vp, _i64, C.c_float, _vp, _i64, _vp, _vp, _i64, _vp]),
-    "gsx_density_voxel_range": (None, [_f32p, C.c_float, C.POINTER(_i64), C.POINTER(_i64)]),
-    "gsx_density_grid_count": (C.c_int, [_vp, _i64, C.c_float, C.POINTER(_i64), C.POINTER(_i64), _vp, _vp, _vp]),
-    "gsx_density_grid_dense": (C.c_int, [_vp, C.POINTER(_i64), C.POINTER(_i64), _i64, _vp, _vp, _i64,
-                                         C.POINTER(_i64), C.POINTER(_i64), _vp, _i64, _vp]),
-    "gsx_lexsort_workspace_bytes": (_i64, [_i64]),
-    "gsx_lexsort_zyx": (C.c_int, [_vp, _i64, _vp, _vp, _i64, _vp]),
-    "gsx_quantize_to_codebook": (C.c_int, [_vp, _i64, _f32p, _i32, _vp, _vp, _i64, _vp]),
-    "gsx_sog_means_minmax": (C.c_int, [_vp, _i64, _i32, C.POINTER(_i32), _vp, _i64, _vp, _vp]),
-    "gsx_sog_means": (C.c_int, [_vp, _i64, _i32, _vp, C.POINTER(_i32), _vp, _i64, _vp, _vp, _vp]),
-    "gsx_sog_quats": (C.c_int, [_vp, _i64, _i32, _vp, C.POINTER(_i32), _i64, _vp, _vp]),
-    "gsx_sog_gather_values": (C.c_int, [_vp, _i64, _i32, _vp, C.POINTER(_i32), _i32, _vp, _i64, _vp, _vp]),
-    "gsx_sog_scales_sh0": (C.c_int, [_vp, _i64, _i32, _vp, C.POINTER(_i32), _vp, _i32, _vp, _i32, _i64, _vp, _vp,
-                                     _vp]),
-    "gsx_sog_sh_gather": (C.c_int, [_vp, _i64, _i32, _vp, C.POINTER(_i32), _i32, _vp, _vp, _vp]),
-    "gsx_sog_labels": (C.c_int, [_vp, _i64, _i64, _i32, C.POINTER(_i32), C.POINTER(_i32), _i64, _vp, _vp]),
-    "gsx_sog_centroids": (C.c_int, [_vp, _i64, _i32, _vp, _i32, _i64, _vp, _vp]),
-    "gsx_kmeans_workspace_bytes": (_i64, [_i64, _i32, _i32, _i32]),
-    "gsx_kmeans_lloyd_device": (C.c_int, [_vp, C.POINTER(_i64), _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _i64,
-                                          _i32, _vp, _vp]),
-    "gsx_kmeans_tensor_core_supported": (_i32, [_i32, _i32]),
-    "gsx_kmeans_tc_debug_scores": (C.c_int, [_vp, _i64, _vp, _i32, _i32, _vp, _vp, _i64, _vp]),
-    "gsx_kmeans_host": (C.c_int, [_vp, _i64, _i32, _i32, _i32, _vp, _vp, _i32]),
-    "gsx_kmeans_host_batched": (C.c_int, [_vp, C.POINTER(_i64), _i32, _i32, _i32, _i32, _vp, _vp, _i32]),
-    "gsx_records_extract_xyz_opacity": (C.c_int, [_vp, _i64, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _vp]),
-    "gsx_records_gather_rows": (C.c_int, [_vp, _vp, _i64, _i32, _vp, _vp]),
-    "gsx_records_color_rgba8": (C.c_int, [_vp, _i64, _i32, _i32, _i32, _i32, _i32, C.c_float, _vp, _vp]),
-    "gsx_records_scale_exp": (C.c_int, [_vp, _i64, _i32, _i32, _i32, _i32, _vp, _vp]),
-    "gsx_morton_workspace_bytes": (_i64, [_i64]),
-    "gsx_morton_order": (C.c_int, [_vp, _i64, _vp, _i32, C.POINTER(_i32), _vp, _i64, _vp]),
-    "gsx_chunk_minmax": (C.c_int, [_vp, _i64, _i32, _vp, _i32, C.POINTER(_i32), _i32, C.c_float, C.c_float, _vp, _vp, _vp,
-                                   _i64, _vp]),
-    "gsx_cply_pack": (C.c_int, [_vp, _i64, _i32, _vp, C.POINTER(_i32), C.POINTER(_i32), _i32, _vp, _vp, _vp, _vp, _vp, _vp,
-                                _vp, _vp, _vp]),
-    "gsx_cply_narrow_sh": (C.c_int, [_vp, _i64, _i32, _i32, _vp, _vp]),
-    "gsx_codec_sh_mask": (C.c_int, [_vp, _i64, _i32, C.POINTER(_i32), _i32, _vp, _vp]),
-    "gsx_ksplat_record_bytes": (_i32, [_i32, _i32]),
-    "gsx_ksplat_centres": (C.c_int, [_vp, _vp, _i64, _vp, _vp]),
-    "gsx_ksplat_pack": (C.c_int, [_vp, _i64, _i32, C.POINTER(_i32), C.POINTER(_i32), _i32, _i32, _i64, C.c_float, _vp,
-                                  _vp, _vp]),
-    "gsx_spz_pack": (C.c_int, [_vp, _i64, _i32, C.POINTER(_i32), C.POINTER(_i32), _i32, _vp, _vp]),
-    "gsx_splat_sort_keys": (C.c_int, [_vp, _i64, _i32, C.POINTER(_i32), _vp, _vp, _vp]),
-    "gsx_splat_pack": (C.c_int, [_vp, _i64, _i32, _vp, C.POINTER(_i32), _vp, _vp]),
-    "gsx_records_from_bytes": (C.c_int, [_vp, _i64, _i64, C.POINTER(_i32), _i32, _vp, _vp]),
-    "gsx_splat_decode": (C.c_int, [_vp, _i64, _vp, _vp, _vp]),
-    "gsx_ksplat_decode_section": (C.c_int, [_vp, _i64, _i32, _i32, C.c_float, C.c_float, _vp, _i64, _i64, _i64, _vp, _i32,
-                                            _vp, _i32, _vp, _vp]),
-    "gsx_spz_decode": (C.c_int, [_vp, _i64, _i32, _i32, _i32, _vp, _i32, _vp, _vp]),
-    "gsx_cply_decode": (C.c_int, [_vp, _i64, _i32, C.POINTER(_i32), _vp, _i64, _i32, C.POINTER(_i32), _vp, _i32,
-                                  C.POINTER(_i32), _i32, _vp, _vp, _vp]),
-    "gsx_ply_transcode": (C.c_int, [_vp, _i64, _i32, _vp, _i32, C.POINTER(_i32), _i32, _vp]),
-    "gsx_sog_decode_palette":(C.c_int, [_vp, _i64, _i32, _vp, _i32, _vp, _vp, _vp]),
-    "gsx_sog_decode": (C.c_int, [C.POINTER(_vp), _i64, _vp, _vp, _i32, _i32, _vp, _i64, _i32, _vp, _vp, _vp]),
-    "gsx_webp_workspace_bytes": (_i64, [_i64, _i64]),
-    "gsx_webp_analyze": (C.c_int, [_vp, _i64, _i64, _vp, _i64, _vp, _vp, _vp]),
-    "gsx_webp_emit": (C.c_int, [_i64, _i64, _i32, _vp, C.c_uint64, _vp, _i64, _vp, _i64, _vp, _vp]),
-    "gsx_webp_patch": (C.c_int, [_vp, _i64, _vp, _i64, _vp]),
-    "gsx_deflate_workspace_bytes": (_i64, [_i64]),
-    "gsx_crc32": (C.c_int, [_vp, _i64, _vp, _i64, _vp, _vp]),
-    "gsx_deflate_stored": (C.c_int, [_vp, _i64, _vp, _vp]),
-    "gsx_deflate_plan": (C.c_int, [_vp, _i64, _vp, _i64, _vp, _i64, C.c_uint64, _vp, _vp]),
-    "gsx_deflate_emit": (C.c_int, [_vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64, _vp, _vp]),
-    "gsx_copy_h2d": (C.c_int, [_vp, _vp, _i64, _vp]),
-    "gsx_copy_d2h": (C.c_int, [_vp, _vp, _i64, _vp]),
-    "gsx_host_gather_rows": (C.c_int, [_vp, _i64, _i64, _vp, _i64, _vp]),
-    "gsx_host_extract_xyz_opacity": (C.c_int, [_vp, _i64, _i64, _i64, _i64, _i64, _i64, _vp, _vp]),
-    "gsx_device_memory": (C.c_int, [C.POINTER(_i64), C.POINTER(_i64)]),
-}
+
+def _ctype(decl: str, proto: str, ret: bool = False):
+    """ctypes type of a return type, or of a parameter declaration (type and name)."""
+    if "*" in decl:
+        return C.c_char_p if ret and decl.split() == ["const", "char*"] else C.c_void_p
+    words = [w for w in decl.split() if w != "const"]
+    t = " ".join(words if ret else words[:-1])
+    if t not in _SCALARS:
+        raise ImportError(f"include/gsx.h: no ctypes type for '{decl.strip()}' in {proto}")
+    return _SCALARS[t]
+
+
+def _signatures(header: Path) -> dict:
+    """{name: (restype, argtypes)} of every gsx_* prototype of include/gsx.h."""
+    if not header.exists():
+        raise ImportError(f"{header} not found: gsx binds libgsx.so from its header")
+    src = re.sub(r"/\*.*?\*/", " ", header.read_text(), flags=re.S)
+    src = re.sub(r"^\s*#.*$", "", src, flags=re.M)
+    sigs = {}
+    for ret, name, args in re.findall(r"([A-Za-z_][\w\s]*?\**)\s*\b(gsx_\w+)\s*\(([^)]*)\)\s*;", src):
+        params = [a for a in args.split(",") if a.strip() and a.strip() != "void"]
+        sigs[name] = (_ctype(ret, name, ret=True), [_ctype(a, name) for a in params])
+    return sigs
+
+
+_SIGS = _signatures(_HEADER)
 
 for _name, (_res, _args) in _SIGS.items():
     _fn = getattr(lib, _name)  # AttributeError here == a symbol declared in gsx.h is missing
@@ -155,3 +77,13 @@ def check(rc: int, what: str = ""):
 
 def f32x(*vals):
     return (C.c_float * len(vals))(*[float(v) for v in vals])
+
+
+def _stream():
+    """The current torch CUDA stream, as the ``void* stream`` of an entry point."""
+    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
+
+
+def _ptr(t):
+    """A tensor's data pointer (NULL for None)."""
+    return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)

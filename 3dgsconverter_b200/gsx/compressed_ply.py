@@ -17,7 +17,7 @@ import numpy as np
 import torch
 
 from ._abi import lib, check
-from .sor import _ptr, _stream
+from ._abi import _ptr, _stream
 
 CHUNK = 256
 PACK_FIELDS = ("x", "y", "z", "f_dc_0", "f_dc_1", "f_dc_2", "opacity", "scale_0", "scale_1", "scale_2",

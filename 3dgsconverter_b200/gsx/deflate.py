@@ -18,7 +18,7 @@ import numpy as np
 import torch
 
 from ._abi import lib, check
-from .sor import _ptr, _stream
+from ._abi import _ptr, _stream
 
 BLOCK = 1 << 20
 STORED_BLOCK = 65535

@@ -13,7 +13,8 @@ import numpy as np
 import torch
 
 from ._abi import lib, check
-from .sor import _ptr, _stream, _check_xyz
+from ._abi import _ptr, _stream
+from .sor import _check_xyz
 
 
 def slider(sensitivity: float):

@@ -9,7 +9,7 @@ import numpy as np
 import torch
 
 from ._abi import lib, check
-from .sor import _ptr, _stream
+from ._abi import _ptr, _stream
 
 _NP2T = {np.dtype(np.float32): torch.float32, np.dtype(np.float64): torch.float64, np.dtype(np.int32): torch.int32,
          np.dtype(np.int64): torch.int64, np.dtype(np.uint8): torch.uint8, np.dtype(np.bool_): torch.bool}

@@ -7,7 +7,7 @@ import numpy as np
 import torch
 
 from ._abi import lib, check, KM_ASSIGN
-from .sor import _ptr, _stream
+from ._abi import _ptr, _stream
 
 
 def tensor_core_supported(K: int, D: int) -> bool:

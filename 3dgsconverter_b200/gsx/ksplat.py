@@ -20,7 +20,7 @@ import torch
 from . import readers
 from ._abi import lib, check
 from .compressed_ply import PACK_FIELDS
-from .sor import _ptr, _stream
+from ._abi import _ptr, _stream
 
 HEADER_SIZE, SECTION_HEADER_SIZE = 4096, 1024
 MAGIC_MAJOR, MAGIC_MINOR = 0, 1

@@ -7,7 +7,8 @@ import numpy as np
 import torch
 
 from ._abi import lib, check, f32x
-from .sor import _ptr, _stream, _check_xyz
+from ._abi import _ptr, _stream
+from .sor import _check_xyz
 
 
 def bbox_mask(xyz: torch.Tensor, min_x, min_y, min_z, max_x, max_y, max_z) -> torch.Tensor:

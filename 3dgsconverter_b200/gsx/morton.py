@@ -8,7 +8,8 @@ import numpy as np
 import torch
 
 from ._abi import lib, check
-from .sor import _ptr, _stream, _check_xyz
+from ._abi import _ptr, _stream
+from .sor import _check_xyz
 
 
 def morton_order(xyz: torch.Tensor, run_limit: int = 256, return_levels: bool = False):

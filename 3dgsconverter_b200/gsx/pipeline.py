@@ -14,7 +14,7 @@ import torch
 
 from . import density as _density, masks as _masks, sor as _sor
 from ._abi import lib, check
-from .sor import _ptr, _stream
+from ._abi import _ptr, _stream
 
 
 def compact(mask: torch.Tensor, xyz: torch.Tensor, opacity: torch.Tensor | None, idx: torch.Tensor | None):

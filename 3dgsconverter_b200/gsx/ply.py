@@ -22,7 +22,7 @@ import numpy as np
 import torch
 
 from ._abi import lib, check
-from .sor import _ptr, _stream
+from ._abi import _ptr, _stream
 
 FLAVORS = ("3dgs", "cc")
 ROW_MAX = 1024          # widest input or output row gsx_ply_transcode takes, bytes

@@ -9,7 +9,7 @@ import numpy as np
 import torch
 
 from ._abi import lib, check
-from .sor import _ptr, _stream
+from ._abi import _ptr, _stream
 
 SH_C0 = 0.28209479177387814
 

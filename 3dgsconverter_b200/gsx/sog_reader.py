@@ -31,7 +31,7 @@ import torch
 
 from . import readers
 from ._abi import lib, check
-from .sor import _ptr, _stream
+from ._abi import _ptr, _stream
 
 COEFFS = (0, 9, 24, 45)        # sog.py:170: f_rest values per splat for 0 .. 3 bands
 ROLES = ("means_l", "means_u", "quats", "scales", "sh0", "labels", "centroids")

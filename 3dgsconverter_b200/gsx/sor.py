@@ -12,15 +12,9 @@ import numpy as np
 import torch
 
 from . import _abi
-from ._abi import lib, check, HASH_MODES
-
-
-def _stream():
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
-
-
-def _ptr(t):
-    return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
+# _ptr and _stream live in _abi; the SOR stages here and in dist.py look them up through this module, so replacing
+# sor._stream reaches every one of them
+from ._abi import lib, check, HASH_MODES, _ptr, _stream
 
 
 def default_hash_mode() -> str:

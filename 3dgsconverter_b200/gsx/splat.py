@@ -19,7 +19,8 @@ import torch
 from . import readers
 from ._abi import lib, check
 from .compressed_ply import PACK_FIELDS
-from .sor import _ptr, _stream, sort_pairs
+from ._abi import _ptr, _stream
+from .sor import sort_pairs
 
 
 @dataclass

@@ -23,7 +23,7 @@ import torch
 from . import readers
 from ._abi import lib, check
 from .compressed_ply import PACK_FIELDS
-from .sor import _ptr, _stream
+from ._abi import _ptr, _stream
 
 MAGIC, VERSION, FRACTIONAL_BITS, FLAG_ANTIALIASED = 0x5053474E, 3, 12, 1
 SH_DIM = {0: 0, 1: 3, 2: 8, 3: 15}

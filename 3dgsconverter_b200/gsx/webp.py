@@ -17,7 +17,7 @@ import numpy as np
 import torch
 
 from ._abi import lib, check
-from .sor import _ptr, _stream
+from ._abi import _ptr, _stream
 
 MAX_SIDE = 16384
 TILE_BITS = 4

@@ -6,6 +6,7 @@
  * exposes is the Python module surface gsconverter.processing.{gpu_ops,data_processor}.
  * Each entry point below names the reference interface it replaces (path:line relative
  * to /root/reference/gsconverter/).  INTEGRATION.md shows the ctypes binding.
+ * The Python binding (gsx/_abi.py) is derived from this file: it parses every gsx_* prototype.
  *
  * Conventions
  *   - plain C types only; device pointers are ordinary pointers into CUDA device

@@ -8,7 +8,7 @@ ROOT = Path(__file__).resolve().parent.parent
 sys.path.insert(0, str(ROOT)); sys.path.insert(0, str(ROOT / "3dgsconverter_b200"))
 from gsx import sor  # noqa: E402
 from gsx._abi import lib, check  # noqa: E402
-from gsx.sor import _ptr, _stream  # noqa: E402
+from gsx._abi import _ptr, _stream  # noqa: E402
 import importlib.util  # noqa: E402
 spec = importlib.util.spec_from_file_location("b", ROOT / "bench.py"); b = importlib.util.module_from_spec(spec); spec.loader.exec_module(b)
 from gsx import synth  # noqa: E402

@@ -20,7 +20,7 @@ import torch  # noqa: E402
 
 from gsx import compressed_ply, morton, records, synth  # noqa: E402
 from gsx._abi import check, lib  # noqa: E402
-from gsx.sor import _ptr, _stream  # noqa: E402
+from gsx._abi import _ptr, _stream  # noqa: E402
 
 PEAK_GBPS = 3350.0   # H100 SXM data-sheet HBM3 bandwidth
 

@@ -25,7 +25,7 @@ import torch  # noqa: E402
 
 from gsx import records, sog, synth, webp  # noqa: E402
 from gsx._abi import lib  # noqa: E402
-from gsx.sor import _ptr, _stream  # noqa: E402
+from gsx._abi import _ptr, _stream  # noqa: E402
 
 
 def card():

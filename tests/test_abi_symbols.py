@@ -20,8 +20,31 @@ def test_header_symbols_exported(gsx_lib):
 
 
 def test_binding_covers_header(gsx_lib):
+    """The ctypes signatures are parsed from include/gsx.h: one per declared function, each from the known types."""
     from gsx import _abi
     assert set(declared_functions()) == set(_abi._SIGS), "gsx/_abi.py and include/gsx.h disagree"
+    known = set(_abi._SCALARS.values()) | {C.c_void_p, C.c_char_p}
+    for name, (res, args) in _abi._SIGS.items():
+        fn = getattr(gsx_lib, name)
+        assert fn.restype is res and fn.argtypes == args, name
+        assert res in known and all(a in known - {None, C.c_char_p} for a in args), name
+    sig = _abi._SIGS
+    assert sig["gsx_last_error"] == (C.c_char_p, [])
+    assert sig["gsx_sor_cell_size"] == (C.c_float, [C.c_void_p, C.c_int64])
+    assert sig["gsx_alpha_logit_threshold"] == (C.c_double, [C.c_double])
+    assert sig["gsx_density_voxel_range"][0] is None
+    assert sig["gsx_webp_emit"][1][4] is C.c_uint64
+    assert len(sig["gsx_sog_decode"][1]) == 12
+
+
+def test_void_pointer_takes_every_argument_form():
+    """Where the old hand-typed table had POINTER(...) parameters, c_void_p accepts what the product passes there."""
+    import numpy as np
+    a = np.arange(3, dtype=np.float32)
+    for arg in ((C.c_int32 * 4)(1, 2, 3, 4), (C.c_float * 3)(1, 2, 3), (C.c_void_p * 6)(), C.byref(C.c_int64()),
+                a.ctypes.data_as(C.POINTER(C.c_float)), a.ctypes.data_as(C.c_void_p), None):
+        C.c_void_p.from_param(arg)
+    assert C.c_void_p.from_param(None) is None
 
 
 def test_no_torch_types_in_abi():

@@ -168,7 +168,7 @@ def ref_grid(xyz, voxel, q0, dim):
 # ------------------------------------------------------------------------------------------------ device calls
 def _lib():
     from gsx._abi import lib, check
-    from gsx.sor import _stream
+    from gsx._abi import _stream
     return lib, check, _stream
 
 

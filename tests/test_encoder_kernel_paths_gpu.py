@@ -273,7 +273,7 @@ def test_sh_gather_case_reaches_its_path(ncols):
 def test_sog_sh_gather_columns_and_mask(ncols, n, cuda, gsx_lib):
     import torch
     from gsx import _abi
-    from gsx.sor import _ptr, _stream
+    from gsx._abi import _ptr, _stream
     rows, cols, order = sh_gather_case(ncols, n)
     rt, ot = torch.from_numpy(rows).to(cuda), torch.from_numpy(order).to(cuda)
     out = torch.full((n, ncols), 7.0, dtype=torch.float32, device=cuda)
@@ -320,7 +320,7 @@ def test_labels_case_reaches_its_path(name):
 def test_sog_labels_passthrough_and_wrap(name, cuda, gsx_lib):
     import torch
     from gsx import _abi
-    from gsx.sor import _ptr, _stream
+    from gsx._abi import _ptr, _stream
     labels, offsets, passthrough, chunk, pixels, want = labels_case(name)
     lt = torch.from_numpy(labels).to(cuda)
     out = torch.full((pixels, 4), 9, dtype=torch.uint8, device=cuda)
@@ -357,7 +357,7 @@ def test_centroids_case_reaches_its_path(P, coeffs):
 def test_sog_centroids_layout(P, coeffs, cuda, gsx_lib):
     import torch
     from gsx import _abi
-    from gsx.sor import _ptr, _stream
+    from gsx._abi import _ptr, _stream
     pal, cb, pixels, want = centroids_case(P, coeffs)
     pt, ct = torch.from_numpy(pal).to(cuda), torch.from_numpy(cb).to(cuda)
     out = torch.zeros((pixels, 4), dtype=torch.uint8, device=cuda)

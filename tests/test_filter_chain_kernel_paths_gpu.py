@@ -463,7 +463,7 @@ def colour_rows(scale, n=1003, F=14):
 # ------------------------------------------------------------------------------------------------ device calls
 def _lib():
     from gsx._abi import lib, check
-    from gsx.sor import _ptr, _stream
+    from gsx._abi import _ptr, _stream
     return lib, check, _ptr, _stream
 
 

@@ -121,7 +121,7 @@ def test_numpy_logf_every_float32(cuda, gsx_lib):
     from gsx._abi import check as gcheck, lib
     from gsx.hostcopy import to_host
     from gsx.readers import tables_on
-    from gsx.sor import _ptr, _stream
+    from gsx._abi import _ptr, _stream
     m = 1 << 24
     rec = torch.zeros((m, 32), dtype=torch.uint8, device=cuda)
     rows = torch.empty((m, 71), dtype=torch.uint8, device=cuda)

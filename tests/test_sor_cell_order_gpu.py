@@ -29,7 +29,7 @@ def test_build_orders_buckets_by_hilbert_code(kind, cuda, gsx_lib):
     import torch
     from gsx import sor, synth
     from gsx._abi import lib, check
-    from gsx.sor import _ptr, _stream
+    from gsx._abi import _ptr, _stream
     xyz_np = synth.xyz(200_000, kind)
     n = len(xyz_np)
     xyz = torch.from_numpy(xyz_np).to(cuda)

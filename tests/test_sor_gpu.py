@@ -110,7 +110,7 @@ def test_build_from_sorted_equals_build(cuda, gsx_lib, cell_scale):
     import oracle
     from gsx import sor, synth
     from gsx._abi import lib, check
-    from gsx.sor import _ptr, _stream
+    from gsx._abi import _ptr, _stream
     xyz_np = synth.xyz(200_000, "mixed")
     xyz = torch.from_numpy(xyz_np).to(cuda)
     n = xyz.shape[0]

@@ -184,7 +184,7 @@ def test_radix_onesweep_pairs_and_keys(n, bits, kind, cuda, gsx_lib):
     less is refused), against np.argsort(kind="stable") of the field, compared as uint64."""
     import torch
     from gsx import _abi
-    from gsx.sor import _ptr, _stream
+    from gsx._abi import _ptr, _stream
     b0, b1 = bits
     keys = radix_keys(n, b0, b1, kind)
     want = np.argsort(field_of(keys, b0, b1), kind="stable")

@@ -299,7 +299,7 @@ def _astype_threads(x, dtype):
 
 def _ksplat_pack_raw(rows, n, level, sh_count, centres, out):
     from gsx import _abi
-    from gsx.sor import _ptr, _stream
+    from gsx._abi import _ptr, _stream
     F = rows.shape[1]
     c14 = (C.c_int32 * 14)(*[k % F for k in range(14)])
     csh = (C.c_int32 * max(sh_count, 1))(*range(sh_count))
@@ -431,7 +431,7 @@ def test_mask_case_reaches_its_path(kind, place):
 def test_codec_sh_mask_lone_value_per_column(kind, place, cuda, gsx_lib):
     import torch
     from gsx import _abi, ksplat, spz
-    from gsx.sor import _ptr, _stream
+    from gsx._abi import _ptr, _stream
     n, _ = MASK_PLACES[place]
     cols = (C.c_int32 * 45)(*MASK_COLS.tolist())
     mask = torch.empty(1, dtype=torch.int64, device=cuda)
@@ -491,7 +491,7 @@ def test_centres_case_reaches_its_paths():
 def test_ksplat_centres_nan_and_overflow(cuda, gsx_lib):
     import torch
     from gsx import _abi
-    from gsx.sor import _ptr, _stream
+    from gsx._abi import _ptr, _stream
     lo, hi = centres_case()
     lt, ht = torch.from_numpy(lo).to(cuda), torch.from_numpy(hi).to(cuda)
     out = torch.full((64, 3), 7.0, dtype=torch.float32, device=cuda)

@@ -14,7 +14,7 @@ pytestmark = pytest.mark.gpu
 def test_sharded_mean_std_matches_numpy(sizes, cuda, gsx_lib):
     import torch
     from gsx._abi import lib, check
-    from gsx.sor import _ptr, _stream
+    from gsx._abi import _ptr, _stream
     rng = np.random.default_rng(sum(sizes))
     n = int(sum(sizes))
     a = (rng.random(n, dtype=np.float32) * np.float32(3.0)).astype(np.float32)
