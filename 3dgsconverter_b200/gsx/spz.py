@@ -1,5 +1,5 @@
 """The .spz reader and writer on the device.  decode: formats/spz.py:18-47, 175-296 (SpzFormat.read, _read_body): gunzip
-and the 16-byte header on the host, the planar body on the GPU (gsx_spz_decode).  encode: formats/spz.py:49-173
+on the GPU (gsx.deflate.gunzip), the 16-byte header on the host, the planar body on the GPU (gsx_spz_decode).  encode: formats/spz.py:49-173
 (SpzFormat.write, _pack_v3) over DeviceRecords.  The SH degree
 rule reads one non-zero mask of the f_rest columns (gsx_codec_sh_mask); the planar body is packed on the GPU
 (gsx_spz_pack) behind the 16-byte header; the host runs gzip, or with where="device" gsx.deflate does, cutting its
@@ -145,15 +145,28 @@ def read_tables():
 
 
 def decode(data, device="cuda") -> readers.Decoded:
-    """SpzFormat.read on the device, `data` the file's bytes or its path (gunzipped on the host when it starts with
-    1f 8b).  Refused (ValueError) where the reference raises or does not read the file as written: a bad magic or
-    version, a body shorter than the header's count needs, 1 << frac_bits beyond float32."""
+    """SpzFormat.read on the device, `data` the file's bytes or its path.  A file that starts with 1f 8b is gunzipped
+    on the device (gsx.deflate.gunzip: gzip.decompress's bytes or exception class), so only the file crosses PCIe and
+    only the 16-byte header comes back -- unless its first block is stored (level 0, the reference writer's default),
+    where gzip.decompress on the host is faster.  Refused (ValueError) where the reference raises or does not read the file
+    as written: a bad magic or version, a body shorter than the header's count needs, 1 << frac_bits beyond
+    float32."""
     buf = readers.file_bytes(data)
+    payload = None
     if len(buf) > 2 and buf[0] == 0x1F and buf[1] == 0x8B:
-        buf = memoryview(gzip.decompress(buf))
-    if len(buf) < 16:
+        from .deflate import first_block_stored, gunzip
+        if first_block_stored(buf):      # level 0: zlib's copy on the host is faster than the device's chunk chain
+            buf = memoryview(gzip.decompress(buf))
+        else:
+            from .hostcopy import to_host
+            payload = gunzip(buf, device)
+    if payload is not None:
+        size, head = payload.numel(), to_host(payload[:16]).tobytes()
+    else:
+        size, head = len(buf), bytes(buf[:16])
+    if size < 16:
         raise ValueError("spz: shorter than its header")
-    magic, version, n, degree, frac_bits, _, _ = struct.unpack_from("<IIIBBBB", buf, 0)
+    magic, version, n, degree, frac_bits, _, _ = struct.unpack_from("<IIIBBBB", head, 0)
     if magic != MAGIC or not 1 <= version <= 3:
         raise ValueError(f"spz: magic {magic:#x} / version {version}")
     if frac_bits > 127:
@@ -162,10 +175,10 @@ def decode(data, device="cuda") -> readers.Decoded:
         raise ValueError("spz: 2^31 splats or more")
     dim = SH_DIM.get(degree, 0)
     need = n * ((6 if version == 1 else 9) + 7 + (4 if version >= 3 else 3) + 3 * dim)
-    if len(buf) - 16 < need:
+    if size - 16 < need:
         raise ValueError("spz: body cut short")
     dtype = readers.gaussian_dtype(has_rgb=True, sh_degree=degree)
-    raw = readers.upload(buf[16:16 + need], device)
+    raw = payload[16:16 + need] if payload is not None else readers.upload(buf[16:16 + need], device)
     rows = torch.empty((n, dtype.itemsize), dtype=torch.uint8, device=raw.device)
     tabs = readers.tables_on(raw.device, *read_tables())
     with torch.cuda.device(raw.device):

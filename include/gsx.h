@@ -296,6 +296,29 @@ int gsx_webp_emit(int64_t width, int64_t height, int32_t image, const uint32_t* 
                   unsigned long long* total_bits_dev, void* stream);
 int gsx_webp_patch(uint32_t* words_dev, int64_t nwords, const uint32_t* patches_dev, int64_t npatches, void* stream);
 
+/* ---- raw DEFLATE (RFC 1951) decoding on the device: the bodies of gzip members (gsx/deflate.py gunzip) -----------
+ * data_dev is n bytes of HBM starting at a DEFLATE stream (64-bit n); bit offsets count LSB first from its byte 0.
+ * The workspace holds 16-bit symbols: gsx_inflate_workspace_bytes(symbols) bytes hold `symbols` of them.
+ * gsx_inflate_run runs njobs jobs, one thread each.  jobs_dev int64 [njobs, 6] = lo, hi, target, symbol offset into
+ * the workspace, capacity in symbols, flags (1 = FIND: start at the first plausible block start in bits [lo, hi), a
+ * dynamic block that decodes to its end-of-block or a stored block with zero padding and LEN = ~NLEN; else start at
+ * lo.  2 = FIRST: the start is the stream's first bit, so a distance past the first byte is an error).  A job decodes
+ * blocks until one ends at or past `target` or the final block ends.  Symbols: a byte (0..255), or 0x8000 | w, byte w
+ * of the 32 KiB before the start.  results_dev int64 [njobs, 6] = start (-1: none found), stop (bit after the last
+ * whole block), symbols written, position of the last 0x8000 symbol (-1: none), status, bit where it stopped.
+ * Status: 0 target reached, 1 final block ended, 2 the input ended (zlib: EOFError), 3 invalid stream (zlib.error),
+ * 4 capacity exceeded, 5 no plausible start, 6 a job outside the input or the workspace.
+ * gsx_inflate_resolve writes the pieces pieces_dev int64 [npieces, 5] = symbols (device pointer), count, output
+ * offset, first and one-past-last position of the markers resolved in chain order (a piece's last 32 KiB: the next
+ * piece's window) into out_dev, pieces in chain order and each window byte before its piece.  A marker before out_dev's
+ * first byte is zlib's "invalid distance too far back": *status_dev (set to 2^64-1 by the caller) becomes the least
+ * such output offset. */
+int64_t gsx_inflate_workspace_bytes(int64_t symbols);
+int gsx_inflate_run(const uint8_t* data_dev, int64_t n, const int64_t* jobs_dev, int64_t njobs, void* ws_dev,
+                    int64_t ws_bytes, int64_t* results_dev, void* stream);
+int gsx_inflate_resolve(const int64_t* pieces_dev, int64_t npieces, uint8_t* out_dev,
+                        unsigned long long* status_dev, void* stream);
+
 /* ---- raw DEFLATE (RFC 1951) and CRC-32 on the device: the body and trailer of .gz files (gsx/deflate.py) ---------
  * data_dev is n bytes of HBM (64-bit n).  Every pointer is a device pointer; every entry runs on `stream`.
  * gsx_deflate_workspace_bytes(nblocks): the workspace of gsx_crc32 (nblocks 0), gsx_deflate_plan and
