@@ -23,7 +23,9 @@ decompresses to the same payload, in gsx's bytes, not zlib's).  With
 host, every splat decoded on the device, byte for byte as the reference readers; files gsx refuses go to the original
 ``read``).  With ``patch(sog_reader="device")`` also ``SogFormat.read`` (gsx.sog_reader.decode: ZIP, meta.json and
 WebP on the host, the shN palette and every splat decoded on the device, byte for byte as the reference reader, its
-palette indexing included; bundles gsx refuses go to the original ``read``).  With ``patch(ply="device")`` also the
+palette indexing included; bundles gsx refuses go to the original ``read``); ``patch(sog_reader="device",
+sog_reader_webp="device")`` also decodes the lossless WebP members on the device (gsx.webp_decode), so only their
+compressed bytes cross PCIe.  With ``patch(ply="device")`` also the
 ``read`` and ``write`` of ``Ply3DGSFormat`` and ``PlyCCFormat`` (gsx.ply: header and field mapping on the host, the rows
 transcoded on the device, byte for byte as the reference; files and records gsx refuses, and writes with
 ``extra_elements``, go to the original method).  The parquet reader and writer stay on the host.
@@ -68,7 +70,7 @@ class _GsxCodebookKMeans:
 
 def patch(verbose: bool = False, defer: bool = True, codebook: str = "sklearn", require_cuda: bool = True,
           sog: str = "host", codecs: str = "host", readers: str = "host", sog_reader: str = "host", ply: str = "host",
-          sog_webp: str = "host", spz_gzip: str = "host"):
+          sog_webp: str = "host", spz_gzip: str = "host", sog_reader_webp: str = "host"):
     """require_cuda: refuse (return False, leave the reference untouched) when no CUDA device is usable, so that a
     CPU-only host keeps the reference's own SciPy / scikit-learn paths (there is no CPU fallback inside gsx).
     sog: "host" keeps the reference's SogFormat.write (with the patched gpu_ops.kmeans and its batch-ahead);
@@ -85,6 +87,9 @@ def patch(verbose: bool = False, defer: bool = True, codebook: str = "sklearn", 
     device readers on them (files gsx refuses go to the original read).
     sog_reader: "host" keeps the reference's SogFormat.read; "device" installs gsx.sog_reader's device reader on it
     (bundles gsx refuses go to the original read).
+    sog_reader_webp: with sog_reader="device" only.  "host" decodes the bundle's WebP members with Pillow, as the
+    reference does; "device" uploads their bytes and decodes the lossless ones on the device (gsx.webp_decode, pixel
+    for pixel as Pillow; a member it refuses sends the bundle to the original read).
     ply: "host" keeps the reference's plain 3DGS and CloudCompare PLY read and write; "device" installs gsx.ply's device
     reader and writer on Ply3DGSFormat and PlyCCFormat (files and records gsx refuses go to the original method)."""
     if sog not in ("host", "device"):
@@ -103,6 +108,10 @@ def patch(verbose: bool = False, defer: bool = True, codebook: str = "sklearn", 
         raise ValueError(f"readers must be 'host' or 'device', not {readers!r}")
     if sog_reader not in ("host", "device"):
         raise ValueError(f"sog_reader must be 'host' or 'device', not {sog_reader!r}")
+    if sog_reader_webp not in ("host", "device"):
+        raise ValueError(f"sog_reader_webp must be 'host' or 'device', not {sog_reader_webp!r}")
+    if sog_reader_webp == "device" and sog_reader != "device":
+        raise ValueError("sog_reader_webp='device' needs sog_reader='device': the reference reader decodes on the host")
     if ply not in ("host", "device"):
         raise ValueError(f"ply must be 'host' or 'device', not {ply!r}")
     if require_cuda:
@@ -157,7 +166,7 @@ def patch(verbose: bool = False, defer: bool = True, codebook: str = "sklearn", 
         install_sog(sog_mod.SogFormat, webp=sog_webp)  # sog.py:249-639 -> textures and palette on the GPU
     if sog_mod is not None and sog_reader == "device" and hasattr(sog_mod, "SogFormat"):
         from .sog_reader import install_reader as install_sog_reader
-        install_sog_reader(sog_mod.SogFormat)         # sog.py:23-247 -> palette and rows on the GPU
+        install_sog_reader(sog_mod.SogFormat, webp=sog_reader_webp)   # sog.py:23-247 -> palette and rows on the GPU
     cply = sys.modules.get("gsconverter.formats.compressed_ply")
     if cply is None:
         try:

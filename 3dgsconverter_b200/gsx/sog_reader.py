@@ -3,7 +3,7 @@
     dec = gsx.sog_reader.decode("in.sog")    # readers.Decoded: dec.to_host() is what SogFormat.read returns
     r = dec.records()                         # DeviceRecords (zero-copy: every field is float32)
 
-The ZIP, meta.json and the WebP members are handled on the host: the members are decoded with Pillow exactly as
+The ZIP, meta.json and (by default) the WebP members are handled on the host: the members are decoded with Pillow exactly as
 read_webp_to_flat does (Image.open, convert('RGBA') unless already RGBA), concurrently on GSX_HOST_THREADS threads, and
 the pixels every step reads go to the device in one copy.  The maps of one stored value -- the three position axes
 (65 536 u16 codes each, float64 exp as NumPy computes it), the quaternion component and opacity bytes -- are tables
@@ -11,7 +11,8 @@ built with the reference's own NumPy expressions.  On the device: the shN palett
 reader's own centroid indexing, which differs from the writer's layout for palette entries >= 64 and is reproduced
 as it is, then one row per splat (gsx_sog_decode).
 
-decode_textures(pixels, meta) is the device stage alone, from already-decoded RGBA pixels.
+decode_textures(pixels, meta) is the device stage alone, from already-decoded RGBA pixels.  decode(..., webp="device")
+uploads the members' compressed bytes instead and decodes the lossless ones on the device (gsx.webp_decode).
 
 Anything the reference rejects, or that gsx does not reproduce (negative `bands`, which the reference accepts through
 Python's negative indexing), raises ValueError; the drop-in reader then runs the reference's own read.
@@ -228,12 +229,67 @@ def open_bundle(data):
     return zf, meta
 
 
-def decode(data, device="cuda", threads: int | None = None) -> readers.Decoded:
+def decode_members_device(zf: zipfile.ZipFile, members: dict, device, threads: int | None = None) -> dict:
+    """member name -> uint8 CUDA tensor of its first `need` RGBA pixels.  Lossless members whose main image has one
+    prefix-code group and no colour cache (every member gsx.webp writes) are decoded on the device by gsx.webp_decode,
+    so only their compressed bytes are uploaded; the others (libwebp's multi-group or cached streams, lossy WebP,
+    ALPH, animation) are decoded with Pillow, concurrently, as decode_members does."""
+    from .webp_decode import container, decode_lossless
+    out, blobs, host = {}, {}, {}
+    for name, need in members.items():
+        try:
+            blobs[name] = blob = zf.read(name)
+        except KeyError:
+            raise ValueError(f"SOG: member {name!r} named in meta.json is missing") from None
+        except (zipfile.BadZipFile, OSError, NotImplementedError, RuntimeError) as e:
+            raise ValueError(f"SOG: member {name!r}: {e}") from None
+        px = None
+        if container(blob) is not None:
+            try:
+                px = decode_lossless(blob, device, parallel_only=True)
+            except ValueError as e:
+                raise ValueError(f"SOG: member {name!r} does not decode: {e}") from None
+        if px is None:
+            host[name] = need
+            continue
+        px = px.reshape(-1)
+        if px.numel() < 4 * need:
+            raise ValueError(f"Image {name} too small: {px.numel() // 4} < {need}")
+        out[name] = px[:4 * need]
+    if host:
+        from .hostcopy import to_device
+        flat = to_device(decode_members(_Members(blobs), host, threads), device)
+        off = 0
+        for name, need in host.items():
+            out[name] = flat[off:off + 4 * need]
+            off += 4 * need
+    return out
+
+
+class _Members:
+    """The read() of a ZipFile whose members are already read, for decode_members."""
+
+    def __init__(self, blobs):
+        self.blobs = blobs
+
+    def read(self, name):
+        return self.blobs[name]
+
+
+def decode(data, device="cuda", threads: int | None = None, webp: str = "host") -> readers.Decoded:
     """SogFormat.read on the device: `data` is the bundle's bytes or a path.  threads: Pillow decode threads
-    (default GSX_HOST_THREADS)."""
+    (default GSX_HOST_THREADS).  webp: "host" decodes the WebP members with Pillow and uploads their pixels;
+    "device" decodes the single-group, cache-free lossless members on the device from their uploaded bytes and the
+    rest with Pillow (decode_members_device)."""
+    if webp not in ("host", "device"):
+        raise ValueError(f"webp must be 'host' or 'device', not {webp!r}")
     zf, meta = open_bundle(data)
     layout = parse_meta(meta)
     members = layout.members()
+    if webp == "device":
+        with zf:
+            pixels = decode_members_device(zf, members, device, threads)
+        return decode_textures(pixels, layout)
     with zf:
         flat = decode_members(zf, members, threads)
     from .hostcopy import to_device
@@ -299,6 +355,10 @@ def decode_textures(pixels: dict, meta) -> readers.Decoded:
     return readers.Decoded(rows, dtype, None)
 
 
-def install_reader(cls) -> None:
-    """Make cls.read the device reader, keeping the original as cls._gsx_reference_read (idempotent)."""
-    readers.install(cls, decode)
+def install_reader(cls, webp: str = "host") -> None:
+    """Make cls.read the device reader, keeping the original as cls._gsx_reference_read (idempotent).  webp: where the
+    WebP members are decoded (see decode)."""
+    if webp not in ("host", "device"):
+        raise ValueError(f"webp must be 'host' or 'device', not {webp!r}")
+    cls._gsx_sog_reader_webp = webp            # read at every call, so a later install changes it
+    readers.install(cls, lambda path: decode(path, webp=getattr(cls, "_gsx_sog_reader_webp", "host")))

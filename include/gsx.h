@@ -296,6 +296,43 @@ int gsx_webp_emit(int64_t width, int64_t height, int32_t image, const uint32_t* 
                   unsigned long long* total_bits_dev, void* stream);
 int gsx_webp_patch(uint32_t* words_dev, int64_t nwords, const uint32_t* patches_dev, int64_t npatches, void* stream);
 
+/* ---- lossless WebP (VP8L, RFC 9649) decoding on the device: the SOG reader's members (gsx/webp_decode.py) ---------
+ * data_dev is the n-byte VP8L payload (from its 0x2f signature); bit offsets count LSB first from its byte 0.
+ * gsx_vp8l_header_words(width, height, groups): uint32 words of the header workspace for an image of that size whose
+ * main image has `groups` prefix-code groups (0 for sides outside 1..16384 or groups outside 1..65536).
+ * gsx_vp8l_header (one thread) parses the header, transforms, sub-images, cache bits, entropy image and every group's
+ * prefix codes into ws_dev; lens_dev is 2328 bytes of scratch.  info_dev int64 [32]: 0 status (0 ok, 1 truncated,
+ * 2 a bad prefix code or sub-image copy, 3 a bad header field, 4 the workspace is too small: [29] words needed), 1 bit
+ * where it stopped, 2 width, 3 height, 4 alpha hint, 5 coded width, 6 cache bits, 7 meta prefix bits, 8 groups,
+ * 9 entropy image word offset (-1: none), 10 codes word offset, 11 first bit of the main image, 12 transforms, then
+ * per transform in reading order 4 values: type (0 predictor, 1 cross-colour, 2 subtract-green, 3 colour indexing),
+ * the width it applies at, its bits, its sub-image's word offset.
+ * gsx_vp8l_run runs njobs jobs, one thread each: jobs_dev int64 [njobs, 5] = start bit, target bit, guessed first
+ * pixel, token offset, capacity in tokens.  A job decodes tokens (16 bytes each in tokens_dev: value, kind << 28 |
+ * pixels, first pixel relative to the job, group) until it stands at or past target, or its pixels reach the image's
+ * end.  results_dev int64 [njobs, 6] = start, stop bit, tokens, pixels, status (0 target, 1 image end, 2 the input
+ * ended, 4 capacity), bit where it stopped.
+ * gsx_vp8l_check sets flags_dev[k] (zeroed by the caller) when a token of piece k (pieces_dev int64 [npieces, 3] =
+ * device address of its tokens, tokens, true first pixel) used a group other than the one at its true position.
+ * gsx_vp8l_resolve writes the chain's pieces (same layout, in pixel order) as ARGB into out_dev [npix], with src_dev
+ * int32 [npix] as scratch; *err_dev (zeroed) gains 1 for a copy from before the first pixel, 2 for one past the last.
+ * gsx_vp8l_inverse applies one inverse transform to the xs x height image: colour indexing reads in_dev (the packed
+ * image) and writes out_dev; the others work in place on out_dev.  scratch_dev: int32 [height / 32 + 2] (predictor).
+ * gsx_vp8l_rgba writes n ARGB pixels as RGBA bytes, alpha 255 when alpha is 0. */
+int64_t gsx_vp8l_header_words(int64_t width, int64_t height, int64_t groups);
+int gsx_vp8l_header(const uint8_t* data_dev, int64_t n, uint32_t* ws_dev, int64_t ws_words, uint8_t* lens_dev,
+                    int64_t* info_dev, void* stream);
+int gsx_vp8l_run(const uint8_t* data_dev, int64_t n, const uint32_t* codes_dev, const uint32_t* entropy_dev,
+                 int64_t xsize, int64_t height, int32_t meta_bits, const int64_t* jobs_dev, int64_t njobs,
+                 void* tokens_dev, int64_t* results_dev, void* stream);
+int gsx_vp8l_check(const uint32_t* codes_dev, const uint32_t* entropy_dev, int64_t xsize, int64_t height,
+                   int32_t meta_bits, const int64_t* pieces_dev, int64_t npieces, int32_t* flags_dev, void* stream);
+int gsx_vp8l_resolve(const int64_t* pieces_dev, int64_t npieces, int64_t xsize, int64_t npix, int32_t cache_bits,
+                     uint32_t* out_dev, int32_t* src_dev, int32_t* err_dev, void* stream);
+int gsx_vp8l_inverse(int32_t type, const uint32_t* in_dev, uint32_t* out_dev, const uint32_t* sub_dev, int64_t xs,
+                     int64_t height, int32_t bits, int32_t* scratch_dev, void* stream);
+int gsx_vp8l_rgba(const uint32_t* argb_dev, uint8_t* rgba_dev, int64_t n, int32_t alpha, void* stream);
+
 /* ---- raw DEFLATE (RFC 1951) decoding on the device: the bodies of gzip members (gsx/deflate.py gunzip) -----------
  * data_dev is n bytes of HBM starting at a DEFLATE stream (64-bit n); bit offsets count LSB first from its byte 0.
  * The workspace holds 16-bit symbols: gsx_inflate_workspace_bytes(symbols) bytes hold `symbols` of them.
