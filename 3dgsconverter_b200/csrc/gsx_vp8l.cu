@@ -74,21 +74,21 @@ struct Reader {
     }
 };
 
-// libwebp's acceptance: not all lengths 0, at most 2^len codes of each length, exactly one symbol of length 1..14 is a
-// 0-bit code, anything else must fill the code space.
+// libwebp's acceptance: not all lengths 0, at most 2^len codes of each length, exactly one used symbol (of any length
+// 1..15) is a 0-bit code, anything else must fill the code space.
 __device__ int64_t build_code(const uint8_t* len, int n, uint32_t* c) {
     uint32_t count[16];
     for (int i = 0; i < 16; ++i) count[i] = 0;
     for (int s = 0; s < n; ++s) ++count[len[s]];
     if (count[0] == uint32_t(n)) return kBadCode;
     uint32_t used = 0;
-    for (int b = 1; b < 15; ++b) {
+    for (int b = 1; b < 16; ++b) {
         if (count[b] > (1u << b)) return kBadCode;
         used += count[b];
     }
     if (used == 1) {
         for (int s = 0; s < n; ++s)
-            if (len[s] >= 1 && len[s] <= 14) c[0] = uint32_t(s);
+            if (len[s]) c[0] = uint32_t(s);
         return kOk;
     }
     int64_t left = 1;
@@ -152,7 +152,8 @@ __device__ __forceinline__ bool decode(Reader& r, const uint32_t* __restrict__ c
     return false;   // unreachable for a complete code
 }
 
-// One prefix code of `alphabet` symbols at r into c.
+// One prefix code of `alphabet` symbols at r into c.  A simple code's symbol past the alphabet (possible only in the
+// 40-symbol distance alphabet) gets no length, as in libwebp: the code is built from the others, and none is an error.
 __device__ int64_t read_code(Reader& r, int alphabet, uint32_t* c, uint8_t* len) {
     uint32_t v;
     if (!r.bits(1, v)) return kTrunc;
@@ -160,12 +161,10 @@ __device__ int64_t read_code(Reader& r, int alphabet, uint32_t* c, uint8_t* len)
     if (v) {
         uint32_t two, wide, s0, s1;
         if (!r.bits(1, two) || !r.bits(1, wide) || !r.bits(wide ? 8 : 1, s0)) return kTrunc;
-        if (int(s0) >= alphabet) return kBadCode;
-        len[s0] = 1;
+        if (int(s0) < alphabet) len[s0] = 1;
         if (two) {
             if (!r.bits(8, s1)) return kTrunc;
-            if (int(s1) >= alphabet) return kBadCode;
-            len[s1] = 1;
+            if (int(s1) < alphabet) len[s1] = 1;
         }
         return build_code(len, alphabet, c);
     }

@@ -9,7 +9,8 @@ The same stages as the device, one function each:
             re-run a chunk that overflowed its capacity with 8x more), then resolve the markers: tails in chain order,
             heads in any order
   gunzip    members, headers, trailers and zero padding as CPython's gzip.decompress
-Errors are the classes gzip.decompress raises: EOFError, gzip.BadGzipFile, zlib.error.
+Errors are the classes gzip.decompress raises: EOFError, gzip.BadGzipFile, zlib.error.  COUNTERS counts the code
+lengths, incomplete codes, stored blocks, long lengths and distances and capacity overflows that decodes reached.
 """
 from __future__ import annotations
 
@@ -19,6 +20,12 @@ import zlib
 
 MARK = 0x8000
 WINDOW = 32768
+COUNTERS: dict = {}      # what the decodes since the last clear reached, so tests can show a case hits its path
+
+
+def _count(key, n=1):
+    COUNTERS[key] = COUNTERS.get(key, 0) + n
+
 OK, FINAL, EOF, DATA, OVERFLOW = range(5)
 
 LBASE = [3, 4, 5, 6, 7, 8, 9, 10, 11, 13, 15, 17, 19, 23, 27, 31, 35, 43, 51, 59, 67, 83, 99, 115, 131, 163, 195, 227,
@@ -58,7 +65,8 @@ class Reader:
 class Code:
     """Canonical Huffman code of `lengths` as zlib's inflate_table judges it: over-subscribed, incomplete, empty."""
 
-    def __init__(self, lengths):
+    def __init__(self, lengths, name: str = ""):
+        self.name = name
         self.count = [0] * 16
         for n in lengths:
             self.count[n] += 1
@@ -80,6 +88,8 @@ class Code:
             code |= r.bits(1)
             c = self.count[n]
             if code - c < first:
+                if self.name:
+                    _count(f"{self.name}_len_{n}")
                 return self.syms[index + code - first]
             if n >= self.max:
                 raise Bad("invalid code")        # zlib reads max(1, longest code) bits of an incomplete code
@@ -104,6 +114,8 @@ def dynamic_codes(r: Reader):
     clc = Code(cl)
     if clc.over or (clc.incomplete and clc.max > 0):
         raise Bad("invalid code lengths set")
+    if not clc.max:
+        _count("cl_empty")
     lens = []
     while len(lens) < nlen + ndist:
         sym = clc.decode(r) if clc.max else (r.bits(1) & 0)   # an empty code-length code reads 1 bit as length 0
@@ -122,10 +134,12 @@ def dynamic_codes(r: Reader):
         lens += [val] * copy
     if lens[256] == 0:
         raise Bad("invalid code -- missing end-of-block")
-    lit, dist = Code(lens[:nlen]), Code(lens[nlen:])
+    lit, dist = Code(lens[:nlen], "lit"), Code(lens[nlen:], "dist")
     for c in (lit, dist):
         if c.over or (c.incomplete and c.max > 1):      # an empty or one-code set of 1 bit passes
             raise Bad("invalid literal/lengths or distances set")
+    if dist.incomplete:
+        _count("dist_empty" if dist.max == 0 else "dist_one_code")
     return lit, dist
 
 
@@ -142,8 +156,10 @@ def block(r: Reader, out, first: bool, cap: int | None) -> bool:
         if out is None:
             r.bits(8 * ln) if ln else None
             return bool(final)
+        _count(f"stored_len_{ln}" if ln in (0, 65535) else "stored")
         for _ in range(ln):
             if cap is not None and len(out) >= cap:
+                _count("overflow_stored")
                 raise Full
             out.append(r.bits(8))
         return bool(final)
@@ -154,6 +170,7 @@ def block(r: Reader, out, first: bool, cap: int | None) -> bool:
         if sym < 256:
             if out is not None:
                 if cap is not None and len(out) >= cap:
+                    _count("overflow_literal")
                     raise Full
                 out.append(sym)
             made += 1
@@ -163,16 +180,21 @@ def block(r: Reader, out, first: bool, cap: int | None) -> bool:
         if sym > 285:
             raise Bad("invalid literal/length code")
         length = LBASE[sym - 257] + r.bits(LEXT[sym - 257])
+        if length == 258 and out is not None:
+            _count("len_285" if sym == 285 else "len_284_31")
         ds = dist.decode(r)
         if ds > 29:
             raise Bad("invalid distance code")
         d = DBASE[ds] + r.bits(DEXT[ds])
+        if d == WINDOW and out is not None:
+            _count("dist_32768")
         if first and d > (len(out) if out is not None else made):
             raise Bad("invalid distance too far back")
         made += length
         if out is None:
             continue
         if cap is not None and len(out) + length > cap:
+            _count("overflow_copy")
             raise Full
         for _ in range(length):
             s = len(out) - d
@@ -287,8 +309,8 @@ def inflate(body: bytes, chunk_bytes: int, ratio: int = 4, stats: dict | None = 
     if chain[-1]["status"] == DATA:
         raise zlib.error("invalid deflate stream")
     out, far = resolve(chain)
-    if far:
-        raise zlib.error("invalid distance too far back")
+    if far is not None:
+        raise zlib.error(f"invalid distance too far back (output byte {far})")
     if chain[-1]["status"] == EOF:
         raise EOFError("Compressed file ended before the end-of-stream marker was reached")
     return bytes(out), chain[-1]["stop"]
@@ -297,12 +319,13 @@ def inflate(body: bytes, chunk_bytes: int, ratio: int = 4, stats: dict | None = 
 def resolve(chain):
     """Write the chain's symbols at their offsets (an exclusive scan of the lengths).  Pass 1 writes the bytes; pass 2
     walks the pieces in order over their last 32 KiB (the next piece's window), from the first to the last marker
-    there; pass 3 replaces the markers before that.  -> (bytes, whether a marker lands before the first byte)."""
+    there; pass 3 replaces the markers before that.  -> (bytes, the first output byte whose marker lands before the
+    first byte, or None)."""
     offs, total = [], 0
     for x in chain:
         offs.append(total)
         total += len(x["syms"])
-    out, far = bytearray(total), False
+    out, far = bytearray(total), None
 
     def fill(x, off, lo, hi):
         nonlocal far
@@ -311,7 +334,7 @@ def resolve(chain):
             if s & MARK:
                 t = off - WINDOW + (s & ~MARK)
                 if t < 0:
-                    far = True
+                    far = off + i if far is None else min(far, off + i)
                 else:
                     out[off + i] = out[t]
 

@@ -53,8 +53,8 @@ class Reader:
 
 
 class Code:
-    """A canonical prefix code from its lengths, libwebp's acceptance rule: not all zero, exactly one used symbol of
-    length 1..14 -> a 0-bit code, else the lengths must fill the code space exactly."""
+    """A canonical prefix code from its lengths, libwebp's acceptance rule: not all zero, exactly one used symbol (of
+    any length 1..15) -> a 0-bit code, else the lengths must fill the code space exactly."""
 
     def __init__(self, lengths):
         lengths = list(lengths)
@@ -66,8 +66,9 @@ class Code:
         for ln in range(1, 15):
             if count[ln] > (1 << ln):
                 raise ValueError("VP8L: an over-subscribed prefix code")
-        if sum(count[1:15]) == 1:
-            self.single = next(s for s, ln in enumerate(lengths) if 1 <= ln <= 14)
+        if sum(count[1:16]) == 1:
+            self.single = next(s for s, ln in enumerate(lengths) if ln)
+            _count(f"single_len_{lengths[self.single]}")
             return
         self.single = None
         left = 1
@@ -101,15 +102,21 @@ def read_code(br: Reader, alphabet: int) -> Code:
         _count("simple_code")
         two = br.read(1)
         lengths = [0] * alphabet
-        s0 = br.read(8 if br.read(1) else 1)
-        if s0 >= alphabet:
-            raise ValueError("VP8L: a simple code's symbol past its alphabet")
-        lengths[s0] = 1
+        wide = br.read(1)
+        _count("simple_code_8bit" if wide else "simple_code_1bit")
+        s0 = br.read(8 if wide else 1)
+        # a symbol past the alphabet (only the 40-symbol distance alphabet has room for one) gets no length, as in
+        # libwebp: the code is built from the other symbol, and Code refuses a simple code with none
+        if s0 < alphabet:
+            lengths[s0] = 1
+        else:
+            _count("simple_code_past_alphabet")
         if two:
             s1 = br.read(8)
-            if s1 >= alphabet:
-                raise ValueError("VP8L: a simple code's symbol past its alphabet")
-            lengths[s1] = 1
+            if s1 < alphabet:
+                lengths[s1] = 1
+            else:
+                _count("simple_code_past_alphabet")
             _count("simple_code_2")
         else:
             _count("simple_code_1")
