@@ -10,11 +10,12 @@
 //   k_cply_narrow_sh out[j, :keep] = sh[j, :keep]: the SH block cut down to the columns of the detected degree (:163-169).
 //
 // Arithmetic follows NumPy-2 float32 semantics (Python float constants are weak scalars, i.e. rounded to float32 first):
-// every step is one __f*_rn operation in the reference's order, with no contraction.  The alpha channel goes through
-// expf and can differ from NumPy's SIMD exp by one count on ~1e-5 of the splats; everything else is bit-exact.
+// every step is one __f*_rn operation in the reference's order, with no contraction, and the alpha channel's exp is
+// NumPy's SIMD float32 exp (gsx_numpy_scalar.cuh): every byte is bit-exact.
 #include "../../include/gsx.h"
 
 #include "gsx_common.cuh"
+#include "gsx_numpy_scalar.cuh"
 #include "gsx_sh_mask.cuh"
 
 namespace gsx {
@@ -136,7 +137,7 @@ __global__ void __launch_bounds__(kChunk) k_cply_pack(const float* __restrict__ 
         const float s2 = clip20(__ldg(r + cols.c[9]));
         const uint32_t scl = unorm(s0, sb[6], sb[9], 2047.f) << 21 | unorm(s1, sb[7], sb[10], 1023.f) << 11 |
                              unorm(s2, sb[8], sb[11], 2047.f);
-        const float a = __fdiv_rn(1.f, __fadd_rn(1.f, expf(-__ldg(r + cols.c[6]))));
+        const float a = __fdiv_rn(1.f, __fadd_rn(1.f, numpy_expf(-__ldg(r + cols.c[6]))));
         const uint32_t col = unorm(dc_color(__ldg(r + cols.c[3])), sb[12], sb[15], 255.f) << 24 |
                              unorm(dc_color(__ldg(r + cols.c[4])), sb[13], sb[16], 255.f) << 16 |
                              unorm(dc_color(__ldg(r + cols.c[5])), sb[14], sb[17], 255.f) << 8 |

@@ -1,10 +1,12 @@
 // gsx_numpy_scalar.cuh -- NumPy 2's float32 scalar semantics on x86-64, for the .splat / .ksplat / .spz writers and
-// readers (device code only).
+// readers, the SOG writer's position log and opacity exp, the compressed PLY alpha and the records' colour alpha and
+// scale exp (device code only).
 //
 //   numpy_expf     NumPy's SIMD float32 exp (AVX2 and AVX-512F give the same bytes): Cody-Waite reduction by ln 2,
 //                  a [5/2] rational approximation and an exact scaling by 2^q.  It is not correctly rounded (up to 2 ulp
 //                  from exp), so expf or a double exp rounded once would not reproduce the writers' raw float32 scales.
-//   numpy_logf     NumPy's SIMD float32 log (AVX-512F), on the .splat reader's domain.
+//   numpy_logf     NumPy's SIMD float32 log (AVX-512F), on the .splat reader's domain (which holds the SOG writer's
+//                  |v| + 1 >= 1).
 //   numpy_h2f      float16 -> float32 as astype(np.float32), NaN payloads kept.
 //   x86_*          float / double add, sub, mul, div and conversions with x86's NaN results (first NaN operand quieted,
 //                  the negative default NaN for invalid operations), where NaN inputs reach a reader's output.

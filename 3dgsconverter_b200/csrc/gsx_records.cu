@@ -11,12 +11,12 @@
 // and the elementwise attribute transforms every writer applies (formats/splat.py:92-147, ksplat.py:464-483,
 // spz.py:112-141, data_processor.py:301-333), fused over the resident rows:
 //   k_color_dc_u8    : clip((0.5 + C0*f_dc) * 255, 0, 255).astype(uint8) x3 + clip(sigmoid(opacity)*255).astype(uint8)
-//                      -> RGBA8 (float32 ops in NumPy's order; the colour channels are bit-exact, the alpha channel
-//                      goes through expf and can differ from NumPy's SIMD exp by one count on ~1e-5 of the splats)
-//   k_scale_exp      : exp(scale_0..2) -> float32 [n,3]
+//                      -> RGBA8 (float32 ops in NumPy's order, NumPy's SIMD float32 exp: bit-exact)
+//   k_scale_exp      : exp(scale_0..2) -> float32 [n,3], NumPy's SIMD float32 exp: bit-exact
 #include "../../include/gsx.h"
 
 #include "gsx_common.cuh"
+#include "gsx_numpy_scalar.cuh"
 
 namespace gsx {
 
@@ -59,7 +59,7 @@ __global__ void __launch_bounds__(256) k_color_dc_u8(const float* __restrict__ r
     o.y = to_u8_clip(__fmul_rn(__fadd_rn(0.5f, __fmul_rn(scale, __ldg(r + c1))), 255.f));
     o.z = to_u8_clip(__fmul_rn(__fadd_rn(0.5f, __fmul_rn(scale, __ldg(r + c2))), 255.f));
     // (1 / (1 + exp(-op))) * 255
-    const float e = expf(-__ldg(r + cop));
+    const float e = numpy_expf(-__ldg(r + cop));
     o.w = to_u8_clip(__fmul_rn(__fdiv_rn(1.0f, __fadd_rn(1.0f, e)), 255.f));
     rgba[i] = o;
 }
@@ -69,9 +69,9 @@ __global__ void __launch_bounds__(256) k_scale_exp(const float* __restrict__ row
     int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const float* r = rows + (size_t)i * F;
-    out[3 * i] = expf(__ldg(r + s0));
-    out[3 * i + 1] = expf(__ldg(r + s1));
-    out[3 * i + 2] = expf(__ldg(r + s2));
+    out[3 * i] = numpy_expf(__ldg(r + s0));
+    out[3 * i + 1] = numpy_expf(__ldg(r + s1));
+    out[3 * i + 2] = numpy_expf(__ldg(r + s2));
 }
 
 static int check_cols(int F, std::initializer_list<int> cols) {

@@ -11,6 +11,7 @@
 #include "../../include/gsx.h"
 
 #include "gsx_common.cuh"
+#include "gsx_numpy_scalar.cuh"
 #include "gsx_sh_mask.cuh"
 #include "gsx_radix.cuh"
 
@@ -74,8 +75,8 @@ __global__ void __launch_bounds__(256) k_quantize_codebook(const float* __restri
 // (row order[j] is the j-th splat of the file); no sorted copy of the records is made.  Textures are uchar4 [pixels]
 // with pixels >= n; the kernels write the padding pixels too.  Float steps are single __f*_rn operations in the
 // reference's NumPy-2 float32 order; float -> u8/u16 conversions clip with fmaxf/fminf, which maps NaN to 0 as NumPy
-// does on x86.  The logarithm of the positions and the exponential of the opacity are not NumPy's SIMD functions, so
-// those bytes can differ by one count on a small fraction of the splats (gsx/sog.py states the bounds).
+// does on x86.  The logarithm of the positions and the exponential of the opacity are NumPy's SIMD float32 log and exp
+// (gsx_numpy_scalar.cuh), so those bytes are exact too.
 
 namespace {
 
@@ -99,10 +100,11 @@ struct SogChunks {  // the shN chunk schedule of sog.py:527-549
 __device__ __forceinline__ float nan_min(float a, float b) { return a != a ? a : (b != b ? b : (b < a ? b : a)); }
 __device__ __forceinline__ float nan_max(float a, float b) { return a != a ? a : (b != b ? b : (b > a ? b : a)); }
 
-// sign(v) * log(|v| + 1) (sog.py:279-280): float32 add, the logarithm rounded once to float32, float32 product
+// sign(v) * log(|v| + 1) (sog.py:279-280): float32 add, NumPy's float32 log (its argument is >= 1 or NaN), float32
+// product
 __device__ __forceinline__ float log_transform(float v) {
     const float s = v > 0.f ? 1.f : (v < 0.f ? -1.f : (v == 0.f ? 0.f : v));
-    return __fmul_rn(s, __double2float_rn(log((double)__fadd_rn(fabsf(v), 1.f))));
+    return __fmul_rn(s, numpy_logf(__fadd_rn(fabsf(v), 1.f)));
 }
 
 // np.clip((l - min) / (max - min) * 65535, 0, 65535).astype(np.uint16) (sog.py:290-292)
@@ -261,7 +263,7 @@ __global__ void __launch_bounds__(256) k_sog_scales_sh0(const float* __restrict_
         scales[p] = make_uchar4(codebook_index(s_scb, ms, __ldg(r + cols.c[0])),
                                 codebook_index(s_scb, ms, __ldg(r + cols.c[1])),
                                 codebook_index(s_scb, ms, __ldg(r + cols.c[2])), 255);
-        const float a = __fdiv_rn(1.f, __fadd_rn(1.f, expf(-__ldg(r + cols.c[6]))));
+        const float a = __fdiv_rn(1.f, __fadd_rn(1.f, numpy_expf(-__ldg(r + cols.c[6]))));
         sh0[p] = make_uchar4(codebook_index(s_ccb, mc, __ldg(r + cols.c[3])),
                              codebook_index(s_ccb, mc, __ldg(r + cols.c[4])),
                              codebook_index(s_ccb, mc, __ldg(r + cols.c[5])),

@@ -17,10 +17,9 @@ in the reference's order, so np.random.seed reproduces a run), the fit of the 25
 (scikit-learn's MiniBatchKMeans by default, at most 65 536 x 45 values), and ZIP in write_sog, with
 the WebP members by Pillow or, given the SogTextures themselves, by gsx.webp on the device.
 
-Parity with the reference writer: every byte is exact except those that go through a transcendental.  The position
-logarithm is computed in double and rounded once, NumPy uses a SIMD float32 log, so a means u16 can differ by one on
-a small fraction of the splats (and meta.means mins/maxs by a few ulp); the opacity goes through expf, so the sh0
-alpha byte can differ by one on ~1e-5 of them.
+Parity with the reference writer: every texture byte and meta.json entry is exact.  The position logarithm and the
+opacity exponential are NumPy's SIMD float32 log and exp, restated exactly on the device.  The one exception is the
+sign of a zero meta.means min or max: NumPy's depends on where the zeros sit in the array, the value does not.
 """
 from __future__ import annotations
 

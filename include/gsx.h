@@ -235,8 +235,9 @@ int gsx_quantize_to_codebook(const float* vals_dev, int64_t n, const float* code
 /* Record rows are float32 [n, F]; every kernel reads row order_dev[j] for the j-th splat of the file (the lexsort
  * order).  Textures are uchar4 [pixels] (pixels >= n, 4-byte aligned); the padding pixels are written too.  Float
  * steps follow NumPy-2 float32 order; float -> u8/u16 conversions map NaN to 0.  n < 2^31.
- * The position logarithm and the opacity exponential are not NumPy's SIMD functions: a means u16 or the sh0 alpha
- * byte can differ by one count on a small fraction of the splats; everything else is bit-exact. */
+ * The position logarithm and the opacity exponential are NumPy's SIMD float32 log and exp, restated exactly: every
+ * byte is bit-exact.  The sign of a zero min or max of gsx_sog_means_minmax is not NumPy's (which depends on where
+ * the zeros sit); the value is. */
 /* sog.py:279-287: minmax_dev[6] = min x, y, z, max x, y, z of sign(v) * log(|v| + 1), NaN-propagating as
  * np.min / np.max.  cols3_host = columns of x, y, z; ws_dev >= 24576 B; n >= 1. */
 int gsx_sog_means_minmax(const float* rows_dev, int64_t n, int32_t F, const int32_t* cols3_host, float* ws_dev,
@@ -422,7 +423,7 @@ int gsx_kmeans_host(const float* X_host, int64_t n, int32_t K, int32_t D, int32_
  *  gather  : vertices[mask] of data_processor.py:114,149,209,224 for the surviving (ascending) row indices
  *  color   : RGBA8 of formats/splat.py:131-144, ksplat.py:464-468: clip((0.5 + scale*f_dc)*255).astype(u8) x3 (bit-exact
  *            float32 ops; scale = SH_C0 for .splat/.ksplat, 0.15 for spz.py:131) and clip(sigmoid(opacity)*255).astype(u8)
- *            (expf: may differ from NumPy's SIMD exp by one count on a ~1e-5 fraction of the splats)
+ *            (NumPy's SIMD float32 exp, restated exactly: bit-exact)
  *  scale   : np.exp(scale_0..2) of formats/splat.py:108, ksplat.py:447 -> float32 [n,3] */
 int gsx_records_extract_xyz_opacity(const float* rows_dev, int64_t n, int32_t F, int32_t cx, int32_t cy, int32_t cz,
                                     int32_t cop, float* xyz_dev, float* opacity_dev, void* stream);
@@ -464,7 +465,7 @@ int gsx_chunk_minmax(const float* rows_dev, int64_t n, int32_t F, const int32_t*
  * vertex_dev uint32[n,4] {packed_position, packed_rotation, packed_scale, packed_color}, sh_dev uint8[n,n_rest]
  * (may be NULL when n_rest == 0), *rest_nonzero_dev (device uint64, zeroed here) = bit k set iff packed SH column k holds
  * a value != 0 -- the input of the SH-degree rule of :141-169, which the caller applies (gsx_cply_narrow_sh).
- * NumPy-2 float32 arithmetic, bit-exact except the alpha byte (expf: one count on ~1e-5 of the splats).  vertex_dev and
+ * NumPy-2 float32 arithmetic and NumPy's SIMD float32 exp, bit-exact.  vertex_dev and
  * sh_dev 16-byte aligned; n < 2^31; n = 0 launches nothing.  A NaN field packs as NumPy's x86 cast gives it,
  * 0x80000000 shifted into the word (DESIGN §4.5); a quaternion's first NaN component is its largest. */
 int gsx_cply_pack(const float* rows_dev, int64_t n, int32_t F, const int32_t* order_dev, const int32_t* cols14_host,
