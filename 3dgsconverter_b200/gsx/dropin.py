@@ -28,7 +28,10 @@ sog_reader_webp="device")`` also decodes the lossless WebP members on the device
 compressed bytes cross PCIe.  With ``patch(ply="device")`` also the
 ``read`` and ``write`` of ``Ply3DGSFormat`` and ``PlyCCFormat`` (gsx.ply: header and field mapping on the host, the rows
 transcoded on the device, byte for byte as the reference; files and records gsx refuses, and writes with
-``extra_elements``, go to the original method).  The parquet reader and writer stay on the host.
+``extra_elements``, go to the original method).  With ``patch(parquet="device")`` also ``ParquetFormat.write``
+(gsx.parquet: columns, statistics, dictionaries, pages and Snappy built on the device; a file that pyarrow and pandas
+read as the same table, in gsx's bytes, not pyarrow's; records gsx refuses go to the original ``write``).  The parquet
+reader stays on the host.
 Host-only helpers and everything else of the reference stay as they are.
 """
 from __future__ import annotations
@@ -70,7 +73,7 @@ class _GsxCodebookKMeans:
 
 def patch(verbose: bool = False, defer: bool = True, codebook: str = "sklearn", require_cuda: bool = True,
           sog: str = "host", codecs: str = "host", readers: str = "host", sog_reader: str = "host", ply: str = "host",
-          sog_webp: str = "host", spz_gzip: str = "host", sog_reader_webp: str = "host"):
+          sog_webp: str = "host", spz_gzip: str = "host", sog_reader_webp: str = "host", parquet: str = "host"):
     """require_cuda: refuse (return False, leave the reference untouched) when no CUDA device is usable, so that a
     CPU-only host keeps the reference's own SciPy / scikit-learn paths (there is no CPU fallback inside gsx).
     sog: "host" keeps the reference's SogFormat.write (with the patched gpu_ops.kmeans and its batch-ahead);
@@ -91,7 +94,10 @@ def patch(verbose: bool = False, defer: bool = True, codebook: str = "sklearn", 
     reference does; "device" uploads their bytes and decodes the lossless ones on the device (gsx.webp_decode, pixel
     for pixel as Pillow; a member it refuses sends the bundle to the original read).
     ply: "host" keeps the reference's plain 3DGS and CloudCompare PLY read and write; "device" installs gsx.ply's device
-    reader and writer on Ply3DGSFormat and PlyCCFormat (files and records gsx refuses go to the original method)."""
+    reader and writer on Ply3DGSFormat and PlyCCFormat (files and records gsx refuses go to the original method).
+    parquet: "host" keeps the reference's ParquetFormat.write (pandas and pyarrow); "device" installs gsx.parquet's
+    device writer on it (records gsx refuses go to the original write).  The file then holds gsx's bytes, the same
+    table pyarrow writes, so this chooses the output, not only the speed."""
     if sog not in ("host", "device"):
         raise ValueError(f"sog must be 'host' or 'device', not {sog!r}")
     if sog_webp not in ("host", "device"):
@@ -114,6 +120,8 @@ def patch(verbose: bool = False, defer: bool = True, codebook: str = "sklearn", 
         raise ValueError("sog_reader_webp='device' needs sog_reader='device': the reference reader decodes on the host")
     if ply not in ("host", "device"):
         raise ValueError(f"ply must be 'host' or 'device', not {ply!r}")
+    if parquet not in ("host", "device"):
+        raise ValueError(f"parquet must be 'host' or 'device', not {parquet!r}")
     if require_cuda:
         from . import backend_available
         if not backend_available():
@@ -217,6 +225,16 @@ def patch(verbose: bool = False, defer: bool = True, codebook: str = "sklearn", 
             if hasattr(fmt, clsname):
                 gply.install_reader(getattr(fmt, clsname), flavor)   # ply_3dgs.py:8-60, ply_cc.py:8-62
                 gply.install(getattr(fmt, clsname), flavor)          # ply_3dgs.py:62-121, ply_cc.py:64-132
+    if parquet == "device":
+        fmt = sys.modules.get("gsconverter.formats.parquet")
+        if fmt is None:
+            try:
+                fmt = importlib.import_module("gsconverter.formats.parquet")
+            except Exception:  # noqa: BLE001  (pandas missing: nothing to patch there)
+                fmt = None
+        if fmt is not None and hasattr(fmt, "ParquetFormat"):
+            from . import parquet as gpq
+            gpq.install(fmt.ParquetFormat)                           # parquet.py:59-112
     if verbose:
         print("[gsx] gsconverter.processing patched: SOR / density / bbox / alpha / K-Means / compressed PLY packing "
               "run on libgsx.so")

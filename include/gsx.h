@@ -384,6 +384,60 @@ int gsx_deflate_emit(const uint8_t* data_dev, int64_t n, const int64_t* starts_d
                      int64_t ws_bytes, uint32_t* words_dev, int64_t nwords, unsigned long long* mismatches_dev,
                      void* stream);
 
+/* ---- Parquet writer on the device: ParquetFormat.write, formats/parquet.py:59-112 (gsx/parquet.py) ---------------
+ * n rows (n <= 2^31) of row_bytes bytes each (1 .. 1024); ncols columns (1 .. 1024).  Row group g is rows
+ * [g * 2^20, (g + 1) * 2^20), data page p rows [p * 2^18, (p + 1) * 2^18), tile t rows [t * 2048, (t + 1) * 2048).
+ * A value is null when its pattern is a float32 NaN; uint8 columns are widened and never null.  Every pointer but
+ * cols_host is a device pointer; every entry runs on `stream`.
+ * gsx_parquet_split (parquet.py:94-108, the frame's columns): cols_host int32 [ncols][2] = (byte offset in the row,
+ * kind: 0 float32, 1 uint8).  Writes out_dev uint32 [ncols][n] (column-major patterns), tile_nulls_dev uint32
+ * [ncols][tiles] and keys_dev uint32 [2][ncols][groups]: each chunk's least and greatest order-preserving key of its
+ * non-null values (float32: sign bit flipped for positives, all bits for negatives; uint8: the value), 0xFFFFFFFF and
+ * 0 for a chunk without one.
+ * gsx_parquet_dict_insert (pyarrow's dictionary encoding): the non-null patterns of row groups [g0, g0 + ng) into
+ * table_dev (uint64 [ng][ncols][2^slots_log2], zeroed by the caller, slots_log2 19 .. 24); distinct_dev uint32
+ * [ncols][groups] (zeroed) counts the distinct patterns of each chunk, exactly up to 262 144, and ends above it
+ * otherwise.
+ * gsx_parquet_dictionary: for jobs_dev int64 [njobs][3] = (table index c + ncols * (g - g0), first key, first
+ * dictionary value), njobs <= 65535, whose first keys leave room for each chunk's distinct count (nkeys in all):
+ * the chunk's patterns ascending to dict_vals_dev, and each one's rank into the table.  Workspace from
+ * gsx_parquet_dictionary_workspace_bytes(nkeys).
+ * gsx_parquet_dict_index: every non-null value of the chunks of row groups [g0, g0 + ng) with dict_chunk_dev[c][g - g0]
+ * != 0 replaced in cols_dev by its rank; page_idx_dev uint32 [2][ncols][pages] (0xFF.. and 0 filled by the caller)
+ * gets each page's least and greatest rank.
+ * gsx_parquet_pages: the page bodies into body_dev (uint32 words, zeroed by the caller).  info_dev int64
+ * [ncols][pages][4] = (body byte offset, 16-byte aligned; nulls; bit width, 0 for PLAIN; all ranks equal) of each data
+ * page; dict_jobs_dev int64 [ndict][3] = (first dictionary value, body offset, entries <= max_dict) of each
+ * dictionary page.  A data page is the 4-byte length and RLE / bit-packed hybrid of its definition levels (one RLE
+ * run, or one bit-packed run over its rows when it has nulls), then PLAIN values, or the bit width byte and the ranks
+ * as one bit-packed run (one RLE run when they are all equal; nothing when the page has no value).
+ * gsx_parquet_snappy: pieces_dev int64 [npieces][3] = (page, body offset (16-byte aligned), bytes 1 .. 65536).  Piece
+ * i's Snappy elements go to scratch_dev + i * gsx_parquet_piece_bytes(), their length to sizes_dev[i], and it is added
+ * to page_csize_dev[page] (zeroed by the caller).  Copies of distance 1 or 4 and length >= 8 inside the piece, taken
+ * greedily from the left (the longer one, distance 1 on a tie); literals elsewhere.
+ * gsx_parquet_assemble: the file: the pieces of each page back to back from page_dst_dev[page] (page_first_dev: its
+ * first piece), and hjobs_dev int64 [nh][3] = (offset in heads_dev, file offset, bytes) of the headers and footer. */
+int gsx_parquet_split(const uint8_t* rows_dev, int64_t n, int32_t row_bytes, const int32_t* cols_host, int32_t ncols,
+                      uint32_t* out_dev, uint32_t* tile_nulls_dev, uint32_t* keys_dev, void* stream);
+int gsx_parquet_dict_insert(const uint32_t* cols_dev, int64_t n, int32_t ncols, int32_t g0, int32_t ng,
+                            unsigned long long* table_dev, int32_t slots_log2, uint32_t* distinct_dev, void* stream);
+int64_t gsx_parquet_dictionary_workspace_bytes(int64_t nkeys);
+int gsx_parquet_dictionary(unsigned long long* table_dev, int32_t slots_log2, const int64_t* jobs_dev, int32_t njobs,
+                           int64_t nkeys, void* ws_dev, int64_t ws_bytes, uint32_t* dict_vals_dev, void* stream);
+int gsx_parquet_dict_index(uint32_t* cols_dev, int64_t n, int32_t ncols, int32_t g0, int32_t ng,
+                           const unsigned long long* table_dev, int32_t slots_log2, const int32_t* dict_chunk_dev,
+                           uint32_t* page_idx_dev, void* stream);
+int gsx_parquet_pages(const uint32_t* cols_dev, int64_t n, int32_t ncols, const uint32_t* tile_nulls_dev,
+                      const int64_t* info_dev, const uint32_t* dict_vals_dev, const int64_t* dict_jobs_dev,
+                      int32_t ndict, int64_t max_dict, uint32_t* body_dev, void* stream);
+int64_t gsx_parquet_piece_bytes(void);
+int gsx_parquet_snappy(const uint8_t* body_dev, const int64_t* pieces_dev, int64_t npieces, uint8_t* scratch_dev,
+                       uint32_t* sizes_dev, uint32_t* page_csize_dev, void* stream);
+int gsx_parquet_assemble(const uint8_t* scratch_dev, const int64_t* pieces_dev, int64_t npieces,
+                         const uint32_t* sizes_dev, const int64_t* page_first_dev, const int64_t* page_dst_dev,
+                         const uint8_t* heads_dev, const int64_t* hjobs_dev, int64_t nh, uint8_t* file_dev,
+                         void* stream);
+
 /* ---- K-Means: gpu_ops.py:57-96 (kernels) + :186-188 (Lloyd loop) ---------------------- */
 /* Batched over `nprob` independent problems stored back to back (SOG shN chunks, sog.py:527-549):
  * problem p has rows [row_off[p], row_off[p+1]) of X[*,D] and K centroids at C[p*K*D].
