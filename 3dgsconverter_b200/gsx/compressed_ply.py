@@ -138,24 +138,16 @@ def write_ply(path, chunk_data: np.ndarray, vertex_data: np.ndarray, sh_data: np
             fh.write(np.ascontiguousarray(a.astype(layout)).tobytes())
 
 
-def dropin_write(self, data: np.ndarray, path, **kwargs) -> None:
-    """Replacement for CompressedPlyFormat.write: packed-float32 records are encoded on the device and written by the
-    class's own _write_ply_file; anything gsx refuses or fails on goes to the original write (the CPU path)."""
+def prepare_write(self, data: np.ndarray, *args, **kwargs):
+    """CompressedPlyFormat.write(data, path, **kwargs) for gsx.dropin.install_writer: packed-float32 records encoded
+    on the device; returns the step that writes them with the class's own _write_ply_file."""
     from .records import DeviceRecords, is_packed_f32
-    try:
-        if not is_packed_f32(data):
-            raise ValueError("compressed PLY on the device needs packed all-float32 records")
-        chunk_data, vertex_data, sh_data = encode(DeviceRecords.from_structured(data)).to_host()
-    except Exception:  # noqa: BLE001  (the reference's convention: exception => CPU path)
-        return self._gsx_reference_write(data, path, **kwargs)
-    self._write_ply_file(path, chunk_data, vertex_data, sh_data)
-
-
-def install(cls) -> None:
-    """Make cls.write the device writer, keeping the original as cls._gsx_reference_write (idempotent)."""
-    if "_gsx_reference_write" not in cls.__dict__:
-        cls._gsx_reference_write = cls.write
-        cls.write = dropin_write
+    if args:
+        raise TypeError("CompressedPlyFormat.write takes no positional arguments after path")
+    if not is_packed_f32(data):
+        raise ValueError("compressed PLY on the device needs packed all-float32 records")
+    chunk_data, vertex_data, sh_data = encode(DeviceRecords.from_structured(data)).to_host()
+    return lambda path: self._write_ply_file(path, chunk_data, vertex_data, sh_data)
 
 
 FIXED_FIELDS = ("x", "y", "z", "nx", "ny", "nz", "f_dc_0", "f_dc_1", "f_dc_2", "opacity", "scale_0", "scale_1",
@@ -242,9 +234,3 @@ def decode(data, device="cuda"):
                                   C.c_void_p(base + sh.offset) if names else None, sh.dtype.itemsize if names else 0,
                                   i32(soffs), len(names), _ptr(tabs), _ptr(rows), _stream()), "gsx_cply_decode")
     return readers.Decoded(rows, dtype, metadata)
-
-
-def install_reader(cls) -> None:
-    """Make cls.read the device reader, keeping the original as cls._gsx_reference_read (idempotent)."""
-    from . import readers
-    readers.install(cls, decode)

@@ -7,31 +7,25 @@ formats/sog.py:11 import from there):
   * ``gpu_ops.kmeans``, ``gpu_ops.filter_sor_gpu``, ``gpu_ops.HAS_TAICHI``
   * the ``DataProcessor`` class (same public surface; the filters run on libgsx and keep their
     working set in HBM; ``defer=True`` gathers the host records once, when ``.data`` is read)
-and, when ``gsconverter.formats.compressed_ply`` imports, ``CompressedPlyFormat.write`` (Morton order, chunk bounds
-and packing on the device, the file still written by the class's own ``_write_ply_file``; records gsx refuses go to
-the original ``write``).  With ``patch(sog="device")`` also ``SogFormat.write`` (gsx.sog.encode: every texture,
-codebook and the chunked SH palette built on the device; opt-in because its position bytes can differ from NumPy's
-log by one count on a small fraction of the splats); ``patch(sog="device", sog_webp="device")`` also encodes its
-WebP members on the device (gsx.webp: lossless VP8L that decodes to the same pixels, in gsx's bytes, not libwebp's).
-With ``patch(codecs="device")`` also ``SplatFormat.write``,
-``KSplatFormat.write`` and ``SpzFormat.write`` (gsx.splat / gsx.ksplat / gsx.spz: sort, bucket bounds and packing on the
-device, gzip and the file on the host; records gsx refuses go to the original ``write``);
-``patch(codecs="device", spz_gzip="device")`` also gzips the .spz payload on the device (gsx.deflate: a file that
-decompresses to the same payload, in gsx's bytes, not zlib's).  With
-``patch(readers="device")`` also the ``read`` of ``SplatFormat``, ``KSplatFormat``, ``SpzFormat`` and
-``CompressedPlyFormat`` (gsx.splat / gsx.ksplat / gsx.spz / gsx.compressed_ply ``decode``: headers and gunzip on the
-host, every splat decoded on the device, byte for byte as the reference readers; files gsx refuses go to the original
-``read``).  With ``patch(sog_reader="device")`` also ``SogFormat.read`` (gsx.sog_reader.decode: ZIP, meta.json and
-WebP on the host, the shN palette and every splat decoded on the device, byte for byte as the reference reader, its
-palette indexing included; bundles gsx refuses go to the original ``read``); ``patch(sog_reader="device",
-sog_reader_webp="device")`` also decodes the lossless WebP members on the device (gsx.webp_decode), so only their
-compressed bytes cross PCIe.  With ``patch(ply="device")`` also the
-``read`` and ``write`` of ``Ply3DGSFormat`` and ``PlyCCFormat`` (gsx.ply: header and field mapping on the host, the rows
-transcoded on the device, byte for byte as the reference; files and records gsx refuses, and writes with
-``extra_elements``, go to the original method).  With ``patch(parquet="device")`` also ``ParquetFormat.write``
-(gsx.parquet: columns, statistics, dictionaries, pages and Snappy built on the device; a file that pyarrow and pandas
-read as the same table, in gsx's bytes, not pyarrow's; records gsx refuses go to the original ``write``).  The parquet
-reader stays on the host.
+and installs gsx's device readers and writers on the reference's format classes:
+
+  =======================  =====================  ==========================================================
+  class                    read / write keyword   gsx
+  =======================  =====================  ==========================================================
+  ``SplatFormat``          readers / codecs       gsx.splat ``decode`` / ``prepare_write``
+  ``KSplatFormat``         readers / codecs       gsx.ksplat
+  ``SpzFormat``            readers / codecs       gsx.spz (``spz_gzip="device"``: gzip with gsx.deflate)
+  ``CompressedPlyFormat``  readers / always       gsx.compressed_ply
+  ``SogFormat``            sog_reader / sog       gsx.sog_reader / gsx.sog (``sog_reader_webp`` / ``sog_webp``)
+  ``Ply3DGSFormat``        ply / ply              gsx.ply, flavour "3dgs"
+  ``PlyCCFormat``          ply / ply              gsx.ply, flavour "cc"
+  ``ParquetFormat``        -- / parquet           gsx.parquet (the reader stays on the host)
+  =======================  =====================  ==========================================================
+
+Each installed method (install_reader / install_writer) keeps the original as ``_gsx_reference_read`` /
+``_gsx_reference_write``.  It runs gsx's device path, and anything gsx refuses or fails on goes to the original method
+with the original arguments and the global NumPy RNG as it was on entry.  The compressed PLY writer is installed
+whatever the keywords; every other class only with its keyword set to "device".
 Host-only helpers and everything else of the reference stay as they are.
 """
 from __future__ import annotations
@@ -41,14 +35,9 @@ import importlib.util
 import sys
 from pathlib import Path
 
+import numpy as np
+
 _HERE = Path(__file__).resolve().parent.parent
-
-
-def _load_ours(modname: str, relpath: str):
-    spec = importlib.util.spec_from_file_location(modname, _HERE / relpath,
-                                                  submodule_search_locations=None)
-    mod = importlib.util.module_from_spec(spec)
-    return spec, mod
 
 
 class _GsxCodebookKMeans:
@@ -69,6 +58,97 @@ class _GsxCodebookKMeans:
         C, L = _km.kmeans_host(x, k, self.max_iter, init)
         self.cluster_centers_, self.labels_ = C, L
         return self
+
+
+def _install(cls, method: str, wrapper, options: dict) -> None:
+    """cls.<method> = wrapper, the original kept once as cls._gsx_reference_<method>; options always replaced."""
+    ref = f"_gsx_reference_{method}"
+    if ref not in cls.__dict__:
+        setattr(cls, ref, getattr(cls, method))
+        setattr(cls, method, wrapper)
+    cls._gsx_options = {**cls.__dict__.get("_gsx_options", {}), method: options}
+
+
+def install_writer(cls, prepare, **options) -> None:
+    """Make cls.write the device writer `prepare`, keeping the original as cls._gsx_reference_write; installing again
+    changes only the options.  prepare(self, data, *args, **kwargs) does all the device work and all the refusing, and
+    returns finish(path), which writes the file.  Anything prepare raises sends the call to the original write with the
+    original arguments and the global NumPy RNG as it was on entry; an error writing the file propagates.  prepare
+    reads `options` at call time as self._gsx_options["write"]."""
+    def write(self, data, path, *args, **kwargs):
+        state = np.random.get_state()
+        try:
+            finish = prepare(self, data, *args, **kwargs)
+        except Exception:  # noqa: BLE001  (the reference's convention: exception => CPU path)
+            np.random.set_state(state)
+            return self._gsx_reference_write(data, path, *args, **kwargs)
+        finish(path)
+
+    _install(cls, "write", write, options)
+
+
+def install_reader(cls, decode, after=None, **options) -> None:
+    """Make cls.read the device reader `decode`, keeping the original as cls._gsx_reference_read; installing again
+    changes only the options.  read(path) returns decode(path, **options).to_host(), with options read at call time,
+    sets self.metadata when the decode has metadata, then runs after(self) if given.  Anything the decode raises sends
+    the call to the original read with the original arguments and the global NumPy RNG as it was on entry."""
+    def read(self, path, *args, **kwargs):
+        state = np.random.get_state()
+        try:
+            dec = decode(path, **self._gsx_options["read"])
+            out = dec.to_host()
+        except Exception:  # noqa: BLE001  (the reference's convention: exception => CPU path)
+            np.random.set_state(state)
+            return self._gsx_reference_read(path, *args, **kwargs)
+        if dec.metadata is not None:
+            self.metadata = dec.metadata
+        if after is not None:
+            after(self)
+        return out
+
+    _install(cls, "read", read, options)
+
+
+def _vertex_only(self) -> None:
+    """What BaseFormat.__init__ leaves in extra_elements after reading a vertex-only PLY."""
+    self.extra_elements = []
+
+
+def _formats(kw: dict):
+    """One row per reference class: (gsconverter.formats module, class, reader, writer).  Reader and writer are each
+    None (left to the reference) or (the patch keyword that turns it on, None for always; the gsx function; the
+    install options), the options taken from the patch keywords in `kw`."""
+    from . import compressed_ply, ksplat, parquet, ply, sog, sog_reader, splat, spz
+    return (
+        ("splat", "SplatFormat", ("readers", splat.decode, {}), ("codecs", splat.prepare_write, {})),
+        ("ksplat", "KSplatFormat", ("readers", ksplat.decode, {}), ("codecs", ksplat.prepare_write, {})),
+        ("spz", "SpzFormat", ("readers", spz.decode, {}), ("codecs", spz.prepare_write, {"gzip": kw["spz_gzip"]})),
+        ("compressed_ply", "CompressedPlyFormat", ("readers", compressed_ply.decode, {}),
+         (None, compressed_ply.prepare_write, {})),
+        ("sog", "SogFormat", ("sog_reader", sog_reader.decode, {"webp": kw["sog_reader_webp"]}),
+         ("sog", sog.prepare_write, {"webp": kw["sog_webp"]})),
+        ("ply_3dgs", "Ply3DGSFormat", ("ply", ply.decode, {"flavor": "3dgs", "after": _vertex_only}),
+         ("ply", ply.prepare_write, {"flavor": "3dgs"})),
+        ("ply_cc", "PlyCCFormat", ("ply", ply.decode, {"flavor": "cc", "after": _vertex_only}),
+         ("ply", ply.prepare_write, {"flavor": "cc"})),
+        ("parquet", "ParquetFormat", None, ("parquet", parquet.prepare_write, {})),
+    )
+
+
+# "X='device' needs Y='device'": the reference's own method has nothing on the device for X to work on
+_NEEDS = (("sog_webp", "sog", "the reference writer has no device textures to encode"),
+          ("spz_gzip", "codecs", "the reference writer has no device payload to gzip"),
+          ("sog_reader_webp", "sog_reader", "the reference reader decodes on the host"))
+
+
+def _format_class(module: str, name: str):
+    """gsconverter.formats.<module>.<name>, or None when the module does not import (its optional dependency, such as
+    plyfile, pandas or Pillow, is missing) or has no such class."""
+    try:
+        mod = importlib.import_module(f"gsconverter.formats.{module}")
+    except Exception:  # noqa: BLE001  (nothing to patch there)
+        return None
+    return getattr(mod, name, None)
 
 
 def patch(verbose: bool = False, defer: bool = True, codebook: str = "sklearn", require_cuda: bool = True,
@@ -98,30 +178,14 @@ def patch(verbose: bool = False, defer: bool = True, codebook: str = "sklearn", 
     parquet: "host" keeps the reference's ParquetFormat.write (pandas and pyarrow); "device" installs gsx.parquet's
     device writer on it (records gsx refuses go to the original write).  The file then holds gsx's bytes, the same
     table pyarrow writes, so this chooses the output, not only the speed."""
-    if sog not in ("host", "device"):
-        raise ValueError(f"sog must be 'host' or 'device', not {sog!r}")
-    if sog_webp not in ("host", "device"):
-        raise ValueError(f"sog_webp must be 'host' or 'device', not {sog_webp!r}")
-    if sog_webp == "device" and sog != "device":
-        raise ValueError("sog_webp='device' needs sog='device': the reference writer has no device textures to encode")
-    if codecs not in ("host", "device"):
-        raise ValueError(f"codecs must be 'host' or 'device', not {codecs!r}")
-    if spz_gzip not in ("host", "device"):
-        raise ValueError(f"spz_gzip must be 'host' or 'device', not {spz_gzip!r}")
-    if spz_gzip == "device" and codecs != "device":
-        raise ValueError("spz_gzip='device' needs codecs='device': the reference writer has no device payload to gzip")
-    if readers not in ("host", "device"):
-        raise ValueError(f"readers must be 'host' or 'device', not {readers!r}")
-    if sog_reader not in ("host", "device"):
-        raise ValueError(f"sog_reader must be 'host' or 'device', not {sog_reader!r}")
-    if sog_reader_webp not in ("host", "device"):
-        raise ValueError(f"sog_reader_webp must be 'host' or 'device', not {sog_reader_webp!r}")
-    if sog_reader_webp == "device" and sog_reader != "device":
-        raise ValueError("sog_reader_webp='device' needs sog_reader='device': the reference reader decodes on the host")
-    if ply not in ("host", "device"):
-        raise ValueError(f"ply must be 'host' or 'device', not {ply!r}")
-    if parquet not in ("host", "device"):
-        raise ValueError(f"parquet must be 'host' or 'device', not {parquet!r}")
+    kw = dict(sog=sog, codecs=codecs, readers=readers, sog_reader=sog_reader, ply=ply, sog_webp=sog_webp,
+              spz_gzip=spz_gzip, sog_reader_webp=sog_reader_webp, parquet=parquet)
+    for name, value in kw.items():
+        if value not in ("host", "device"):
+            raise ValueError(f"{name} must be 'host' or 'device', not {value!r}")
+    for name, needs, why in _NEEDS:
+        if kw[name] == "device" and kw[needs] != "device":
+            raise ValueError(f"{name}='device' needs {needs}='device': {why}")
     if require_cuda:
         from . import backend_available
         if not backend_available():
@@ -161,80 +225,15 @@ def patch(verbose: bool = False, defer: bool = True, codebook: str = "sklearn", 
     if conv is not None and hasattr(conv, "DataProcessor"):
         conv.DataProcessor = Ours
     ref_gpu_ops._gsx_module = g     # batch-ahead statistics: gpu_ops._gsx_module.batch_stats
-    sog_mod = sys.modules.get("gsconverter.formats.sog")
-    if sog_mod is None:
-        try:
-            sog_mod = importlib.import_module("gsconverter.formats.sog")
-        except Exception:  # noqa: BLE001  (optional dependency of the writer missing: nothing to patch there)
-            sog_mod = None
-    if sog_mod is not None and codebook == "gpu" and hasattr(sog_mod, "MiniBatchKMeans"):
-        sog_mod.MiniBatchKMeans = _GsxCodebookKMeans  # sog.py:561 -> exact 1-D Lloyd on the GPU
-    if sog_mod is not None and sog == "device" and hasattr(sog_mod, "SogFormat"):
-        from .sog import install as install_sog
-        install_sog(sog_mod.SogFormat, webp=sog_webp)  # sog.py:249-639 -> textures and palette on the GPU
-    if sog_mod is not None and sog_reader == "device" and hasattr(sog_mod, "SogFormat"):
-        from .sog_reader import install_reader as install_sog_reader
-        install_sog_reader(sog_mod.SogFormat, webp=sog_reader_webp)   # sog.py:23-247 -> palette and rows on the GPU
-    cply = sys.modules.get("gsconverter.formats.compressed_ply")
-    if cply is None:
-        try:
-            cply = importlib.import_module("gsconverter.formats.compressed_ply")
-        except Exception:  # noqa: BLE001  (writer not importable: nothing to patch there)
-            cply = None
-    if cply is not None and hasattr(cply, "CompressedPlyFormat"):
-        from .compressed_ply import install
-        install(cply.CompressedPlyFormat)             # compressed_ply.py:126-250 -> packing on the GPU
-    if codecs == "device":
-        from . import ksplat, splat, spz
-        for modname, clsname, ours in (("splat", "SplatFormat", splat), ("ksplat", "KSplatFormat", ksplat),
-                                       ("spz", "SpzFormat", spz)):
-            fmt = sys.modules.get(f"gsconverter.formats.{modname}")
-            if fmt is None:
-                try:
-                    fmt = importlib.import_module(f"gsconverter.formats.{modname}")
-                except Exception:  # noqa: BLE001  (writer not importable: nothing to patch there)
-                    continue
-            if hasattr(fmt, clsname):                 # splat.py:82-166, ksplat.py:319-544, spz.py:49-173
-                if ours is spz:
-                    ours.install(getattr(fmt, clsname), where=spz_gzip)
-                else:
-                    ours.install(getattr(fmt, clsname))
-    if readers == "device":
-        from . import compressed_ply, ksplat, splat, spz
-        for modname, clsname, ours in (("splat", "SplatFormat", splat), ("ksplat", "KSplatFormat", ksplat),
-                                       ("spz", "SpzFormat", spz), ("compressed_ply", "CompressedPlyFormat",
-                                                                   compressed_ply)):
-            fmt = sys.modules.get(f"gsconverter.formats.{modname}")
-            if fmt is None:
-                try:
-                    fmt = importlib.import_module(f"gsconverter.formats.{modname}")
-                except Exception:  # noqa: BLE001  (reader not importable: nothing to patch there)
-                    continue
-            if hasattr(fmt, clsname):
-                ours.install_reader(getattr(fmt, clsname))   # splat.py:9-80, ksplat.py:29-317, spz.py:18-296,
-                #                                               compressed_ply.py:14-123
-    if ply == "device":
-        from . import ply as gply
-        for modname, clsname, flavor in (("ply_3dgs", "Ply3DGSFormat", "3dgs"), ("ply_cc", "PlyCCFormat", "cc")):
-            fmt = sys.modules.get(f"gsconverter.formats.{modname}")
-            if fmt is None:
-                try:
-                    fmt = importlib.import_module(f"gsconverter.formats.{modname}")
-                except Exception:  # noqa: BLE001  (plyfile missing: nothing to patch there)
-                    continue
-            if hasattr(fmt, clsname):
-                gply.install_reader(getattr(fmt, clsname), flavor)   # ply_3dgs.py:8-60, ply_cc.py:8-62
-                gply.install(getattr(fmt, clsname), flavor)          # ply_3dgs.py:62-121, ply_cc.py:64-132
-    if parquet == "device":
-        fmt = sys.modules.get("gsconverter.formats.parquet")
-        if fmt is None:
-            try:
-                fmt = importlib.import_module("gsconverter.formats.parquet")
-            except Exception:  # noqa: BLE001  (pandas missing: nothing to patch there)
-                fmt = None
-        if fmt is not None and hasattr(fmt, "ParquetFormat"):
-            from . import parquet as gpq
-            gpq.install(fmt.ParquetFormat)                           # parquet.py:59-112
+    if codebook == "gpu" and _format_class("sog", "MiniBatchKMeans") is not None:
+        sys.modules["gsconverter.formats.sog"].MiniBatchKMeans = _GsxCodebookKMeans  # sog.py:561 -> 1-D Lloyd on the GPU
+    for module, name, *sides in _formats(kw):
+        for install, side in zip((install_reader, install_writer), sides):
+            if side is None or (side[0] is not None and kw[side[0]] != "device"):
+                continue
+            cls = _format_class(module, name)
+            if cls is not None:
+                install(cls, side[1], **side[2])
     if verbose:
         print("[gsx] gsconverter.processing patched: SOR / density / bbox / alpha / K-Means / compressed PLY packing "
               "run on libgsx.so")

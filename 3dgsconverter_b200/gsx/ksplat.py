@@ -13,6 +13,7 @@ from __future__ import annotations
 import ctypes as C
 import struct
 from dataclasses import dataclass
+from pathlib import Path
 
 import numpy as np
 import torch
@@ -114,26 +115,14 @@ def write_ksplat(path, enc: KSplat) -> None:
         fh.write(enc.to_host())
 
 
-def dropin_write(self, data: np.ndarray, path, *args, **kwargs) -> None:
-    """Replacement for KSplatFormat.write(data, path, compression_level=0, **kwargs): the file is packed on the
-    device; anything gsx refuses or fails on goes to the original write with the original arguments."""
+def prepare_write(self, data: np.ndarray, *args, **kwargs):
+    """KSplatFormat.write(data, path, compression_level=0, **kwargs) for gsx.dropin.install_writer: the file's bytes,
+    packed on the device; returns the step that writes them to path."""
     from .records import DeviceRecords
-    try:
-        level = args[0] if args else kwargs.get("compression_level", 0)
-        enc = encode(DeviceRecords.from_writer_input(data), level, kwargs.get("sh_level"), kwargs.get("bucket_size"),
-                     kwargs.get("block_size"))
-        blob = enc.to_host()
-    except Exception:  # noqa: BLE001  (the reference's convention: exception => CPU path)
-        return self._gsx_reference_write(data, path, *args, **kwargs)
-    with open(path, "wb") as fh:
-        fh.write(blob)
-
-
-def install(cls) -> None:
-    """Make cls.write the device writer, keeping the original as cls._gsx_reference_write (idempotent)."""
-    if "_gsx_reference_write" not in cls.__dict__:
-        cls._gsx_reference_write = cls.write
-        cls.write = dropin_write
+    level = args[0] if args else kwargs.get("compression_level", 0)
+    blob = encode(DeviceRecords.from_writer_input(data), level, kwargs.get("sh_level"), kwargs.get("bucket_size"),
+                  kwargs.get("block_size")).to_host()
+    return lambda path: Path(path).write_bytes(blob)
 
 
 def read_tables():
@@ -228,8 +217,3 @@ def decode(data, device="cuda") -> readers.Decoded:
                 _ptr(rows[row:row + n]), _stream()), "gsx_ksplat_decode_section")
             row += n
     return readers.Decoded(rows, dtype, metadata)
-
-
-def install_reader(cls) -> None:
-    """Make cls.read the device reader, keeping the original as cls._gsx_reference_read (idempotent)."""
-    readers.install(cls, decode)

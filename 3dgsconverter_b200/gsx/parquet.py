@@ -514,23 +514,18 @@ def write_parquet(path, enc: Encoded) -> None:
         fh.write(enc.to_host())
 
 
-def dropin_write(self, data, path, **kwargs) -> None:
-    """Replacement for ParquetFormat.write: the file is built on the device and written, then the reference's status
-    line is printed; anything gsx refuses or fails on goes to the original write with the original arguments."""
+def prepare_write(self, data, *args, **kwargs):
+    """ParquetFormat.write(data, path, **kwargs) for gsx.dropin.install_writer: the file built on the device; returns
+    the step that writes it to path and then prints the reference's status line."""
     import sys
-    try:
-        enc = encode(data)
-        blob = enc.to_host()
-    except Exception:  # noqa: BLE001  (the reference's convention: exception => CPU path)
-        return self._gsx_reference_write(data, path, **kwargs)
-    with open(path, "wb") as fh:
-        fh.write(blob)
-    status = getattr(sys.modules.get(type(self).__module__), "status_print", print)
-    status(f"Parquet write completed. {enc.rows} rows.")
+    if args:
+        raise TypeError("ParquetFormat.write takes no positional arguments after path")
+    enc = encode(data)
+    blob = enc.to_host()
 
-
-def install(cls) -> None:
-    """Make cls.write the device writer, keeping the original as cls._gsx_reference_write (idempotent)."""
-    if "_gsx_reference_write" not in cls.__dict__:
-        cls._gsx_reference_write = cls.write
-        cls.write = dropin_write
+    def finish(path):
+        with open(path, "wb") as fh:
+            fh.write(blob)
+        status = getattr(sys.modules.get(type(self).__module__), "status_print", print)
+        status(f"Parquet write completed. {enc.rows} rows.")
+    return finish

@@ -282,45 +282,13 @@ def write_ply(path, enc: Encoded) -> None:
         fh.write(memoryview(body).cast("B"))
 
 
-# ---------------------------------------------------------------------------------------------------------- drop-in
-def install_reader(cls, flavor: str) -> None:
-    """Make cls.read the device reader of `flavor`, keeping the original as cls._gsx_reference_read (idempotent)."""
-    _check_flavor(flavor)
-    if "_gsx_reference_read" in cls.__dict__:
-        return
-
-    def read(self, path, *args, **kwargs):
-        """Device replacement of the reference's read: decode(path).to_host(), and extra_elements = [] as
-        BaseFormat.__init__ leaves it for a vertex-only file; anything gsx refuses or fails on goes to the original
-        read with the original arguments."""
-        try:
-            out = decode(path, flavor).to_host()
-        except Exception:  # noqa: BLE001  (the reference's convention: exception => CPU path)
-            return self._gsx_reference_read(path, *args, **kwargs)
-        self.extra_elements = []
-        return out
-
-    cls._gsx_reference_read = cls.read
-    cls.read = read
-
-
-def install(cls, flavor: str) -> None:
-    """Make cls.write the device writer of `flavor`, keeping the original as cls._gsx_reference_write (idempotent)."""
-    _check_flavor(flavor)
-    if "_gsx_reference_write" in cls.__dict__:
-        return
-
-    def write(self, data, path, *args, **kwargs):
-        """Device replacement of the reference's write: encode(data, crop_sh=...) and write_ply.  A non-empty
-        extra_elements, extra positional arguments, and anything gsx refuses or fails on go to the original write with
-        the original arguments."""
-        if args or kwargs.get("extra_elements"):
-            return self._gsx_reference_write(data, path, *args, **kwargs)
-        try:
-            enc = encode(data, flavor, crop_sh=kwargs.get("crop_sh", False))
-        except Exception:  # noqa: BLE001  (the reference's convention: exception => CPU path)
-            return self._gsx_reference_write(data, path, *args, **kwargs)
-        write_ply(path, enc)
-
-    cls._gsx_reference_write = cls.write
-    cls.write = write
+def prepare_write(self, data, *args, **kwargs):
+    """Ply3DGSFormat.write / PlyCCFormat.write (data, path, **kwargs) for gsx.dropin.install_writer, in the install
+    option flavor: encode(data, crop_sh=...); returns the step that writes the file with write_ply.  Positional
+    arguments and a non-empty extra_elements are refused, so the reference's write handles them."""
+    if args:
+        raise TypeError("PLY write on the device takes no positional arguments after path")
+    if kwargs.get("extra_elements"):
+        raise ValueError("PLY write on the device writes no extra_elements")
+    enc = encode(data, self._gsx_options["write"]["flavor"], crop_sh=kwargs.get("crop_sh", False))
+    return lambda path: write_ply(path, enc)

@@ -1,6 +1,6 @@
 """What the device readers share (gsx.splat / gsx.ksplat / gsx.spz / gsx.compressed_ply `decode`): the file's bytes,
-uploaded once; the reference's output dtype (structures.py:23-59); the result object; the drop-in `read`; and the
-binary little-endian PLY header parser of the compressed PLY reader.
+uploaded once; the reference's output dtype (structures.py:23-59); the result object; and the binary little-endian PLY
+header parser of the compressed PLY reader.
 
     dec = gsx.ksplat.decode("in.ksplat")     # Decoded: rows (uint8 [n, itemsize] on the device), dtype, metadata
     a = dec.to_host()                        # what KSplatFormat.read returns, byte for byte
@@ -72,27 +72,6 @@ class Decoded:
             rows = self.rows.view(torch.float32).view(len(self), len(self.dtype.names))
             return DeviceRecords(rows, self.dtype.names, self.dtype)
         return DeviceRecords.from_device_bytes(self.rows, self.dtype)
-
-
-def install(cls, decode) -> None:
-    """Make cls.read the device reader `decode`, keeping the original as cls._gsx_reference_read (idempotent)."""
-    if "_gsx_reference_read" in cls.__dict__:
-        return
-
-    def read(self, path, *args, **kwargs):
-        """Device replacement of the reference's read: decode(path).to_host(), self.metadata set as the reference sets
-        it; anything gsx refuses or fails on goes to the original read with the original arguments."""
-        try:
-            dec = decode(path)
-            out = dec.to_host()
-        except Exception:  # noqa: BLE001  (the reference's convention: exception => CPU path)
-            return self._gsx_reference_read(path, *args, **kwargs)
-        if dec.metadata is not None:
-            self.metadata = dec.metadata
-        return out
-
-    cls._gsx_reference_read = cls.read
-    cls.read = read
 
 
 # ---------------------------------------------------------------------------------------------- binary PLY header

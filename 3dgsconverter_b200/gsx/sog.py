@@ -441,31 +441,17 @@ def _module_codebook_fit(cls):
     return fit
 
 
-def dropin_write(self, data: np.ndarray, path, **kwargs) -> None:
-    """Replacement for SogFormat.write: packed-float32 records are encoded on the device and bundled by write_sog
-    (its WebP members by Pillow, or by gsx.webp from HBM when the class was installed with webp="device");
-    anything gsx refuses or fails on goes to the original write with the global NumPy RNG as it was on entry."""
+def prepare_write(self, data: np.ndarray, *args, **kwargs):
+    """SogFormat.write(data, path, **kwargs) for gsx.dropin.install_writer: packed-float32 records encoded on the
+    device; returns the step that bundles them with write_sog, its WebP members by Pillow (install option webp="host",
+    libwebp's bytes) or by gsx.webp from HBM (webp="device")."""
     from .records import DeviceRecords, is_packed_f32
-    state = np.random.get_state()
-    try:
-        if not is_packed_f32(data):
-            raise ValueError("SOG on the device needs packed all-float32 records")
-        import PIL.Image  # noqa: F401  (the reference refuses without Pillow)
-        tex = encode(DeviceRecords.from_structured(data), kwargs.get("compression_level", 0),
-                     codebook_fit=_module_codebook_fit(type(self)))
-        textures = tex if getattr(type(self), "_gsx_sog_webp", "host") == "device" else tex.to_host()
-    except Exception:  # noqa: BLE001  (the reference's convention: exception => CPU path)
-        np.random.set_state(state)
-        return self._gsx_reference_write(data, path, **kwargs)
-    write_sog(path, textures, tex.meta)
-
-
-def install(cls, webp: str = "host") -> None:
-    """Make cls.write the device writer, keeping the original as cls._gsx_reference_write (idempotent).
-    webp: "host" bundles the members through Pillow (libwebp's bytes); "device" encodes them with gsx.webp."""
-    if webp not in ("host", "device"):
-        raise ValueError(f"webp must be 'host' or 'device', not {webp!r}")
-    if "_gsx_reference_write" not in cls.__dict__:
-        cls._gsx_reference_write = cls.write
-        cls.write = dropin_write
-    cls._gsx_sog_webp = webp
+    if args:
+        raise TypeError("SogFormat.write takes no positional arguments after path")
+    if not is_packed_f32(data):
+        raise ValueError("SOG on the device needs packed all-float32 records")
+    import PIL.Image  # noqa: F401  (the reference refuses without Pillow)
+    tex = encode(DeviceRecords.from_structured(data), kwargs.get("compression_level", 0),
+                 codebook_fit=_module_codebook_fit(type(self)))
+    textures = tex if self._gsx_options["write"]["webp"] == "device" else tex.to_host()
+    return lambda path: write_sog(path, textures, tex.meta)

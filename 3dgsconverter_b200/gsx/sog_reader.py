@@ -353,12 +353,3 @@ def decode_textures(pixels: dict, meta) -> readers.Decoded:
         raise ValueError("SOG: the reference raises IndexError here: " +
                          ", ".join(msg for b, msg in _ERRORS.items() if bits & b))
     return readers.Decoded(rows, dtype, None)
-
-
-def install_reader(cls, webp: str = "host") -> None:
-    """Make cls.read the device reader, keeping the original as cls._gsx_reference_read (idempotent).  webp: where the
-    WebP members are decoded (see decode)."""
-    if webp not in ("host", "device"):
-        raise ValueError(f"webp must be 'host' or 'device', not {webp!r}")
-    cls._gsx_sog_reader_webp = webp            # read at every call, so a later install changes it
-    readers.install(cls, lambda path: decode(path, webp=getattr(cls, "_gsx_sog_reader_webp", "host")))

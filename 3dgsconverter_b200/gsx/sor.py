@@ -158,7 +158,7 @@ def sor_filter_host(data_np: np.ndarray, k: int = 25, threshold_factor: float = 
     return (mask, means) if return_means else mask
 
 
-# ------------------------------------------------------------------ cKDTree semantics (the reference's CPU path)
+# ---------------------------------------------------------------- cKDTree semantics (the reference's SciPy path)
 def ckdtree_mean_dists(xyz: torch.Tensor, k: int) -> torch.Tensor:
     """data_processor.py:160-173 on device: exact (k+1)-NN in float64, mean of neighbours 1..k -> float32."""
     _check_xyz(xyz)

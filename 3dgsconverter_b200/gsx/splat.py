@@ -12,6 +12,7 @@ from __future__ import annotations
 
 import ctypes as C
 from dataclasses import dataclass
+from pathlib import Path
 
 import numpy as np
 import torch
@@ -57,23 +58,14 @@ def write_splat(path, enc: Splat) -> None:
         fh.write(enc.to_host())
 
 
-def dropin_write(self, data: np.ndarray, path, **kwargs) -> None:
-    """Replacement for SplatFormat.write: sorted and packed on the device; anything gsx refuses or fails on goes to the
-    original write with the original arguments."""
+def prepare_write(self, data: np.ndarray, *args, **kwargs):
+    """SplatFormat.write(data, path, **kwargs) for gsx.dropin.install_writer: the file's bytes, sorted and packed on
+    the device; returns the step that writes them to path."""
     from .records import DeviceRecords
-    try:
-        blob = encode(DeviceRecords.from_writer_input(data)).to_host()
-    except Exception:  # noqa: BLE001  (the reference's convention: exception => CPU path)
-        return self._gsx_reference_write(data, path, **kwargs)
-    with open(path, "wb") as fh:
-        fh.write(blob)
-
-
-def install(cls) -> None:
-    """Make cls.write the device writer, keeping the original as cls._gsx_reference_write (idempotent)."""
-    if "_gsx_reference_write" not in cls.__dict__:
-        cls._gsx_reference_write = cls.write
-        cls.write = dropin_write
+    if args:
+        raise TypeError("SplatFormat.write takes no positional arguments after path")
+    blob = encode(DeviceRecords.from_writer_input(data)).to_host()
+    return lambda path: Path(path).write_bytes(blob)
 
 
 def read_tables():
@@ -96,8 +88,3 @@ def decode(data, device="cuda") -> readers.Decoded:
     with torch.cuda.device(raw.device):
         check(lib.gsx_splat_decode(_ptr(raw), n, _ptr(tabs), _ptr(rows), _stream()), "gsx_splat_decode")
     return readers.Decoded(rows, dtype, None)
-
-
-def install_reader(cls) -> None:
-    """Make cls.read the device reader, keeping the original as cls._gsx_reference_read (idempotent)."""
-    readers.install(cls, decode)

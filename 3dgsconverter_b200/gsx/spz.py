@@ -16,6 +16,7 @@ import ctypes as C
 import gzip
 import struct
 from dataclasses import dataclass
+from pathlib import Path
 
 import numpy as np
 import torch
@@ -105,32 +106,20 @@ def write_spz(path, enc: Spz, compression_level=0, where: str = "host") -> None:
         fh.write(blob)
 
 
-def dropin_write(self, data: np.ndarray, path, **kwargs) -> None:
-    """Replacement for SpzFormat.write: the payload is packed on the device and gzipped on the host (or on the device
-    when installed with where="device"); anything gsx refuses or fails on goes to the original write with the
-    original arguments."""
+def prepare_write(self, data: np.ndarray, *args, **kwargs):
+    """SpzFormat.write(data, path, **kwargs) for gsx.dropin.install_writer: the payload packed on the device and
+    gzipped where the install option gzip says ("host": gzip.compress, the reference's bytes; "device": gsx.deflate);
+    returns the step that writes the file to path."""
     from .records import DeviceRecords
-    try:
-        enc = encode(DeviceRecords.from_writer_input(data))
-        level = kwargs.get("compression_level", 0)
-        if getattr(self, "_gsx_spz_gzip", "host") == "device":
-            blob = enc.compress(level)
-        else:
-            blob = gzip.compress(enc.to_host(), compresslevel=level)
-    except Exception:  # noqa: BLE001  (the reference's convention: exception => CPU path)
-        return self._gsx_reference_write(data, path, **kwargs)
-    with open(path, "wb") as fh:
-        fh.write(blob)
-
-
-def install(cls, where: str = "host") -> None:
-    """Make cls.write the device writer, keeping the original as cls._gsx_reference_write (idempotent).
-    where: "host" gzips with gzip.compress (the reference's bytes); "device" with gsx.deflate."""
-    _where(where)
-    if "_gsx_reference_write" not in cls.__dict__:
-        cls._gsx_reference_write = cls.write
-        cls.write = dropin_write
-    cls._gsx_spz_gzip = where
+    if args:
+        raise TypeError("SpzFormat.write takes no positional arguments after path")
+    enc = encode(DeviceRecords.from_writer_input(data))
+    level = kwargs.get("compression_level", 0)
+    if self._gsx_options["write"]["gzip"] == "device":
+        blob = enc.compress(level)
+    else:
+        blob = gzip.compress(enc.to_host(), compresslevel=level)
+    return lambda path: Path(path).write_bytes(blob)
 
 
 def read_tables():
@@ -185,8 +174,3 @@ def decode(data, device="cuda") -> readers.Decoded:
         check(lib.gsx_spz_decode(_ptr(raw), n, version, dim, frac_bits, _ptr(tabs), dtype.itemsize, _ptr(rows),
                                  _stream()), "gsx_spz_decode")
     return readers.Decoded(rows, dtype, None)
-
-
-def install_reader(cls) -> None:
-    """Make cls.read the device reader, keeping the original as cls._gsx_reference_read (idempotent)."""
-    readers.install(cls, decode)

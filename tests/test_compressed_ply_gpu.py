@@ -175,7 +175,7 @@ def test_gathered_survivors(cuda, gsx_lib):
 
 def test_dropin_write_on_stand_in_class(cuda, gsx_lib, tmp_path):
     import torch
-    from gsx import compressed_ply, morton, synth
+    from gsx import compressed_ply, dropin, morton, synth
 
     class StandIn:
         def __init__(self):
@@ -187,8 +187,10 @@ def test_dropin_write_on_stand_in_class(cuda, gsx_lib, tmp_path):
         def _write_ply_file(self, path, chunk_data, vertex_data, sh_data):
             self.calls.append(("file", path, chunk_data, vertex_data, sh_data))
 
-    compressed_ply.install(StandIn)
-    compressed_ply.install(StandIn)                  # idempotent
+    original = StandIn.write
+    dropin.install_writer(StandIn, compressed_ply.prepare_write)
+    dropin.install_writer(StandIn, compressed_ply.prepare_write)     # idempotent
+    assert StandIn._gsx_reference_write is original and StandIn.write is not original
     a = synth.structured(5_000, "mixed")
     w = StandIn()
     w.write(a, tmp_path / "a.ply")

@@ -151,7 +151,7 @@ def test_write_spz_device_reads_back(cuda, gsx_lib, tmp_path):
 
 
 def test_dropin_write_device_gzip_on_stand_in_class(cuda, gsx_lib, tmp_path):
-    from gsx import spz, synth
+    from gsx import dropin, spz, synth
 
     class StandIn:
         def write(self, data, path, **kwargs):
@@ -161,10 +161,8 @@ def test_dropin_write_device_gzip_on_stand_in_class(cuda, gsx_lib, tmp_path):
         def write(self, data, path, **kwargs):
             raise AssertionError("the original write must not run for packed float32 records")
 
-    spz.install(StandIn, where="device")
-    spz.install(HostGzip)
-    with pytest.raises(ValueError):
-        spz.install(type("Bad", (), {"write": lambda *a: None}), where="gpu")
+    dropin.install_writer(StandIn, spz.prepare_write, gzip="device")
+    dropin.install_writer(HostGzip, spz.prepare_write, gzip="host")
     a = synth.structured(3_000, "mixed")
     StandIn().write(a, tmp_path / "dev.spz", compression_level=6)
     HostGzip().write(a, tmp_path / "host.spz", compression_level=6)

@@ -140,9 +140,10 @@ def test_dropin_on_a_stand_in_class(gsx_lib, cuda, tmp_path, capsys):
         def write(self, data, path, **kwargs):
             calls.append((len(data), path, kwargs))
 
-    gp.install(ParquetFormat)
-    gp.install(ParquetFormat)
-    assert ParquetFormat._gsx_reference_write is not ParquetFormat.write
+    original = ParquetFormat.write
+    dropin.install_writer(ParquetFormat, gp.prepare_write)
+    dropin.install_writer(ParquetFormat, gp.prepare_write)
+    assert ParquetFormat._gsx_reference_write is original and ParquetFormat.write is not original
     ok = np.zeros(5, [("x", "<f4"), ("opacity", "<f4")])
     ParquetFormat().write(ok, str(tmp_path / "a.parquet"))
     assert not calls and "Parquet write completed. 5 rows." in capsys.readouterr().out
@@ -150,5 +151,3 @@ def test_dropin_on_a_stand_in_class(gsx_lib, cuda, tmp_path, capsys):
     for bad in (np.zeros(3, [("x", "<f4"), ("d", "<f8")]), np.zeros(3, [("opacity", "<f4"), ("alpha", "<f4")])):
         ParquetFormat().write(bad, str(tmp_path / "b.parquet"), flag=1)
         assert calls[-1] == (3, str(tmp_path / "b.parquet"), {"flag": 1})
-    with pytest.raises(ValueError):
-        dropin.patch(parquet="gpu")

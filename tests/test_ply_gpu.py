@@ -3,10 +3,6 @@ reference's own results (g15) and the NumPy oracle (ply_oracle.py) at 1 M and 10
 row stride residue, partial last tiles and 1024-byte rows; every float32 pattern and the integer and float64 edges of
 its casts; round trips between the flavours; a decode -> filters -> gather -> encode chain that never builds the host
 array; and the drop-in.  Bytes are compared, not values."""
-import subprocess
-import sys
-import textwrap
-from pathlib import Path
 
 import numpy as np
 import pytest
@@ -16,8 +12,6 @@ import splat_codecs_oracle as sco
 from test_ply_cpu import GOLDEN, expected, golden_cases, writer_input
 
 pytestmark = pytest.mark.gpu
-
-ROOT = Path(__file__).resolve().parent.parent
 
 
 def assert_same(got: np.ndarray, want: np.ndarray, what: str):
@@ -250,15 +244,15 @@ class StandIn:
 
 
 def test_dropin_on_stand_in_classes(cuda, gsx_lib, tmp_path):
-    from gsx import ply
+    from gsx import dropin, ply
     z = np.load(GOLDEN)
     for flavor in ("3dgs", "cc"):
         cls = type(f"StandIn_{flavor}", (StandIn,), {})
-        ply.install_reader(cls, flavor)
-        ply.install(cls, flavor)
-        ply.install_reader(cls, flavor)                        # idempotent
-        ply.install(cls, flavor)
+        for _ in range(2):                                     # idempotent
+            dropin.install_reader(cls, ply.decode, after=dropin._vertex_only, flavor=flavor)
+            dropin.install_writer(cls, ply.prepare_write, flavor=flavor)
         assert cls._gsx_reference_read is StandIn.read and cls._gsx_reference_write is StandIn.write
+        assert cls.read is not StandIn.read and cls.write is not StandIn.write
         r = cls()
         good = z[f"read_{flavor}_extras_file"].tobytes()
         p = tmp_path / f"{flavor}.ply"
@@ -278,35 +272,6 @@ def test_dropin_on_stand_in_classes(cuda, gsx_lib, tmp_path):
         bad = np.zeros(3, [("x", "<f4"), ("flag", "?")])
         r.write(bad, str(out), crop_sh=False)                   # refused: the reference's write
         assert r.calls[-1] == ("write", str(out), (), {"crop_sh": False}) and len(r.calls) == 3
-
-
-PATCH_PROBE = textwrap.dedent("""
-    import sys, types
-    sys.path[:0] = [{root!r}, {pkg!r}]
-    import gsconverter
-    fm = types.ModuleType("gsconverter.formats"); fm.__path__ = []
-    sys.modules["gsconverter.formats"] = fm
-    classes = []
-    for mod, name in (("ply_3dgs", "Ply3DGSFormat"), ("ply_cc", "PlyCCFormat")):
-        m = types.ModuleType("gsconverter.formats." + mod)
-        cls = type(name, (), {{"read": lambda self, *a, **k: None, "write": lambda self, *a, **k: None}})
-        setattr(m, name, cls)
-        sys.modules[m.__name__] = m
-        classes.append(cls)
-    from gsx import dropin
-    assert dropin.patch({kw})
-    print([("_gsx_reference_read" in c.__dict__, "_gsx_reference_write" in c.__dict__) for c in classes])
-""")
-
-
-@pytest.mark.parametrize("kw, want", [("", False), ("ply='host'", False), ("readers='device', codecs='device'", False),
-                                      ("ply='device'", True)])
-def test_patch_ply_keyword(kw, want, cuda, gsx_lib):
-    src = PATCH_PROBE.format(root=str(ROOT), pkg=str(ROOT / "3dgsconverter_b200"), kw=kw)
-    out = subprocess.run([sys.executable, "-c", src], capture_output=True, text=True, timeout=600)
-    assert out.returncode == 0, out.stderr[-2000:]
-    got = eval(out.stdout.strip().splitlines()[-1])   # noqa: S307  (our own probe's list literal)
-    assert got == [(want, want)] * 2
 
 
 def test_patch_refuses_unknown_ply_value(gsx_lib):

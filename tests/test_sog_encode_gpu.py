@@ -118,7 +118,7 @@ def test_refusals_leave_the_rng_alone(cuda, gsx_lib):
 
 
 def test_dropin_write_on_stand_in_class(cuda, gsx_lib, tmp_path):
-    from gsx import sog, synth
+    from gsx import dropin, sog, synth
 
     class StandIn:
         def __init__(self):
@@ -127,9 +127,10 @@ def test_dropin_write_on_stand_in_class(cuda, gsx_lib, tmp_path):
         def write(self, data, path, **kwargs):
             self.calls.append(("original", data, path, kwargs, np.random.get_state()))
 
-    sog.install(StandIn)
-    sog.install(StandIn)                             # idempotent
-    assert StandIn._gsx_reference_write is not StandIn.write and StandIn.write is sog.dropin_write
+    original = StandIn.write
+    dropin.install_writer(StandIn, sog.prepare_write, webp="host")
+    dropin.install_writer(StandIn, sog.prepare_write, webp="host")       # idempotent
+    assert StandIn._gsx_reference_write is original and StandIn.write is not original
     a = synth.structured(3_000, "mixed")
     np.random.seed(8)
     StandIn().write(a, tmp_path / "a.sog", compression_level=7)

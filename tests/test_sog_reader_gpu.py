@@ -1,10 +1,6 @@
 """GPU: the SOG reader on the device (gsx.sog_reader) against the reference reader's own results (g14) and the NumPy
 oracle (sog_reader_oracle.py): every fixture bundle, every quaternion byte triple, every position code, every opacity
 byte, the index checks, a 1 M-splat SH-3 round trip through the device writer, the records view and the drop-in."""
-import subprocess
-import sys
-import textwrap
-from pathlib import Path
 
 import numpy as np
 import pytest
@@ -13,8 +9,6 @@ import sog_reader_oracle as sro
 from test_sog_reader_cpu import GOLDEN, blob_of, golden_cases
 
 pytestmark = pytest.mark.gpu
-
-ROOT = Path(__file__).resolve().parent.parent
 
 
 def assert_same(got: np.ndarray, want: np.ndarray, what: str):
@@ -197,12 +191,12 @@ class StandIn:
 
 
 def test_dropin_read_on_stand_in_class(cuda, gsx_lib, tmp_path):
-    from gsx import sog_reader
+    from gsx import dropin, sog_reader
     z = np.load(GOLDEN)
     cls = type("StandInSog", (StandIn,), {})
-    sog_reader.install_reader(cls)
-    sog_reader.install_reader(cls)                                   # idempotent
-    assert cls._gsx_reference_read is StandIn.read
+    dropin.install_reader(cls, sog_reader.decode, webp="host")
+    dropin.install_reader(cls, sog_reader.decode, webp="host")       # idempotent
+    assert cls._gsx_reference_read is StandIn.read and cls.read is not StandIn.read
     r = cls()
     p = tmp_path / "a.sog"
     p.write_bytes(blob_of(z, "custom_names"))
@@ -215,33 +209,6 @@ def test_dropin_read_on_stand_in_class(cuda, gsx_lib, tmp_path):
         r.calls.clear()
         assert r.read(str(q), 7, level=4) == "reference"
         assert r.calls == [(str(q), (7,), {"level": 4})]
-
-
-PATCH_PROBE = textwrap.dedent("""
-    import sys, types
-    sys.path[:0] = [{root!r}, {pkg!r}]
-    import gsconverter
-    fm = types.ModuleType("gsconverter.formats"); fm.__path__ = []
-    sys.modules["gsconverter.formats"] = fm
-    m = types.ModuleType("gsconverter.formats.sog")
-    cls = type("SogFormat", (), {{"read": lambda self, *a, **k: None, "write": lambda self, *a, **k: None}})
-    m.SogFormat = cls
-    sys.modules[m.__name__] = m
-    from gsx import dropin
-    assert dropin.patch({kw})
-    print(("_gsx_reference_read" in cls.__dict__, "_gsx_reference_write" in cls.__dict__))
-""")
-
-
-@pytest.mark.parametrize("kw, want", [("", (False, False)), ("sog_reader='host'", (False, False)),
-                                      ("readers='device'", (False, False)),
-                                      ("sog_reader='device'", (True, False)),
-                                      ("sog_reader='device', sog='device'", (True, True))])
-def test_patch_sog_reader_keyword(kw, want, cuda, gsx_lib):
-    src = PATCH_PROBE.format(root=str(ROOT), pkg=str(ROOT / "3dgsconverter_b200"), kw=kw)
-    out = subprocess.run([sys.executable, "-c", src], capture_output=True, text=True, timeout=600)
-    assert out.returncode == 0, out.stderr[-2000:]
-    assert eval(out.stdout.strip().splitlines()[-1]) == want   # noqa: S307  (our own probe's tuple literal)
 
 
 def test_patch_rejects_unknown_sog_reader(gsx_lib):

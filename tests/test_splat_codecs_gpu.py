@@ -2,10 +2,6 @@
 writers' own files (g12) and the NumPy oracle (splat_codecs_oracle.py), the trailing-field upload, the drop-ins, and
 NumPy's float32 exp over every float32 bit pattern."""
 import gzip
-import subprocess
-import sys
-import textwrap
-from pathlib import Path
 
 import numpy as np
 import pytest
@@ -14,8 +10,6 @@ import splat_codecs_oracle as sco
 from test_splat_codecs_cpu import GOLDEN, TAGS
 
 pytestmark = pytest.mark.gpu
-
-ROOT = Path(__file__).resolve().parent.parent
 
 
 def device_files(a, cuda, records=None):
@@ -128,13 +122,15 @@ class StandIn:
 
 
 def test_dropin_writes_on_stand_in_classes(cuda, gsx_lib, tmp_path):
-    from gsx import ksplat, splat, spz, synth
+    from gsx import dropin, ksplat, splat, spz, synth
     a = with_rgb(synth.structured(3_000, "mixed"))
     plain = sco.golden_inputs()["fields0"]
     for mod in (ksplat, spz, splat):
         cls = type(f"StandIn_{mod.__name__}", (StandIn,), {})
-        mod.install(cls)
-        mod.install(cls)                              # idempotent
+        opts = {"gzip": "host"} if mod is spz else {}
+        dropin.install_writer(cls, mod.prepare_write, **opts)
+        dropin.install_writer(cls, mod.prepare_write, **opts)         # idempotent
+        assert cls._gsx_reference_write is StandIn.write and cls.write is not StandIn.write
         w = cls()
         p = tmp_path / mod.__name__
         if mod is ksplat:
@@ -157,38 +153,11 @@ def test_dropin_writes_on_stand_in_classes(cuda, gsx_lib, tmp_path):
         assert len(w.calls) == 1 and w.calls[0][0] is b and w.calls[0][1:] == ("b.out", args, {"level": 4})
     # the degree-1 field set with SH content: the reference SPZ writer raises, and so does the drop-in's fallback
     cls = type("StandInSpz", (StandIn,), {})
-    spz.install(cls)
+    dropin.install_writer(cls, spz.prepare_write, gzip="host")
     w = cls()
     d1 = sco.golden_inputs()["fields1"]
     w.write(d1, tmp_path / "d1.spz", compression_level=0)
     assert len(w.calls) == 1 and w.calls[0][0] is d1 and w.calls[0][3] == {"compression_level": 0}
-
-
-PATCH_PROBE = textwrap.dedent("""
-    import sys, types
-    sys.path[:0] = [{root!r}, {pkg!r}]
-    import gsconverter
-    fm = types.ModuleType("gsconverter.formats"); fm.__path__ = []
-    sys.modules["gsconverter.formats"] = fm
-    classes = []
-    for mod, name in (("splat", "SplatFormat"), ("ksplat", "KSplatFormat"), ("spz", "SpzFormat")):
-        m = types.ModuleType("gsconverter.formats." + mod)
-        cls = type(name, (), {{"write": lambda self, *a, **k: None}})
-        setattr(m, name, cls)
-        sys.modules[m.__name__] = m
-        classes.append(cls)
-    from gsx import dropin
-    assert dropin.patch({kw})
-    print(["_gsx_reference_write" in c.__dict__ for c in classes])
-""")
-
-
-@pytest.mark.parametrize("kw, want", [("", [False] * 3), ("codecs='host'", [False] * 3), ("codecs='device'", [True] * 3)])
-def test_patch_codecs_keyword(kw, want, cuda, gsx_lib):
-    src = PATCH_PROBE.format(root=str(ROOT), pkg=str(ROOT / "3dgsconverter_b200"), kw=kw)
-    out = subprocess.run([sys.executable, "-c", src], capture_output=True, text=True, timeout=600)
-    assert out.returncode == 0, out.stderr[-2000:]
-    assert out.stdout.strip().splitlines()[-1] == str(want)
 
 
 def test_numpy_expf_every_float32(cuda, gsx_lib):

@@ -105,7 +105,7 @@ def test_sog_reader_webp_device_on_gsx_bundles(cuda, gsx_lib, tmp_path):
 
 
 def test_dropin_falls_back_on_a_bad_member(cuda, gsx_lib, tmp_path):
-    from gsx import sog_reader
+    from gsx import dropin, sog_reader
 
     class StandIn:
         def read(self, path, *args, **kwargs):
@@ -122,5 +122,5 @@ def test_dropin_falls_back_on_a_bad_member(cuda, gsx_lib, tmp_path):
     p.write_bytes(out.getvalue())
     with pytest.raises(ValueError):
         sog_reader.decode(out.getvalue(), cuda, webp="device")
-    sog_reader.install_reader(StandIn, webp="device")
+    dropin.install_reader(StandIn, sog_reader.decode, webp="device")
     assert StandIn().read(str(p)) == "reference"

@@ -122,7 +122,7 @@ def test_write_sog_device_bundle_matches_pillow_bundle(sog_1m, cuda, gsx_lib, tm
 
 
 def test_dropin_write_device_webp_on_stand_in_class(cuda, gsx_lib, tmp_path):
-    from gsx import sog, sog_reader, synth
+    from gsx import dropin, sog, sog_reader, synth
 
     class StandIn:
         def write(self, data, path, **kwargs):
@@ -131,10 +131,8 @@ def test_dropin_write_device_webp_on_stand_in_class(cuda, gsx_lib, tmp_path):
     class HostWebp(StandIn):
         pass
 
-    sog.install(StandIn, webp="device")
-    sog.install(HostWebp, webp="host")
-    with pytest.raises(ValueError):
-        sog.install(type("Bad", (), {"write": lambda *a: None}), webp="gpu")
+    dropin.install_writer(StandIn, sog.prepare_write, webp="device")
+    dropin.install_writer(HostWebp, sog.prepare_write, webp="host")
     a = synth.structured(3_000, "mixed")
     np.random.seed(8)
     StandIn().write(a, tmp_path / "dev.sog", compression_level=7)
