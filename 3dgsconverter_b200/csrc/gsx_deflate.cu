@@ -16,6 +16,7 @@
 #include "../../include/gsx.h"
 
 #include "gsx_common.cuh"
+#include "gsx_deflate_format.cuh"
 
 #include <algorithm>
 #include <climits>
@@ -34,7 +35,6 @@ constexpr int kMaxCopy = 258;
 constexpr int64_t kCrcChunk = 4096;
 constexpr int kCrcParts = 1024;
 constexpr uint32_t kPoly = 0xEDB88320u;
-__constant__ uint8_t kClOrder[kClSyms] = {16, 17, 18, 0, 8, 7, 9, 6, 10, 5, 11, 4, 12, 3, 13, 2, 14, 1, 15};
 
 struct BlockPlan {
     uint32_t lit[kLitSyms];     // bit-reversed code | length << 16
@@ -78,23 +78,6 @@ __device__ __forceinline__ T block_scan(T v, T ident, Op op, T* sh, T& total) {
     __syncthreads();
     total = t;
     return op(w, prev);
-}
-
-// length 3..258 -> symbol 257..285, its extra bits and their value
-__device__ __forceinline__ void length_code(uint32_t L, uint32_t& sym, uint32_t& nextra, uint32_t& extra) {
-    if (L == kMaxCopy) {
-        sym = 285, nextra = 0, extra = 0;
-        return;
-    }
-    const uint32_t v = L - 3;
-    if (v < 8) {
-        sym = 257 + v, nextra = 0, extra = 0;
-        return;
-    }
-    const uint32_t h = 31 - __clz(v);
-    nextra = h - 2;
-    sym = 257 + 4 * (h - 1) + ((v >> nextra) & 3);
-    extra = v & ((1u << nextra) - 1);
 }
 
 // ORs the bits of v at bit o of words (up to three words; bits past nwords are dropped)

@@ -17,7 +17,9 @@
 // A marker that lands before the member's first byte is zlib's "invalid distance too far back".
 #include "../../include/gsx.h"
 
+#include "gsx_bits.cuh"
 #include "gsx_common.cuh"
+#include "gsx_deflate_format.cuh"
 
 #include <algorithm>
 
@@ -30,38 +32,6 @@ constexpr int kLitFast = 10, kDistFast = 8;
 constexpr int kRunThreads = 64;
 enum : int64_t { kOk = 0, kFinal = 1, kEof = 2, kData = 3, kOverflow = 4, kNone = 5, kBadJob = 6 };
 enum : int64_t { kFind = 1, kFirst = 2 };
-
-__constant__ uint16_t kLBase[29] = {3,  4,  5,  6,  7,  8,  9,  10, 11,  13,  15,  17,  19,  23, 27,
-                                    31, 35, 43, 51, 59, 67, 83, 99, 115, 131, 163, 195, 227, 258};
-__constant__ uint8_t kLExt[29] = {0, 0, 0, 0, 0, 0, 0, 0, 1, 1, 1, 1, 2, 2, 2, 2, 3, 3, 3, 3, 4, 4, 4, 4, 5, 5, 5, 5, 0};
-__constant__ uint16_t kDBase[30] = {1,   2,   3,   4,   5,   7,    9,    13,   17,   25,   33,   49,   65,    97,    129,
-                                    193, 257, 385, 513, 769, 1025, 1537, 2049, 3073, 4097, 6145, 8193, 12289, 16385, 24577};
-__constant__ uint8_t kDExt[30] = {0, 0, 0, 0, 1, 1, 2, 2, 3, 3, 4, 4, 5, 5, 6, 6, 7, 7, 8, 8, 9, 9, 10, 10, 11, 11, 12, 12, 13, 13};
-__constant__ uint8_t kClOrder[19] = {16, 17, 18, 0, 8, 7, 9, 6, 10, 5, 11, 4, 12, 3, 13, 2, 14, 1, 15};
-
-// LSB-first bit reader over d[0, nbytes): never reads past the end; need(k) is false when fewer than k bits remain.
-struct Reader {
-    const uint8_t* d;
-    int64_t nbytes, next;
-    uint64_t buf;
-    int cnt;
-
-    __device__ void init(const uint8_t* d_, int64_t n, int64_t bit) {
-        d = d_, nbytes = n, next = bit >> 3, buf = 0, cnt = 0;
-        refill();
-        drop(int(bit & 7));
-    }
-    __device__ __forceinline__ void refill() {
-        while (cnt <= 56 && next < nbytes) buf |= uint64_t(__ldg(d + next++)) << cnt, cnt += 8;
-    }
-    __device__ __forceinline__ bool need(int k) {
-        if (cnt < k) refill();
-        return cnt >= k;
-    }
-    __device__ __forceinline__ uint32_t peek(int k) const { return uint32_t(buf & ((uint64_t(1) << k) - 1)); }
-    __device__ __forceinline__ void drop(int k) { buf >>= k, cnt -= k; }
-    __device__ __forceinline__ int64_t pos() const { return next * 8 - cnt; }
-};
 
 // Canonical Huffman code: counts and symbols sorted by (length, symbol), and a FAST-bit table of the codes that fit
 // (symbol | length << 9; 0 = look further).

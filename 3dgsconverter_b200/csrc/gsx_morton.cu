@@ -19,6 +19,7 @@
 // truncation to uint32.
 #include "../../include/gsx.h"
 
+#include "gsx_bits.cuh"
 #include "gsx_common.cuh"
 #include "gsx_radix.cuh"
 #include "gsx_sor.cuh"
@@ -39,24 +40,16 @@ __device__ __forceinline__ uint32_t part1by2(uint32_t n) {
     return n;
 }
 
-// order-preserving float <-> uint mapping for atomicMin/Max
-__device__ __forceinline__ uint32_t f2o(float f) {
-    uint32_t u = __float_as_uint(f);
-    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-// the same for a min (max) slot, with every NaN mapped below (above) every number, so a NaN wins the slot; o2f of
-// either extreme is a NaN
-__device__ __forceinline__ uint32_t f2o_lo(float f) { return f != f ? 0u : f2o(f); }
-__device__ __forceinline__ uint32_t f2o_hi(float f) { return f != f ? 0xffffffffu : f2o(f); }
+// float_to_ord for a min (max) slot of atomicMin/Max, with every NaN mapped below (above) every number, so a NaN wins
+// the slot; ord_to_float of either extreme is a NaN
+__device__ __forceinline__ uint32_t f2o_lo(float f) { return f != f ? 0u : float_to_ord(f); }
+__device__ __forceinline__ uint32_t f2o_hi(float f) { return f != f ? 0xffffffffu : float_to_ord(f); }
 // NaN-propagating min / max (np.min / np.max); -0.0 is below +0.0, so the result does not depend on the order
 __device__ __forceinline__ float nan_min(float a, float b) {
     return a != a ? a : (b != b ? b : (b < a || (b == a && signbit(b)) ? b : a));
 }
 __device__ __forceinline__ float nan_max(float a, float b) {
     return a != a ? a : (b != b ? b : (b > a || (b == a && !signbit(b)) ? b : a));
-}
-__device__ __forceinline__ float o2f(uint32_t o) {
-    return __uint_as_float((o & 0x80000000u) ? (o & 0x7fffffffu) : ~o);
 }
 
 // segment of the e-th active element: largest s with seg_off[s] <= e
@@ -130,7 +123,7 @@ __global__ void __launch_bounds__(256) k_mo_keys(const float* __restrict__ xyz, 
     bool flat = true;
 #pragma unroll
     for (int a = 0; a < 3; ++a) {
-        const float mn = o2f(bounds[6 * s + a]), mx = o2f(bounds[6 * s + 3 + a]);
+        const float mn = ord_to_float(bounds[6 * s + a]), mx = ord_to_float(bounds[6 * s + 3 + a]);
         const float len = __fsub_rn(mx, mn);
         const float mul = len > 0.f ? __fdiv_rn(1024.0f, len) : 0.f;
         if (len != 0.f) flat = false;

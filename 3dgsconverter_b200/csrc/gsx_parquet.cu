@@ -23,6 +23,7 @@
 //   k_pq_assemble    the host's page headers and footer and the compressed pieces into the file buffer.
 #include "../../include/gsx.h"
 
+#include "gsx_bits.cuh"
 #include "gsx_common.cuh"
 #include "gsx_radix.cuh"
 #include "gsx_staged.cuh"
@@ -46,7 +47,7 @@ constexpr int kJobs = 1024;              // literal copies per walk round
 __device__ __forceinline__ bool is_null(uint32_t v) { return (v & 0x7FFFFFFFu) > 0x7F800000u; }
 
 __device__ __forceinline__ uint32_t order_key(uint32_t v, int kind) {
-    return kind ? v : ((v >> 31) ? ~v : v ^ 0x80000000u);
+    return kind ? v : float_to_ord(__uint_as_float(v));
 }
 
 __device__ __forceinline__ uint32_t mix(uint32_t h) {   // murmur3's finaliser

@@ -19,6 +19,7 @@
 // Every other pairing is refused.  Field offsets may be any byte; rows up to kRowMax bytes.
 #include "../../include/gsx.h"
 
+#include "gsx_bits.cuh"
 #include "gsx_common.cuh"
 #include "gsx_numpy_scalar.cuh"
 #include "gsx_staged.cuh"
@@ -88,8 +89,6 @@ __device__ __forceinline__ void transcode_one(const uint8_t* s, uint8_t* d, cons
                                 : (uint8_t)v;
     }
 }
-
-__host__ __device__ __forceinline__ size_t up16(size_t x) { return (x + 15) & ~(size_t)15; }
 
 __global__ void __launch_bounds__(kThreads) k_ply_transcode(const uint8_t* __restrict__ src, int64_t n, int32_t src_row,
                                                             uint8_t* __restrict__ dst, int32_t dst_row, const PlyFields T,

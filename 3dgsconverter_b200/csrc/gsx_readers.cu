@@ -24,6 +24,7 @@
 // order and precision (gsx_numpy_scalar.cuh), with x86's NaN results where NaN inputs can reach the output.
 #include "../../include/gsx.h"
 
+#include "gsx_bits.cuh"
 #include "gsx_common.cuh"
 #include "gsx_numpy_scalar.cuh"
 #include "gsx_staged.cuh"
@@ -42,16 +43,6 @@ constexpr float kEps6 = (float)1e-6;
 constexpr float kSqrt2 = (float)1.41421356;
 constexpr float kSqrt1_2 = (float)0.707106781186547524401;
 
-__device__ __forceinline__ uint32_t get32(const uint8_t* p) {
-    return (uint32_t)p[0] | (uint32_t)p[1] << 8 | (uint32_t)p[2] << 16 | (uint32_t)p[3] << 24;
-}
-__device__ __forceinline__ uint16_t get16(const uint8_t* p) { return (uint16_t)(p[0] | p[1] << 8); }
-__device__ __forceinline__ float getf(const uint8_t* p) { return __uint_as_float(get32(p)); }
-__device__ __forceinline__ void put32(uint8_t* p, uint32_t v) {
-    p[0] = (uint8_t)v, p[1] = (uint8_t)(v >> 8), p[2] = (uint8_t)(v >> 16), p[3] = (uint8_t)(v >> 24);
-}
-__device__ __forceinline__ void putf(uint8_t*& p, float v) { put32(p, __float_as_uint(v)), p += 4; }
-
 // staged row width `crow`, of which the first `head` bytes precede the zero run; output rows of row_bytes bytes
 struct RowOut {
     int32_t crow, head;
@@ -67,8 +58,6 @@ __device__ __forceinline__ void store_rows(uint8_t* __restrict__ out, int64_t ba
 __device__ __forceinline__ void load_tables(float* tab, const float* __restrict__ tables, int ntab) {
     for (int i = threadIdx.x; i < ntab * 256; i += blockDim.x) tab[i] = __ldg(tables + i);
 }
-
-__host__ __device__ __forceinline__ size_t up16(size_t x) { return (x + 15) & ~(size_t)15; }
 
 // ---------------------------------------------------------------------------------------------------------- .splat
 // tables: DC (splat.py:75-77), opacity logit (:67-69)

@@ -10,6 +10,7 @@
 // clip, then the reference's left-neighbour test |v - cb[left]| < |v - cb[idx]| in float32.
 #include "../../include/gsx.h"
 
+#include "gsx_bits.cuh"
 #include "gsx_common.cuh"
 #include "gsx_numpy_scalar.cuh"
 #include "gsx_sh_mask.cuh"
@@ -17,18 +18,11 @@
 
 namespace gsx {
 
-__device__ __forceinline__ uint32_t float_key(float f) {
-    if (f != f) return 0xffffffffu;  // NaN: after +inf (0xff800000), all NaNs equal
-    f = f + 0.0f;  // -0.0 -> +0.0 (equal keys in NumPy)
-    uint32_t u = __float_as_uint(f);
-    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-
 __global__ void __launch_bounds__(256) k_lex_keys_z(const float* __restrict__ xyz, int64_t n,
                                                     uint64_t* __restrict__ keys, int32_t* __restrict__ vals) {
     int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    keys[i] = (uint64_t)float_key(xyz[3 * i + 2]);
+    keys[i] = (uint64_t)numpy_sort_key(xyz[3 * i + 2]);
     vals[i] = (int32_t)i;
 }
 
@@ -37,7 +31,7 @@ __global__ void __launch_bounds__(256) k_lex_keys_xy(const float* __restrict__ x
     int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (j >= n) return;
     int64_t i = order[j];
-    keys[j] = ((uint64_t)float_key(xyz[3 * i]) << 32) | (uint64_t)float_key(xyz[3 * i + 1]);
+    keys[j] = ((uint64_t)numpy_sort_key(xyz[3 * i]) << 32) | (uint64_t)numpy_sort_key(xyz[3 * i + 1]);
 }
 
 constexpr int kMaxCodebook = 4096;

@@ -30,6 +30,7 @@
 //     test, mean = 0 when no candidate was found.
 #include "../../include/gsx.h"
 
+#include "gsx_bits.cuh"
 #include "gsx_common.cuh"
 #include "gsx_sor.cuh"
 
@@ -288,15 +289,6 @@ __global__ void __launch_bounds__(256) k_sor_keys(const float* __restrict__ xyz,
 // bucket is re-hashed from the position.  Outputs: {start,end} of every occupied bucket (tab_se pre-zeroed:
 // start == end == 0 <=> the reference's cell_start == -1), one bit per sorted position that starts a bucket,
 // and the bounding boxes of every chunk and super.
-// order-preserving float <-> uint32 (for redux.sync min/max); +/-inf map to the extremes, -0 < +0
-__device__ __forceinline__ uint32_t float_to_ord(float f) {
-    const uint32_t u = __float_as_uint(f);
-    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-__device__ __forceinline__ float ord_to_float(uint32_t o) {
-    return __uint_as_float((o & 0x80000000u) ? (o & 0x7fffffffu) : ~o);
-}
-
 template <bool GATHER>
 __device__ __forceinline__ void
     sor_finish_tile(const int64_t tile, const float* __restrict__ xyz, const uint64_t* __restrict__ keys, PackFmt fmt,

@@ -22,6 +22,7 @@
 // operation in the reference's order.
 #include "../../include/gsx.h"
 
+#include "gsx_bits.cuh"
 #include "gsx_common.cuh"
 #include "gsx_numpy_scalar.cuh"
 #include "gsx_sh_mask.cuh"
@@ -48,11 +49,6 @@ struct CodecCols {
     int32_t c[kMaxCols];   // row column of tile column k
     int32_t ncol;
 };
-
-__device__ __forceinline__ void put16(uint8_t* p, uint16_t v) { p[0] = (uint8_t)v, p[1] = (uint8_t)(v >> 8); }
-__device__ __forceinline__ void put32(uint8_t* p, uint32_t v) {
-    p[0] = (uint8_t)v, p[1] = (uint8_t)(v >> 8), p[2] = (uint8_t)(v >> 16), p[3] = (uint8_t)(v >> 24);
-}
 
 // Columns of this CTA's rows [base, base + rows_here) into tile[row * ncol + k]; warp w loads rows 32w .. 32w+31 with
 // its lanes striding over the row's columns.  Only the warp's own rows are touched, so __syncwarp() is enough before a
@@ -258,14 +254,7 @@ __global__ void __launch_bounds__(256) k_splat_sort_keys(const float* __restrict
     const float ssum = __fadd_rn(__fadd_rn(__ldg(r + c0), __ldg(r + c1)), __ldg(r + c2));
     const float opt = __fdiv_rn(1.f, __fadd_rn(1.f, numpy_expf(-__ldg(r + cop))));
     const float v = -__fmul_rn(numpy_expf(ssum), opt);
-    uint32_t key;
-    if (v != v) {
-        key = 0xffffffffu;   // above +inf's key: np.argsort puts NaN last
-    } else {
-        const uint32_t b = __float_as_uint(v == 0.f ? 0.f : v);   // -0.0 sorts as +0.0
-        key = b & 0x80000000u ? ~b : b | 0x80000000u;
-    }
-    keys[i] = key;
+    keys[i] = numpy_sort_key(v);
     vals[i] = (int32_t)i;
 }
 

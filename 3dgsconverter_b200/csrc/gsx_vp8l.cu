@@ -17,6 +17,7 @@
 #include "../../include/gsx.h"
 
 #include "gsx_common.cuh"
+#include "gsx_vp8l_format.cuh"
 
 namespace gsx {
 namespace {
@@ -42,37 +43,6 @@ __constant__ uint8_t kPlane[120] = {
     0x66, 0x6a, 0x22, 0x2e, 0x54, 0x5c, 0x43, 0x4d, 0x65, 0x6b, 0x32, 0x3e, 0x78, 0x01, 0x77, 0x79, 0x53, 0x5d, 0x11, 0x1f,
     0x64, 0x6c, 0x42, 0x4e, 0x76, 0x7a, 0x21, 0x2f, 0x75, 0x7b, 0x31, 0x3f, 0x63, 0x6d, 0x52, 0x5e, 0x00, 0x74, 0x7c, 0x41,
     0x4f, 0x10, 0x20, 0x62, 0x6e, 0x30, 0x73, 0x7d, 0x51, 0x5f, 0x40, 0x72, 0x7e, 0x61, 0x6f, 0x50, 0x71, 0x7f, 0x60, 0x70};
-
-struct Reader {
-    const uint8_t* d;
-    int64_t nbytes, next;
-    uint64_t buf;
-    int cnt;
-
-    __device__ void init(const uint8_t* d_, int64_t n, int64_t bit) {
-        d = d_, nbytes = n, next = bit >> 3, buf = 0, cnt = 0;
-        if (next > nbytes) next = nbytes;
-        refill();
-        drop(min(int(bit & 7), cnt));
-    }
-    __device__ __forceinline__ void refill() {
-        while (cnt <= 56 && next < nbytes) buf |= uint64_t(__ldg(d + next++)) << cnt, cnt += 8;
-    }
-    __device__ __forceinline__ bool need(int k) {
-        if (cnt < k) refill();
-        return cnt >= k;
-    }
-    __device__ __forceinline__ uint32_t peek(int k) const { return uint32_t(buf & ((uint64_t(1) << k) - 1)); }
-    __device__ __forceinline__ void drop(int k) { buf >>= k, cnt -= k; }
-    __device__ __forceinline__ int64_t pos() const { return next * 8 - cnt; }
-    // false when the stream ends first
-    __device__ __forceinline__ bool bits(int k, uint32_t& v) {
-        if (!need(k)) return false;
-        v = peek(k);
-        drop(k);
-        return true;
-    }
-};
 
 // libwebp's acceptance: not all lengths 0, at most 2^len codes of each length, exactly one used symbol (of any length
 // 1..15) is a 0-bit code, anything else must fill the code space.
@@ -205,18 +175,6 @@ __device__ int64_t read_code(Reader& r, int alphabet, uint32_t* c, uint8_t* len)
         for (int i = 0; i < int(rep) + base; ++i) len[s++] = k == 16 ? prev : 0;
     }
     return build_code(len, alphabet, c);
-}
-
-__device__ __forceinline__ bool prefix_value(Reader& r, uint32_t sym, uint32_t& out) {
-    if (sym < 4) {
-        out = sym + 1;
-        return true;
-    }
-    const int extra = int(sym - 2) >> 1;
-    uint32_t v;
-    if (!r.bits(extra, v)) return false;
-    out = ((2 + (sym & 1)) << extra) + v + 1;
-    return true;
 }
 
 __device__ __forceinline__ int64_t plane_distance(uint32_t code, int64_t xsize) {
@@ -560,49 +518,6 @@ __global__ void k_vp8l_cross(uint32_t* __restrict__ px, const uint32_t* __restri
         const uint32_t red = ((v >> 16) + delta(m, g)) & 0xFF;
         const uint32_t blue = (v + delta(m >> 8, g) + delta(m >> 16, red)) & 0xFF;
         px[i] = (v & 0xFF00FF00u) | red << 16 | blue;
-    }
-}
-
-__device__ __forceinline__ uint32_t avg2(uint32_t a, uint32_t b) {
-    return (((a ^ b) & 0xFEFEFEFEu) >> 1) + (a & b);
-}
-
-__device__ __forceinline__ int ch(uint32_t v, int c) { return int((v >> (8 * c)) & 0xFF); }
-
-__device__ __forceinline__ uint32_t clamp_full(uint32_t a, uint32_t b, uint32_t c) {
-    uint32_t o = 0;
-    for (int k = 0; k < 4; ++k) o |= uint32_t(min(255, max(0, ch(a, k) + ch(b, k) - ch(c, k)))) << (8 * k);
-    return o;
-}
-
-__device__ __forceinline__ uint32_t clamp_half(uint32_t a, uint32_t b) {
-    uint32_t o = 0;
-    for (int k = 0; k < 4; ++k) o |= uint32_t(min(255, max(0, ch(a, k) + (ch(a, k) - ch(b, k)) / 2))) << (8 * k);
-    return o;
-}
-
-__device__ __forceinline__ uint32_t select(uint32_t L, uint32_t T, uint32_t TL) {
-    int pl = 0, pt = 0;
-    for (int k = 0; k < 4; ++k) pl += abs(ch(T, k) - ch(TL, k)), pt += abs(ch(L, k) - ch(TL, k));
-    return pl < pt ? L : T;
-}
-
-__device__ __forceinline__ uint32_t predict(int mode, uint32_t L, uint32_t T, uint32_t TR, uint32_t TL) {
-    switch (mode) {
-        case 1: return L;
-        case 2: return T;
-        case 3: return TR;
-        case 4: return TL;
-        case 5: return avg2(avg2(L, TR), T);
-        case 6: return avg2(L, TL);
-        case 7: return avg2(L, T);
-        case 8: return avg2(TL, T);
-        case 9: return avg2(T, TR);
-        case 10: return avg2(avg2(L, TL), avg2(T, TR));
-        case 11: return select(L, T, TL);
-        case 12: return clamp_full(L, T, TL);
-        case 13: return clamp_half(avg2(L, T), TL);
-        default: return 0xFF000000u;
     }
 }
 

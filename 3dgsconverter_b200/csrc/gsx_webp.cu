@@ -18,6 +18,7 @@
 
 #include "gsx_common.cuh"
 #include "gsx_radix.cuh"
+#include "gsx_vp8l_format.cuh"
 
 #include <algorithm>
 
@@ -36,62 +37,9 @@ constexpr int64_t kScanChunk = int64_t(1) << 26;   // 2^26 tokens of at most 60 
 constexpr int kGreen = 0, kRed = 280, kBlue = 536, kAlpha = 792, kDist = 1048;
 constexpr int kLeftDistSymbol = 1;                 // plane code 2 (the left pixel) -> prefix symbol 1, no extra bits
 
-__device__ __forceinline__ uint32_t chan(uint32_t p, int k) { return (p >> (8 * k)) & 0xFF; }
-
 __device__ __forceinline__ uint32_t subtract_green(uint32_t p) {
     uint32_t g = chan(p, 1);
     return (p & 0xFF00FF00u) | (((chan(p, 2) - g) & 0xFF) << 16) | ((chan(p, 0) - g) & 0xFF);
-}
-
-__device__ __forceinline__ uint32_t avg2(uint32_t a, uint32_t b) {
-    return (((a ^ b) & 0xFEFEFEFEu) >> 1) + (a & b);
-}
-
-__device__ __forceinline__ uint32_t select_pred(uint32_t L, uint32_t T, uint32_t TL) {
-    int pl = 0, pt = 0;
-    for (int k = 0; k < 4; ++k) {
-        pl += abs(int(chan(T, k)) - int(chan(TL, k)));
-        pt += abs(int(chan(L, k)) - int(chan(TL, k)));
-    }
-    return pl < pt ? L : T;
-}
-
-__device__ __forceinline__ uint32_t clamp_full(uint32_t L, uint32_t T, uint32_t TL) {
-    uint32_t out = 0;
-    for (int k = 0; k < 4; ++k) {
-        int v = int(chan(L, k)) + int(chan(T, k)) - int(chan(TL, k));
-        out |= uint32_t(min(max(v, 0), 255)) << (8 * k);
-    }
-    return out;
-}
-
-__device__ __forceinline__ uint32_t clamp_half(uint32_t a, uint32_t b) {
-    uint32_t out = 0;
-    for (int k = 0; k < 4; ++k) {
-        int ak = int(chan(a, k));
-        int v = ak + (ak - int(chan(b, k))) / 2;   // C division: truncation toward zero, as the RFC states it
-        out |= uint32_t(min(max(v, 0), 255)) << (8 * k);
-    }
-    return out;
-}
-
-__device__ __forceinline__ uint32_t predictor(int m, uint32_t L, uint32_t T, uint32_t TR, uint32_t TL) {
-    switch (m) {
-        case 0: return 0xFF000000u;
-        case 1: return L;
-        case 2: return T;
-        case 3: return TR;
-        case 4: return TL;
-        case 5: return avg2(avg2(L, TR), T);
-        case 6: return avg2(L, TL);
-        case 7: return avg2(L, T);
-        case 8: return avg2(TL, T);
-        case 9: return avg2(T, TR);
-        case 10: return avg2(avg2(L, TL), avg2(T, TR));
-        case 11: return select_pred(L, T, TL);
-        case 12: return clamp_full(L, T, TL);
-        default: return clamp_half(avg2(L, T), TL);
-    }
 }
 
 // sum over the four channels of |residual as int8|
@@ -142,7 +90,7 @@ __global__ void __launch_bounds__(256) k_webp_predict(const uint32_t* __restrict
         TL = load_src<SUBTRACT_GREEN>(src, i - W - 1);
         TR = load_src<SUBTRACT_GREEN>(src, i - W + 1);   // the rightmost column: the first pixel of this row
 #pragma unroll
-        for (int m = 0; m < kModes; ++m) cost[m] = residual_cost(__vsub4(c, predictor(m, L, T, TR, TL)));
+        for (int m = 0; m < kModes; ++m) cost[m] = residual_cost(__vsub4(c, predict(m, L, T, TR, TL)));
     }
     // edge pixels are predicted the same way under every mode, so they do not move the argmin
 #pragma unroll
@@ -167,7 +115,7 @@ __global__ void __launch_bounds__(256) k_webp_predict(const uint32_t* __restrict
     if (!valid) return;
     uint32_t pred;
     if (inner) {
-        pred = predictor(best, L, T, TR, TL);
+        pred = predict(best, L, T, TR, TL);
     } else {
         c = load_src<SUBTRACT_GREEN>(src, i);
         pred = x == 0 && y == 0 ? 0xFF000000u : load_src<SUBTRACT_GREEN>(src, y == 0 ? i - 1 : i - W);
@@ -186,18 +134,6 @@ __global__ void k_webp_run_starts(const uint32_t* __restrict__ sym, int64_t n, c
                                   uint32_t* __restrict__ starts) {
     for (int64_t i = blockIdx.x * int64_t(blockDim.x) + threadIdx.x; i < n; i += int64_t(gridDim.x) * blockDim.x)
         if (is_break(sym, i)) starts[run[i]] = uint32_t(i);
-}
-
-__device__ __forceinline__ void length_prefix(uint32_t length, uint32_t& code, uint32_t& nbits, uint32_t& extra) {
-    uint32_t v = length - 1;
-    if (v < 4) {
-        code = v, nbits = 0, extra = 0;
-        return;
-    }
-    uint32_t h = 31 - __clz(v);
-    code = 2 * h + ((v >> (h - 1)) & 1);
-    nbits = h - 1;
-    extra = v & ((1u << nbits) - 1);
 }
 
 // tok: 1 = literal, L >= 3 = the first pixel of a copy of L pixels, 0 = inside a copy
