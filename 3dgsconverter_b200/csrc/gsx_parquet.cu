@@ -18,8 +18,9 @@
 //                    counts of the tiles before it in the page), PLAIN or bit-packed indices ORed into 32-bit words.
 //   k_pq_dict_pages  the dictionary pages: the sorted values, PLAIN.
 //   k_pq_snappy      a CTA per 64 KiB piece of a page body: Snappy elements with copies of distance 1 (byte runs) or 4
-//                    (repeated 32-bit values) of >= 8 bytes inside the piece, taken greedily from the left, and
-//                    literals.  The candidates come from two ballots and an AND of 8 shifted words; warp 0 walks them.
+//                    (repeated 32-bit values) of >= 8 bytes inside the piece, taken greedily from the left (the longer
+//                    of the two: they never tie), and literals.  The candidates come from two ballots and an AND of 8
+//                    shifted words; warp 0 walks them.
 //   k_pq_assemble    the host's page headers and footer and the compressed pieces into the file buffer.
 #include "../../include/gsx.h"
 
@@ -40,6 +41,10 @@ constexpr int kStage = 64;               // rows staged in shared memory at a ti
 constexpr int kMaxCols = 1024;
 constexpr int kRowMax = 1024;
 constexpr uint32_t kDictMax = 1u << 18;  // pyarrow's 1 MiB dictionary page limit, in float32 values
+// Least table size: k_pq_insert stops a chunk only once a thread reads its count above kDictMax, so every thread past
+// that check (up to one resident grid, 132 SMs x 2048 threads on an H100) may still insert.  2^19 slots < 2^18 + 132 *
+// 2048 could fill, and a full table's failing threads could wrap the count back below the limit.
+constexpr int kSlotsMin = 20;
 constexpr int kPiece = 1 << 16;
 constexpr int kPieceCap = kPiece + 16;   // a piece's elements never exceed its literal-only encoding (3 tag bytes)
 constexpr int kJobs = 1024;              // literal copies per walk round
@@ -496,6 +501,9 @@ __global__ void __launch_bounds__(kThreads) k_pq_snappy(const uint8_t* __restric
                     done = true;
                     break;
                 }
+                // L1 == L4 cannot happen: e1[j - 1] and e4[j - 1] are clear at a chosen start (else j - 1 was the
+                // candidate, or the previous copy went on), so b[j - 2] != b[j - 1]: beside a distance-1 run of >= 8
+                // (b[j - 1 .. j + 7] equal) the distance-4 run is <= 2 bytes
                 const uint32_t L1 = run_from(s_e1, j, len), L4 = run_from(s_e4, j, len);
                 const uint32_t L = L1 >= L4 ? L1 : L4;
                 const uint32_t d = L1 >= L4 ? 1 : 4;
@@ -614,7 +622,7 @@ int gsx_parquet_dict_insert(const uint32_t* cols_dev, int64_t n, int32_t ncols, 
     GSX_REQUIRE(n > 0 && n <= (1ll << 31) && ncols >= 1 && ncols <= kMaxCols, GSX_ERR_ARG,
                 "parquet_dict_insert: n=%lld, %d columns", (long long)n, ncols);
     const int64_t ngroups = (n + kRowGroup - 1) / kRowGroup;
-    GSX_REQUIRE(g0 >= 0 && ng >= 1 && g0 + ng <= ngroups && slots_log2 >= 19 && slots_log2 <= 24, GSX_ERR_ARG,
+    GSX_REQUIRE(g0 >= 0 && ng >= 1 && g0 + ng <= ngroups && slots_log2 >= kSlotsMin && slots_log2 <= 24, GSX_ERR_ARG,
                 "parquet_dict_insert: row groups %d + %d of %lld, 2^%d slots", g0, ng, (long long)ngroups, slots_log2);
     const int64_t rows = (g0 + ng) * kRowGroup < n ? (int64_t)ng * kRowGroup : n - g0 * kRowGroup;
     k_pq_insert<<<dim3((unsigned)((rows + kThreads - 1) / kThreads), ncols), kThreads, 0, st>>>(
@@ -632,8 +640,8 @@ int gsx_parquet_dictionary(unsigned long long* table_dev, int32_t slots_log2, co
                            int64_t nkeys, void* ws_dev, int64_t ws_bytes, uint32_t* dict_vals_dev, void* stream) {
     cudaStream_t st = (cudaStream_t)stream;
     GSX_NVTX("gsx_parquet_dictionary");
-    GSX_REQUIRE(njobs >= 0 && njobs <= 65535 && nkeys >= 0 && slots_log2 >= 19 && slots_log2 <= 24, GSX_ERR_ARG,
-                "parquet_dictionary: %d jobs, %lld keys", njobs, (long long)nkeys);
+    GSX_REQUIRE(njobs >= 0 && njobs <= 65535 && nkeys >= 0 && slots_log2 >= kSlotsMin && slots_log2 <= 24, GSX_ERR_ARG,
+                "parquet_dictionary: %d jobs, %lld keys, 2^%d slots", njobs, (long long)nkeys, slots_log2);
     if (njobs == 0 || nkeys == 0) return GSX_OK;
     GSX_REQUIRE(ws_bytes >= gsx_parquet_dictionary_workspace_bytes(nkeys), GSX_ERR_WORKSPACE,
                 "parquet_dictionary: workspace too small");
@@ -665,8 +673,8 @@ int gsx_parquet_dict_index(uint32_t* cols_dev, int64_t n, int32_t ncols, int32_t
     GSX_REQUIRE(n > 0 && n <= (1ll << 31) && ncols >= 1 && ncols <= kMaxCols, GSX_ERR_ARG,
                 "parquet_dict_index: n=%lld, %d columns", (long long)n, ncols);
     const int64_t ngroups = (n + kRowGroup - 1) / kRowGroup;
-    GSX_REQUIRE(g0 >= 0 && ng >= 1 && g0 + ng <= ngroups && slots_log2 >= 19 && slots_log2 <= 24, GSX_ERR_ARG,
-                "parquet_dict_index: row groups %d + %d of %lld", g0, ng, (long long)ngroups);
+    GSX_REQUIRE(g0 >= 0 && ng >= 1 && g0 + ng <= ngroups && slots_log2 >= kSlotsMin && slots_log2 <= 24, GSX_ERR_ARG,
+                "parquet_dict_index: row groups %d + %d of %lld, 2^%d slots", g0, ng, (long long)ngroups, slots_log2);
     const int64_t rows = (g0 + ng) * kRowGroup < n ? (int64_t)ng * kRowGroup : n - g0 * kRowGroup;
     k_pq_index<<<dim3((unsigned)((rows + kThreads - 1) / kThreads), ncols), kThreads, 0, st>>>(
         cols_dev, n, g0, ng, table_dev, slots_log2, dict_chunk_dev, page_idx_dev, (n + kPage - 1) / kPage);

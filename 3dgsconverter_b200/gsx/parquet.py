@@ -30,6 +30,8 @@ PAGE = 1 << 18               # rows per data page: 1 MiB of float32
 DICT_MAX = 1 << 18           # distinct values a dictionary may hold: 1 MiB (pyarrow's dictionary page limit)
 PIECE = 1 << 16              # Snappy piece, bytes: each is encoded on its own
 MAX_ROWS = 1 << 31
+MAX_COLS = 1024              # columns and row bytes gsx_parquet_split takes
+ROW_MAX = 1024
 CREATED_BY = "gsx (3dgsconverter H100 backend)"
 
 F4, U1 = 0, 1                # column kinds, as gsx_parquet_split numbers them
@@ -385,17 +387,22 @@ TABLE_BYTES = 1 << 30        # dictionary tables of one batch of row groups
 
 def encode(src, device="cuda") -> Encoded:
     """ParquetFormat.write's file (parquet.py:59-112), built on the device from `src`: DeviceRecords, readers.Decoded
-    or a 1-D structured NumPy array (uploaded once), the inputs gsx.ply.encode takes.  ValueError for what
-    column_plan refuses and for more than 2^31 rows."""
+    or a 1-D structured NumPy array (uploaded once), the inputs gsx.ply.encode takes.  ValueError, before anything is
+    uploaded, for what column_plan refuses, for more than 2^31 rows, rows wider than 1024 bytes and more than 1024
+    columns."""
     import torch
     from ._abi import lib, check, _ptr, _stream
     from .hostcopy import to_device, to_host
     from .ply import _device_rows
-    rows, dt, _ = _device_rows(src, device)
+    n, dt = _source_shape(src)
     plan = column_plan(dt)
-    n = int(rows.shape[0])
     if n > MAX_ROWS:
         raise ValueError(f"parquet: {n} rows; at most 2^31 are written on the device")
+    if len(plan) > MAX_COLS:
+        raise ValueError(f"parquet: {len(plan)} columns; at most {MAX_COLS} are written on the device")
+    if dt.itemsize > ROW_MAX:
+        raise ValueError(f"parquet: rows of {dt.itemsize} bytes; at most {ROW_MAX} are written on the device")
+    rows, dt, _ = _device_rows(src, device)
     dev = rows.device
     nc, (G, P) = len(plan), shape(n)
     T = -(-n // 2048)
@@ -494,6 +501,17 @@ def encode(src, device="cuda") -> Encoded:
         check(lib.gsx_parquet_assemble(_ptr(scratch), _ptr(pcs_dev), len(pcs), _ptr(sizes), *[_ptr(t) for t in up],
                                        len(hjobs), _ptr(out), st), "gsx_parquet_assemble")
     return Encoded(out, n)
+
+
+def _source_shape(src):
+    """(rows, dtype) of an input encode takes, without touching its data."""
+    from .readers import Decoded
+    from .records import DeviceRecords
+    if isinstance(src, DeviceRecords):
+        return len(src), np.dtype([(f, "<f4") for f in src.names])
+    if isinstance(src, Decoded) or (isinstance(src, np.ndarray) and src.dtype.names and src.ndim == 1):
+        return len(src), src.dtype
+    raise ValueError("encode takes DeviceRecords, readers.Decoded or a 1-D structured NumPy array")
 
 
 def chunk_nulls(nulls: np.ndarray, G: int) -> np.ndarray:

@@ -395,9 +395,12 @@ int gsx_deflate_emit(const uint8_t* data_dev, int64_t n, const int64_t* starts_d
  * non-null values (float32: sign bit flipped for positives, all bits for negatives; uint8: the value), 0xFFFFFFFF and
  * 0 for a chunk without one.
  * gsx_parquet_dict_insert (pyarrow's dictionary encoding): the non-null patterns of row groups [g0, g0 + ng) into
- * table_dev (uint64 [ng][ncols][2^slots_log2], zeroed by the caller, slots_log2 19 .. 24); distinct_dev uint32
+ * table_dev (uint64 [ng][ncols][2^slots_log2], zeroed by the caller, slots_log2 20 .. 24); distinct_dev uint32
  * [ncols][groups] (zeroed) counts the distinct patterns of each chunk, exactly up to 262 144, and ends above it
- * otherwise.
+ * otherwise.  2^20 slots is the least safe table: a chunk stops inserting only once a thread sees its count above
+ * 262 144, so every thread already past that check (up to one resident grid, 132 x 2048 on an H100) may still insert;
+ * 262 144 + 270 336 > 2^19, and a full table could wrap the count back below the limit.  gsx_parquet_dictionary and
+ * gsx_parquet_dict_index take the same slots_log2 (20 .. 24).
  * gsx_parquet_dictionary: for jobs_dev int64 [njobs][3] = (table index c + ncols * (g - g0), first key, first
  * dictionary value), njobs <= 65535, whose first keys leave room for each chunk's distinct count (nkeys in all):
  * the chunk's patterns ascending to dict_vals_dev, and each one's rank into the table.  Workspace from
@@ -414,7 +417,7 @@ int gsx_deflate_emit(const uint8_t* data_dev, int64_t n, const int64_t* starts_d
  * gsx_parquet_snappy: pieces_dev int64 [npieces][3] = (page, body offset (16-byte aligned), bytes 1 .. 65536).  Piece
  * i's Snappy elements go to scratch_dev + i * gsx_parquet_piece_bytes(), their length to sizes_dev[i], and it is added
  * to page_csize_dev[page] (zeroed by the caller).  Copies of distance 1 or 4 and length >= 8 inside the piece, taken
- * greedily from the left (the longer one, distance 1 on a tie); literals elsewhere.
+ * greedily from the left (the longer one; the two never tie at a chosen start); literals elsewhere.
  * gsx_parquet_assemble: the file: the pieces of each page back to back from page_dst_dev[page] (page_first_dev: its
  * first piece), and hjobs_dev int64 [nh][3] = (offset in heads_dev, file offset, bytes) of the headers and footer. */
 int gsx_parquet_split(const uint8_t* rows_dev, int64_t n, int32_t row_bytes, const int32_t* cols_host, int32_t ncols,

@@ -4,12 +4,23 @@ device writes them.  The page headers and the footer come from gsx.parquet's hos
 of the same file), which the device path uses as well.
 
     blob = encode(a)            # a: 1-D structured array -> the file's bytes
+
+Each kernel has its restatement here: split_kernel (k_pq_split: the columns, per-tile nulls and min / max keys),
+distinct_counts (k_pq_insert), dictionary (k_pq_collect + k_pq_rank), page_ranks (k_pq_index), data_page and the
+dictionary page bytes (k_pq_data_pages, k_pq_dict_pages), snappy_piece (k_pq_snappy) and write_file (k_pq_assemble
+with the host's headers).  COUNTERS counts the forms they reach, so tests can show that a case hits its path.
 """
 from __future__ import annotations
 
 import numpy as np
 
 from gsx import parquet as gp
+
+COUNTERS: dict = {}      # what the calls since the last clear reached
+
+
+def _count(key, n: int = 1) -> None:
+    COUNTERS[key] = COUNTERS.get(key, 0) + n
 
 
 # ------------------------------------------------------------------------------------------- split and statistics
@@ -36,6 +47,82 @@ def key(v: np.ndarray, kind: int) -> np.ndarray:
     return np.where(v >> 31 == 0, v ^ 0x80000000, ~v & 0xFFFFFFFF).astype(np.int64)
 
 
+TILE = 2048                  # rows per k_pq_split / k_pq_data_pages CTA
+STAGE = 64                   # rows k_pq_split stages in shared memory at a time
+
+
+def split_smem(ncols: int, row_bytes: int) -> int:
+    """k_pq_split's dynamic shared memory (gsx_parquet_split); above 48 KiB the entry point raises the limit."""
+    return ncols * 12 + 4 + ncols * 8 + 16 + STAGE * row_bytes + 16
+
+
+def split_kernel(raw: np.ndarray, spec) -> tuple:
+    """gsx_parquet_split on raw uint8 [n, row_bytes] rows and spec [(offset, kind)]: out uint32 [C, n], tile_nulls
+    uint32 [C, tiles], keys uint32 [2, C, groups] (least / greatest key of the chunk's non-null values; 0xFFFFFFFF and 0
+    for a chunk without one)."""
+    n = raw.shape[0]
+    G = max(1, -(-n // gp.ROW_GROUP))
+    T = -(-n // TILE)
+    out = np.empty((len(spec), n), np.uint32)
+    tnull = np.zeros((len(spec), T), np.uint32)
+    keys = np.empty((2, len(spec), G), np.uint32)
+    keys[0], keys[1] = 0xFFFFFFFF, 0
+    if split_smem(len(spec), raw.shape[1] if raw.ndim == 2 else 1) > 48 * 1024:
+        _count("split_smem_over_48k")
+    for c, (off, kind) in enumerate(spec):
+        out[c] = raw[:, off] if kind == gp.U1 else raw[:, off:off + 4].copy().view("<u4").reshape(-1)
+        null = is_null(out[c], kind)
+        tnull[c] = np.add.reduceat(null, np.arange(0, n, TILE)) if n else tnull[c]
+        for g in range(G):
+            s = slice(g * gp.ROW_GROUP, (g + 1) * gp.ROW_GROUP)
+            v = out[c, s][~null[s]]
+            if len(v):
+                k = key(v, kind)
+                keys[0, c, g], keys[1, c, g] = k.min(), k.max()
+            elif n:
+                _count("split_chunk_without_value")
+    return out, tnull, keys
+
+
+def distinct_counts(cols: np.ndarray, kinds) -> np.ndarray:
+    """k_pq_insert: int64 [C, G] distinct non-null patterns of each chunk (the kernel's count is exact up to DICT_MAX
+    and only known to be above it otherwise)."""
+    n = cols.shape[1]
+    G = max(1, -(-n // gp.ROW_GROUP))
+    out = np.zeros((len(cols), G), np.int64)
+    for c in range(len(cols)):
+        for g in range(G):
+            v = cols[c, g * gp.ROW_GROUP:(g + 1) * gp.ROW_GROUP]
+            out[c, g] = len(np.unique(v[~is_null(v, kinds[c])]))
+    return out
+
+
+def dictionary(v: np.ndarray, kind: int) -> tuple:
+    """k_pq_collect + radix sort + k_pq_rank + k_pq_index for one chunk's patterns v: (the dictionary, ascending
+    patterns; v with every non-null value replaced by its rank)."""
+    null = is_null(v, kind)
+    d = np.unique(v[~null])
+    _count(("dictionary_width", gp.bit_width(len(d))))
+    return d, np.where(null, v, np.searchsorted(d, v)).astype(np.uint32)
+
+
+def page_ranks(ranks: np.ndarray, null: np.ndarray) -> np.ndarray:
+    """k_pq_index's page_idx for one column: uint32 [2, pages] = least and greatest rank of each page, 0xFFFFFFFF and 0
+    (what the caller filled) for a page without a value."""
+    P = -(-len(ranks) // gp.PAGE)
+    out = np.empty((2, P), np.uint32)
+    out[0], out[1] = 0xFFFFFFFF, 0
+    for p in range(P):
+        s = slice(p * gp.PAGE, (p + 1) * gp.PAGE)
+        r = ranks[s][~null[s]]
+        if len(r):
+            out[:, p] = r.min(), r.max()
+            _count("index_page_equal" if r.min() == r.max() else "index_page_mixed")
+        else:
+            _count("index_page_empty")
+    return out
+
+
 # ----------------------------------------------------------------------------------------------------- hybrid runs
 def _bitpack(v: np.ndarray, w: int) -> bytes:
     """v as one bit-packed run's payload: ceil(len / 8) groups of 8 values, w bits each, LSB first."""
@@ -54,15 +141,23 @@ def data_page(v: np.ndarray, null: np.ndarray, w: int, idx) -> bytes:
     else:
         defs = gp.Thrift.varint(2 * rows) + b"\x01"
     out = len(defs).to_bytes(4, "little") + defs
+    hn = bool(null.any())
     if w == 0:
+        _count(("page", "plain", 0, hn))
         return out + v[~null].astype("<u4").tobytes()
     out += bytes([w])
     i = idx[~null]
     if nn == 0:
+        _count(("page", "empty", w, hn))
         return out
     if (i == i[0]).all():
+        _count(("page", "rle", w, hn))
+        _count(("rle_value_bytes", (w + 7) // 8))
         return out + gp.Thrift.varint(2 * nn) + int(i[0]).to_bytes((w + 7) // 8, "little")
-    return out + gp.Thrift.varint(2 * ((nn + 7) // 8) + 1) + _bitpack(i, w)
+    head = gp.Thrift.varint(2 * ((nn + 7) // 8) + 1)
+    _count(("page", "packed", w, hn))
+    _count(("packed_start_mod4", (len(out) + len(head)) % 4))
+    return out + head + _bitpack(i, w)
 
 
 # ---------------------------------------------------------------------------------------------------------- snappy
@@ -76,15 +171,18 @@ def _run_lengths(eq: np.ndarray) -> np.ndarray:
 
 def _literal(b) -> bytes:
     m = len(b) - 1
+    _count(("literal", len(b)))
     tag = bytes([m << 2]) if m < 60 else bytes([60 << 2, m]) if m < 256 else bytes([61 << 2, m & 255, m >> 8])
     return tag + bytes(b)
 
 
 def _copy(d: int, L: int) -> bytes:
     out = bytearray()
+    _count(("copy", d, L))
     while L > 64:
         out += bytes([(63 << 2) | 2, d, 0])
         L -= 64
+    _count(("copy_last", L))
     if 4 <= L <= 11:
         out += bytes([((L - 4) << 2) | 1, d])
     else:
@@ -94,7 +192,9 @@ def _copy(d: int, L: int) -> bytes:
 
 def snappy_piece(b: np.ndarray) -> bytes:
     """One piece's elements: greedy from the left, a copy where the bytes from i on repeat those 1 or 4 bytes back
-    for >= 8 bytes inside the piece (the longer of the two, distance 1 on a tie), literals elsewhere."""
+    for >= 8 bytes inside the piece (the longer of the two), literals elsewhere.  The two never tie at a chosen start j:
+    the bytes j - 1 and j - 2 differ there (else j - 1 was the candidate, or the copy before went on), so where a
+    distance-1 copy starts the distance-4 run is at most 2 bytes long (COUNTERS["snappy_tie"] would count one)."""
     n = len(b)
     e1 = np.zeros(n, bool)
     e4 = np.zeros(n, bool)
@@ -102,19 +202,30 @@ def snappy_piece(b: np.ndarray) -> bytes:
     e4[4:] = b[4:] == b[:-4]
     L1, L4 = _run_lengths(e1), _run_lengths(e4)
     cand = np.flatnonzero((L1 >= 8) | (L4 >= 8))
-    out, i, lit, k = bytearray(), 0, 0, 0
+    out, i, lit, k, jobs = bytearray(), 0, 0, 0, 0
+    _count(("piece_len", n))
     while True:
         k = int(np.searchsorted(cand, i, "left"))
         if k >= len(cand):
             break
         j = int(cand[k])
+        if (j >> 5) - (i >> 5) >= 32:
+            _count("snappy_scan_second_step")        # warp 0's 32-word scan does not reach j in its first step
+        if L1[j] == L4[j]:
+            _count("snappy_tie")
         L, d = (int(L1[j]), 1) if L1[j] >= L4[j] else (int(L4[j]), 4)
         if j > lit:
             out += _literal(b[lit:j])
+            jobs += 1
         out += _copy(d, L)
+        if (j + L) % 32 == 0:
+            _count(("copy_end_word", j + L == n))
         i = lit = j + L
     if n > lit:
         out += _literal(b[lit:])
+        jobs += 1
+    if jobs > 1024:
+        _count("snappy_walk_rounds")                 # more literal jobs than one walk round records
     return bytes(out)
 
 
@@ -157,10 +268,14 @@ def encode(a: np.ndarray) -> bytes:
     n = len(a)
     if n > gp.MAX_ROWS:
         raise ValueError("parquet: more than 2^31 rows")
-    G, P = gp.shape(n)
     cols, nulls, distinct, keys, dicts = kernel_outputs(a, plan)
-    rows = gp.page_rows(n)
-    width = gp.choose_dictionary(distinct, rows[None, :] - nulls)
+    width = gp.choose_dictionary(distinct, gp.page_rows(n)[None, :] - nulls)
+    return write_file(plan, n, cols, nulls, distinct, keys, dicts, width)
+
+
+def write_file(plan, n, cols, nulls, distinct, keys, dicts, width) -> bytes:
+    """The file of kernel_outputs' results with the dictionary bit widths `width` [C, G] (0: PLAIN)."""
+    G, P = gp.shape(n)
     idx, equal = {}, np.zeros((len(plan), P), bool)
     for c, col in enumerate(plan):
         for g in range(G):
